@@ -25,8 +25,11 @@
  * Batch layout (all arrays have n entries, device memory):
  *   unit i reads  in_base[in_off[i] .. in_off[i]+in_len[i])           (any byte alignment; 16-B aligned is fastest)
  *   unit i writes out_base[out_off[i] .. out_off[i]+out_cap[i])       (out_off[i] must be a multiple of 16)
- *   results: out_len[i] (bytes produced; on SWC_ERR_OUTPUT_OVERFLOW the size required), consumed[i], status[i].
- *   Output regions must not overlap.  Bytes between out_len[i] and out_cap[i] are scratch and may be clobbered.
+ *   results: out_len[i] (bytes produced), consumed[i], status[i].  On SWC_ERR_OUTPUT_OVERFLOW the Deflate and LZ4 batches
+ *   report the size required in out_len[i]; the BZip2 and LZMA decoders need their output as the window and stop at the
+ *   capacity, so theirs is only a lower bound of it.
+ *   Output regions must not overlap.  Bytes between out_len[i] and out_cap[i] are scratch and may be clobbered; nothing
+ *   outside the regions is written (this holds for the *_batch_host forms too: the caller's bytes between regions stay).
  */
 #ifndef SWCGPU_H
 #define SWCGPU_H

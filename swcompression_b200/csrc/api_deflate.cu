@@ -167,7 +167,6 @@ int32_t swc_deflate_decompress_batch_host(const uint8_t *in_base, const uint64_t
         cudaStream_t s = streams[k % 3];
         SWC_CUDA_TRY(cudaStreamWaitEvent(s, tables_ready, 0));
         const uint64_t i0 = S == 1 ? 0 : in_off[b], i1 = S == 1 ? in_total : in_off[e - 1] + in_len[e - 1];
-        const uint64_t o0 = S == 1 ? 0 : out_off[b], o1 = S == 1 ? out_total : out_off[e - 1] + out_cap[e - 1];
         SWC_CUDA_TRY(cudaMemcpyAsync((u8 *)p_in + i0, in_base + i0, i1 - i0, cudaMemcpyHostToDevice, s));
         inflate::BatchArgs a;
         a.in_base = (const u8 *)p_in; a.in_off = d_in_off + b; a.in_len = d_in_len + b; a.start_bits = nullptr;
@@ -177,7 +176,14 @@ int32_t swc_deflate_decompress_batch_host(const uint8_t *in_base, const uint64_t
         a.rec_count = (u32 *)((u8 *)p_scr + 256 * 64) + b;
         a.rec_base = (u32 *)((u8 *)p_scr + hdr);
         if ((st = inflate::launch(a, s))) return st;
-        SWC_CUDA_TRY(cudaMemcpyAsync(out_base + o0, (u8 *)p_out + o0, o1 - o0, cudaMemcpyDeviceToHost, s));
+        // only the output regions come back: the caller's bytes between and around them are not ours to overwrite
+        // (regions that touch are merged, so a densely packed slice is still one copy)
+        for (uint64_t i = b; i < e;) {
+            const uint64_t r0 = out_off[i];
+            uint64_t r1 = r0 + out_cap[i++];
+            while (i < e && out_off[i] == r1) r1 += out_cap[i++];
+            if (r1 > r0) SWC_CUDA_TRY(cudaMemcpyAsync(out_base + r0, (u8 *)p_out + r0, r1 - r0, cudaMemcpyDeviceToHost, s));
+        }
         SWC_CUDA_TRY(cudaMemcpyAsync(h_out_len + b, d_out_len + b, (e - b) * 8, cudaMemcpyDeviceToHost, s));
         SWC_CUDA_TRY(cudaMemcpyAsync(h_cons + b, d_cons + b, (e - b) * 8, cudaMemcpyDeviceToHost, s));
         SWC_CUDA_TRY(cudaMemcpyAsync(h_status + b, d_status + b, (e - b) * 4, cudaMemcpyDeviceToHost, s));

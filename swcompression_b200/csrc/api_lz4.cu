@@ -329,7 +329,12 @@ int32_t swc_lz4_block_decompress_batch_host(const uint8_t *in_base, const uint64
     st = swc_lz4_block_decompress_batch(d_in.as<u8>(), (u64 *)(m + 0 * tb), (u64 *)(m + 1 * tb), nullptr, 0, d_out.as<u8>(),
                                         (u64 *)(m + 2 * tb), (u64 *)(m + 3 * tb), (u64 *)(m + 4 * tb), (int32_t *)(m + 5 * tb), n, s);
     if (st) return st;
-    SWC_CUDA_TRY(cudaMemcpyAsync(out_base, d_out.p, out_total, cudaMemcpyDeviceToHost, s));
+    for (uint64_t i = 0; i < n;) {                         // only the output regions come back (touching ones as one copy)
+        const uint64_t r0 = out_off[i];
+        uint64_t r1 = r0 + out_cap[i++];
+        while (i < n && out_off[i] == r1) r1 += out_cap[i++];
+        if (r1 > r0) SWC_CUDA_TRY(cudaMemcpyAsync(out_base + r0, d_out.as<u8>() + r0, r1 - r0, cudaMemcpyDeviceToHost, s));
+    }
     SWC_CUDA_TRY(cudaMemcpyAsync(out_len, m + 4 * tb, tb, cudaMemcpyDeviceToHost, s));
     SWC_CUDA_TRY(cudaMemcpyAsync(status, m + 5 * tb, n * 4, cudaMemcpyDeviceToHost, s));
     SWC_CUDA_TRY(cudaStreamSynchronize(s));
