@@ -1,503 +1,24 @@
-// inflate.cu — batched Deflate decode for sm_90a.  Replaces Deflate.decompress(_: LsbBitReader)
+// inflate.cu — batched Deflate decode for sm_90a: the LZ77 stage and the launcher.  Replaces Deflate.decompress(_: LsbBitReader)
 // (reference Sources/Deflate/Deflate.swift:30-249) + Code.huffmanCodes / DecodingTree (Sources/Common/CodingTree).
 //
-// Two kernels per batch (DESIGN.md §4):
-//   K1 inflate_huffman_kernel  — ONE THREAD PER UNIT. Walks the Huffman bitstream; literals (and stored-block bytes)
-//        are written straight to their final output position through a per-lane 8-byte accumulator, every match
-//        becomes a 4-byte record {literal-run, length, distance} in a per-unit record stream.  Per-lane canonical
-//        decode tables live in shared memory, word-interleaved across the 32 lanes so that lane l only ever touches
-//        bank l (conflict-free for any index pattern).  The compressed stream is fetched with 16-byte streaming loads,
-//        double-buffered in registers one chunk ahead of the bit buffer.
-//   K2 lz_resolve_kernel       — ONE WARP PER UNIT. Replays the records 8 at a time on 4-lane sub-groups (period-replicating
-//        when distance < length).  Positions come from a warp inclusive scan of the records.
+// Two kernels per batch (DESIGN.md §4.1):
+//   K1 the Huffman stage — K1L inflate_lut_kernel (inflate_lut.cu, one thread per unit) for large batches, K1w
+//        inflate_warp_kernel (inflate_warp.cu, one warp per unit) for small ones.  Literals go straight to their final
+//        output position, every match becomes a record (format in inflate.cuh).
+//   K2 lz_resolve_kernel (here) — ONE WARP PER UNIT.  Replays the records 8 at a time on 4-lane sub-groups
+//        (period-replicating when distance < length).  Positions come from a warp inclusive scan of the records.
 //
 // Semantics are those of the reference, including its error cases and the inputs on which it traps
 // (SWC_ERR_REFERENCE_TRAP).  Code sets whose Kraft sum exceeds 1 (which the reference accepts through heap-slot
 // overwrites) are routed to the generic serial decoder in inflate_slow.cu via SWC_INTERNAL_NEEDS_SLOW.
 #include <cstdlib>
+#include <cstring>
 #include "common.cuh"
 #include "inflate.cuh"
 #include "host_util.h"
 
 namespace swc {
 namespace inflate {
-
-// ---- per-lane shared-memory layout (32-bit words; word w of lane l lives at warp_base[w * 32 + l]) ----
-constexpr int W_LIT_SYM = 0;     // 288 x u8  : low byte of the lit/len symbols sorted by (code length, symbol)
-constexpr int W_LIT_TH = 72;     // [1..15]   : sorted index of the first symbol >= 256 among the codes of length L
-constexpr int W_DST_SYM = 88;    // 32 x u8   : distance symbols sorted likewise
-constexpr int W_LIT_BO = 96;     // [1..15]   : first left-justified 15-bit code of length L | index of its first symbol << 16
-constexpr int W_DST_BO = 112;
-constexpr int W_CL_SYM = 128;    // 19 x u8   : code-length-alphabet symbols, sorted
-constexpr int W_CL_BO = 133;     // [1..7]
-constexpr int W_TOTAL = 141;     // 564 B per lane -> 12 resident warps per SM
-constexpr int WARPS_PER_CTA = 4;
-constexpr int CTAS_PER_SM = 3;
-#ifndef SWC_KLIT
-#define SWC_KLIT 4
-#endif
-constexpr int KLIT = SWC_KLIT;          // lit/len symbols a lane may decode per round before the warp services pending matches
-constexpr int SMEM_LUT_WORDS = 64;   // CTA-shared length/distance base+extra tables
-constexpr size_t SMEM_BYTES = (size_t)WARPS_PER_CTA * W_TOTAL * 32 * 4 + SMEM_LUT_WORDS * 4;
-
-// RFC 1951 3.2.5 tables as {base | extra_bits << 16}; Deflate+Constants.swift:179-186 + Deflate.swift:188-189,206
-__constant__ u32 c_len_tab[32] = {
-    3, 4, 5, 6, 7, 8, 9, 10, 11 | 1 << 16, 13 | 1 << 16, 15 | 1 << 16, 17 | 1 << 16, 19 | 2 << 16, 23 | 2 << 16, 27 | 2 << 16,
-    31 | 2 << 16, 35 | 3 << 16, 43 | 3 << 16, 51 | 3 << 16, 59 | 3 << 16, 67 | 4 << 16, 83 | 4 << 16, 99 | 4 << 16,
-    115 | 4 << 16, 131 | 5 << 16, 163 | 5 << 16, 195 | 5 << 16, 227 | 5 << 16, 258, 0, 0, 0};
-__constant__ u32 c_dist_tab[32] = {
-    1, 2, 3, 4, 5 | 1 << 16, 7 | 1 << 16, 9 | 2 << 16, 13 | 2 << 16, 17 | 3 << 16, 25 | 3 << 16, 33 | 4 << 16, 49 | 4 << 16,
-    65 | 5 << 16, 97 | 5 << 16, 129 | 6 << 16, 193 | 6 << 16, 257 | 7 << 16, 385 | 7 << 16, 513 | 8 << 16, 769 | 8 << 16,
-    1025 | 9 << 16, 1537 | 9 << 16, 2049 | 10 << 16, 3073 | 10 << 16, 4097 | 11 << 16, 6145 | 11 << 16, 8193 | 12 << 16,
-    12289 | 12 << 16, 16385 | 13 << 16, 24577 | 13 << 16, 0, 0};
-__constant__ u8 c_cl_order[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
-
-struct Limits {
-    u32 p[8];   // p[k] = limit[2k+1] | limit[2k+2] << 16 ; limit[L] = left-justified end of the length-L code range
-};
-
-// ------------------------------------------------------------------------------------------------ bit reader
-struct BitReader {
-    const u32 *p, *pend;   // next 32-bit word to prefetch / first word past the unit
-    u32 wnext;             // prefetched word (loaded one refill ahead, so its latency is off the decode chain)
-    u64 bb;                // bit buffer, LSB first
-    int bc;                // valid bits in bb
-    i64 avail;             // the reference's bitsLeft: real input bits not yet consumed
-
-    __device__ __forceinline__ u32 fetch() {
-        u32 v = 0;
-        if (p < pend) v = __ldg(p);
-        p++;
-        return v;
-    }
-    __device__ __forceinline__ void refill() {   // requires bc <= 32
-        bb |= (u64)wnext << bc;
-        bc += 32;
-        wnext = fetch();
-    }
-    __device__ __forceinline__ void need32() { if (bc <= 32) refill(); }
-    __device__ void init(const u8 *base, u64 off, u64 len, u32 bitskip) {
-        uintptr_t a = (uintptr_t)(base + off);
-        p = (const u32 *)(a & ~(uintptr_t)3);
-        pend = (const u32 *)((a + len + 3) & ~(uintptr_t)3);
-        wnext = fetch();
-        bb = 0; bc = 0;
-        refill();
-        u32 drop = (u32)(a & 3) * 8 + bitskip;    // < 32
-        bb >>= drop; bc -= drop;
-        need32();
-        avail = (i64)len * 8 - bitskip;
-    }
-    __device__ __forceinline__ u32 peek(int n) const { return (u32)bb & ((1u << n) - 1); }
-    __device__ __forceinline__ void skip(int n) { bb >>= n; bc -= n; avail -= n; }
-};
-
-// ------------------------------------------------------------------------------------------------ canonical decode
-__device__ __forceinline__ int code_length(u32 r15, const Limits &lim) {
-    // count the limits that r15 has reached; limits are non-decreasing so this is the code length - 1
-    const u32 X = (r15 | (r15 << 16)) + 0x80008000u;
-    u32 t[8];
-#pragma unroll
-    for (int k = 0; k < 8; k++) t[k] = X - lim.p[k];       // bit15 / bit31 = (r15 >= limit)
-    // gather the 16 flag bytes (byte1/byte3 of each t) into 4 words, fold, one popc
-    u32 a = __byte_perm(t[0], t[1], 0x7531), b = __byte_perm(t[2], t[3], 0x7531);
-    u32 c = __byte_perm(t[4], t[5], 0x7531), d = __byte_perm(t[6], t[7], 0x7531);
-    u32 v = (a & 0x80808080u) | ((b & 0x80808080u) >> 1) | ((c & 0x80808080u) >> 2) | ((d & 0x80808080u) >> 3);
-    return 1 + __popc(v);                                    // 16 => no code matches (incomplete set)
-}
-
-// finalize one alphabet: bo[L] holds count[L] on entry, {first_code_lj | first_index << 16} on exit.
-// Returns the Kraft sum scaled to 2^15 (exactly 0x8000 for a complete code).
-__device__ __forceinline__ u32 finalize_tables(u32 *bo /* lane word 0 of the BO area */, Limits &lim, int maxlen) {
-    u32 code = 0, off = 0;
-    u32 l[17];
-#pragma unroll
-    for (int L = 1; L <= 15; L++) {
-        u32 c = L <= maxlen ? bo[L * 32] : 0;
-        if (L <= maxlen) bo[L * 32] = (code & 0xFFFF) | (off << 16);
-        code += c << (15 - L);
-        off += c;
-        l[L] = code > 0x8000u ? 0x8000u : code;
-    }
-    l[16] = 0x8000u;
-#pragma unroll
-    for (int k = 0; k < 8; k++) lim.p[k] = l[2 * k + 1] | (l[2 * k + 2] << 16);
-    return code;
-}
-
-// after the scatter pass every first_index has advanced by count[L]; shift them back down one slot
-__device__ __forceinline__ void rewind_offsets(u32 *bo, int maxlen) {
-    u32 prev = 0;
-#pragma unroll
-    for (int L = 1; L <= 15; L++) {
-        if (L <= maxlen) {
-            u32 w = bo[L * 32];
-            bo[L * 32] = (w & 0xFFFFu) | (prev << 16);
-            prev = w >> 16;
-        }
-    }
-}
-
-// ------------------------------------------------------------------------------------------------ output side
-struct Emitter {
-    u8 *out;        // unit output base (16-byte aligned)
-    u32 *rec;       // unit record stream
-    u32 op;         // bytes produced so far
-    u32 cap;
-    u32 last_end;   // end of the previous match (start of the current literal run)
-    u32 nrec;
-    typedef u64 acc_t;                       // 8-byte words: a 4-byte accumulator doubles the store count (slower)
-    static constexpr u32 AM = 7, AS = 3;
-    acc_t acc;      // pending bytes of the aligned word that contains `op`
-    bool dirty;     // acc holds at least one literal
-
-    __device__ __forceinline__ void literal(u32 byte) {
-        acc |= (acc_t)byte << ((op & AM) * 8);
-        dirty = true;
-        op++;
-        if ((op & AM) == 0) {
-            if (op <= cap) *(acc_t *)(out + op - (AM + 1)) = acc;
-            acc = 0; dirty = false;
-        }
-    }
-    __device__ __forceinline__ void match(u32 len, u32 dist) {
-        u32 nop = op + len;
-        if (nop <= cap) {
-            u32 run = op - last_end;
-            if (run > 255) {                       // escape record: skip (run & ~255) literal bytes
-                u32 skip = run & ~255u;
-                rec[nrec++] = 0x8000u | (skip & 0x7FFFu) | ((skip >> 15) << 16);
-                run &= 255u;
-            }
-            rec[nrec++] = (dist - 1) | ((len - 3) << 16) | (run << 24);
-        }
-        last_end = nop;
-        if ((op >> AS) != (nop >> AS)) {           // leaving the current word: its remaining bytes belong to the match (K2 fills them)
-            if (dirty && (op | AM) < cap) *(acc_t *)(out + (op & ~AM)) = acc;
-            else if (dirty) flush_bytes();
-            acc = 0; dirty = false;
-        }
-        op = nop;
-    }
-    __device__ void flush_bytes() {                // byte-granular flush of the literal bytes of the current word
-        u32 base = op & ~AM;
-        for (u32 i = base; i < op; i++)
-            if (i < cap) out[i] = (u8)(acc >> ((i & AM) * 8));
-    }
-    __device__ __forceinline__ void finish() {
-        if (dirty) flush_bytes();
-    }
-};
-
-// ------------------------------------------------------------------------------------------------ code-length stream
-// Iterates the HLIT+HDIST code lengths of a dynamic block (Deflate.swift:119-161) or the fixed lengths of a static
-// block (Deflate+Constants.swift:11-173).  next() returns the next length or a negative status.
-struct LenStream {
-    bool dynamic;
-    int idx, count;
-    int rep, rep_val, prev;
-
-    __device__ __forceinline__ void start(bool dyn, int total) { dynamic = dyn; idx = 0; count = total; rep = 0; rep_val = 0; prev = -1; }
-};
-
-__device__ __forceinline__ int static_len(int i) {   // i < 288: lit/len, else distance (32 symbols of 5 bits)
-    return i < 144 ? 8 : i < 256 ? 9 : i < 280 ? 7 : i < 288 ? 8 : 5;
-}
-
-// KIND 0: lit/len alphabet (u8 table + high-bit vector), KIND 1: u8 table (distance / code-length alphabets)
-template <int KIND>
-__device__ __forceinline__ int decode_symbol(BitReader &br, const Limits &lim, const u32 *bo, const u32 *symw, int &len_out) {
-    u32 r15 = __brev(br.peek(15)) >> 17;
-    int L = code_length(r15, lim);
-    len_out = L;
-    if (L > 15) return -1;
-    u32 w = bo[L * 32];
-    u32 idx = (w >> 16) + ((r15 - (w & 0xFFFFu)) >> (15 - L));
-    u32 lo = ((const u8 *)(symw + (idx >> 2) * 32))[idx & 3];
-    if (KIND == 0) {
-        const u32 th = symw[(W_LIT_TH - W_LIT_SYM + L) * 32];
-        lo |= idx >= th ? 256u : 0u;
-    }
-    return (int)lo;
-}
-
-// One pass over the code lengths. PASS 0 counts lengths into the BO areas, PASS 1 scatters symbols into the sorted
-// tables. Returns SWC_OK or the reference's error for this header.
-template <int PASS>
-__device__ int run_lengths(BitReader &br, u32 *S, const Limits &cl_lim, bool dynamic, int hlit, int hdist) {
-    const int count = hlit + hdist;
-    int n = 0, prev = 0;
-    while (n < count) {
-        int len, reps = 1;
-        if (!dynamic) {
-            len = static_len(n < hlit ? n : 288 + (n - hlit));
-        } else {
-            br.need32();
-            int cl;
-            int sym = decode_symbol<1>(br, cl_lim, S + W_CL_BO * 32, S + W_CL_SYM * 32, cl);
-            if (sym < 0 || br.avail < cl) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-            br.skip(cl);
-            if (sym <= 15) {
-                len = sym;
-            } else if (sym == 16) {
-                if (n == 0) return SWC_DEFLATE_WRONG_SYMBOL;
-                if (br.avail < 2) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-                reps = (int)br.peek(2) + 3; br.skip(2);
-                if (n + reps > count) return SWC_DEFLATE_WRONG_SYMBOL;
-                len = prev;
-            } else if (sym == 17) {
-                if (br.avail < 3) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-                reps = (int)br.peek(3) + 3; br.skip(3);
-                len = 0;
-            } else {   // 18 (the alphabet has 19 symbols)
-                if (br.avail < 7) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-                reps = (int)br.peek(7) + 11; br.skip(7);
-                len = 0;
-            }
-        }
-        if (len == 0) {
-            n += reps;      // zeros: nothing to count or place (may overshoot `count`: checked below)
-        } else {
-            for (int r = 0; r < reps; r++, n++) {
-                const bool is_lit = n < hlit;
-                u32 *bo = S + (is_lit ? W_LIT_BO : W_DST_BO) * 32;
-                if (PASS == 0) {
-                    bo[len * 32] += 1;
-                    if (is_lit && n < 256) S[(W_LIT_TH + len) * 32] += 1;
-                } else {
-                    u32 w = bo[len * 32];
-                    bo[len * 32] = w + 0x10000u;
-                    u32 pos = w >> 16;
-                    if (is_lit) {
-                        ((u8 *)(S + (W_LIT_SYM + (pos >> 2)) * 32))[pos & 3] = (u8)n;
-                    } else {
-                        ((u8 *)(S + (W_DST_SYM + (pos >> 2)) * 32))[pos & 3] = (u8)(n - hlit);
-                    }
-                }
-            }
-        }
-        prev = len;
-    }
-    if (n != count) return SWC_DEFLATE_WRONG_SYMBOL;          // Deflate.swift:161
-    return SWC_OK;
-}
-
-// ------------------------------------------------------------------------------------------------ K1
-// Control flow is a per-lane state machine driven by ONE warp-wide loop: every round starts with a full-mask vote,
-// which forces the 32 lanes back into lock-step.  (A plain per-lane `for(;;)` with early exits lets independent thread
-// scheduling split the warp into sub-groups that never re-converge: far slower.)
-// A round = up to KLIT lit/len symbols per lane, then ONE pass of the (long) match path for every lane that has a
-// length symbol pending — so the match instructions are issued with many lanes active instead of ~15 % of them.
-enum { ST_HEADER = 0, ST_SYMBOLS = 1, ST_MATCH = 2, ST_DONE = 3 };
-
-struct BlockCtx {
-    Limits lit_lim, dst_lim;
-    bool is_last;
-};
-
-// Block header (Deflate.swift:41-168): stored blocks are copied here; for Huffman blocks the per-lane tables are built.
-// Returns SWC_OK or the reference's error; `next` receives the state to continue in.
-__device__ __forceinline__ int begin_block(BitReader &br, Emitter &em, u32 *S, BlockCtx &bc, int &next) {
-    br.need32();
-    if (br.avail < 3) return SWC_ERR_REFERENCE_TRAP;                                    // :41-43 unguarded reads
-    const u32 hdr = br.peek(3); br.skip(3);
-    bc.is_last = (hdr & 1) != 0;
-    const u32 btype = hdr >> 1;
-    if (btype == 3) return SWC_DEFLATE_WRONG_BLOCK_TYPE;                                 // :239
-    if (btype == 0) {                                                                   // :45-65
-        br.skip((int)(br.avail & 7));
-        br.need32();
-        if (br.avail < 32) return SWC_DEFLATE_WRONG_UNCOMPRESSED_BLOCK_LENGTHS;
-        const u32 length = br.peek(16); br.skip(16);
-        br.need32();
-        const u32 nlength = br.peek(16); br.skip(16);
-        if ((length & nlength) != 0) return SWC_DEFLATE_WRONG_UNCOMPRESSED_BLOCK_LENGTHS;
-        if ((br.avail >> 3) < (i64)length) return SWC_DEFLATE_WRONG_UNCOMPRESSED_BLOCK_LENGTHS;
-        for (u32 i = 0; i < length; i++) {
-            br.need32();
-            em.literal(br.peek(8));
-            br.skip(8);
-        }
-        next = bc.is_last ? ST_DONE : ST_HEADER;
-        return SWC_OK;
-    }
-    const bool dynamic = btype == 2;
-    int hlit = 288, hdist = 32;
-    Limits cl_lim;
-    BitReader saved;
-#pragma unroll
-    for (int L = 1; L <= 15; L++) { S[(W_LIT_BO + L) * 32] = 0; S[(W_DST_BO + L) * 32] = 0; }
-#pragma unroll
-    for (int L = 1; L <= 15; L++) S[(W_LIT_TH + L) * 32] = 0;
-    if (dynamic) {
-        br.need32();
-        if (br.avail < 14) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-        hlit = (int)br.peek(5) + 257; br.skip(5);
-        if (hlit > 286) return SWC_DEFLATE_WRONG_SYMBOL;                                 // :94
-        hdist = (int)br.peek(5) + 1; br.skip(5);
-        const int hclen = (int)br.peek(4) + 4; br.skip(4);
-        if (br.avail < 3 * hclen) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-        u64 cl = 0;                                 // 19 x 3-bit code lengths, indexed by symbol
-        for (int i = 0; i < hclen; i++) {
-            br.need32();
-            cl |= (u64)br.peek(3) << (3 * c_cl_order[i]);
-            br.skip(3);
-        }
-        u64 cnt = 0;                                // 8 x 8-bit counters
-        for (int s = 0; s < 19; s++) cnt += 1ull << (8 * ((cl >> (3 * s)) & 7));
-#pragma unroll
-        for (int L = 1; L <= 7; L++) S[(W_CL_BO + L) * 32] = (u32)(cnt >> (8 * L)) & 0xFF;
-        const u32 kraft = finalize_tables(S + W_CL_BO * 32, cl_lim, 7);
-        if (kraft > 0x8000u) return SWC_INTERNAL_NEEDS_SLOW;
-        for (int s = 0; s < 19; s++) {
-            const u32 l = (u32)(cl >> (3 * s)) & 7;
-            if (l) {
-                const u32 w = S[(W_CL_BO + l) * 32];
-                S[(W_CL_BO + l) * 32] = w + 0x10000u;
-                const u32 pos = w >> 16;
-                ((u8 *)(S + (W_CL_SYM + (pos >> 2)) * 32))[pos & 3] = (u8)s;
-            }
-        }
-        rewind_offsets(S + W_CL_BO * 32, 7);
-        saved = br;
-    }
-    int st = run_lengths<0>(br, S, cl_lim, dynamic, hlit, hdist);
-    if (st) return st;
-    const u32 k1 = finalize_tables(S + W_LIT_BO * 32, bc.lit_lim, 15);
-    const u32 k2 = finalize_tables(S + W_DST_BO * 32, bc.dst_lim, 15);
-    if (k1 > 0x8000u || k2 > 0x8000u) return SWC_INTERNAL_NEEDS_SLOW;
-#pragma unroll
-    for (int L = 1; L <= 15; L++) S[(W_LIT_TH + L) * 32] += S[(W_LIT_BO + L) * 32] >> 16;   // first index + #literals of length L
-    if (dynamic) br = saved;
-    run_lengths<1>(br, S, cl_lim, dynamic, hlit, hdist);
-    rewind_offsets(S + W_LIT_BO * 32, 15);
-    rewind_offsets(S + W_DST_BO * 32, 15);
-    next = ST_SYMBOLS;
-    return SWC_OK;
-}
-
-// One lit/len symbol (Deflate.swift:171-198). Literals are emitted; any other symbol (end-of-block or a length) is only
-// parked in `pend_sym` and the lane moves to ST_MATCH: the rare tail (EOB test, range test, length extra bits) then runs once
-// per round in match_step with every parked lane taking part, instead of in each of the KLIT steps with ~4 of 32 lanes
-// (ncu source view: that tail was 9.8 % of all issued instructions at 3.7 active threads).
-__device__ __forceinline__ int litlen_step(BitReader &br, Emitter &em, const u32 *S, const BlockCtx &bc,
-                                           int &state, u32 &pend_sym) {
-    br.need32();
-    int L;
-    const int sym = decode_symbol<0>(br, bc.lit_lim, S + W_LIT_BO * 32, S + W_LIT_SYM * 32, L);
-    if (sym < 0 || br.avail < L) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-    br.skip(L);
-    if (sym < 256) { em.literal((u32)sym); return SWC_OK; }
-    pend_sym = (u32)sym;
-    state = ST_MATCH;
-    return SWC_OK;
-}
-
-// Distance half of a match (Deflate.swift:199-232).
-__device__ __forceinline__ int dist_step(BitReader &br, Emitter &em, const u32 *S, const BlockCtx &bc, const u32 *lut,
-                                         int &state, u32 sym) {
-    if (sym == 256) { state = bc.is_last ? ST_DONE : ST_HEADER; return SWC_OK; }
-    if (sym > 285) return SWC_DEFLATE_WRONG_SYMBOL;
-    const u32 le = lut[sym - 257];
-    const int eb = (int)(le >> 16);                                // <= 5 bits: still inside the 33 bits need32() gave the symbol
-    if (br.avail < eb) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-    const u32 length = (le & 0xFFFFu) + br.peek(eb);
-    br.skip(eb);
-    br.need32();
-    int DL;
-    const int dsym = decode_symbol<1>(br, bc.dst_lim, S + W_DST_BO * 32, S + W_DST_SYM * 32, DL);
-    if (dsym < 0 || br.avail < DL) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-    br.skip(DL);
-    if (dsym > 29) return SWC_DEFLATE_WRONG_SYMBOL;
-    const u32 de = lut[32 + dsym];
-    const int db = (int)(de >> 16);
-    if (br.avail < db) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-    const u32 dist = (de & 0xFFFFu) + br.peek(db);
-    br.skip(db);
-    if (dist > em.op) return SWC_ERR_REFERENCE_TRAP;                                     // :219 negative array index
-    if ((u64)em.op + length > 0xFFFFFFF0ull) return SWC_ERR_UNSUPPORTED;
-    em.match(length, dist);
-    return SWC_OK;
-}
-
-__global__ void __launch_bounds__(WARPS_PER_CTA * 32, CTAS_PER_SM)
-inflate_huffman_kernel(BatchArgs a) {
-    extern __shared__ u32 smem[];
-    u32 *lut = smem;                                   // [0,32) length table, [32,64) distance table
-    if (threadIdx.x < 32) { lut[threadIdx.x] = c_len_tab[threadIdx.x]; lut[32 + threadIdx.x] = c_dist_tab[threadIdx.x]; }
-    __syncthreads();
-    const u32 lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    u32 *S = smem + SMEM_LUT_WORDS + warp * (W_TOTAL * 32) + lane;     // this lane's word 0
-
-    // Persistent lanes: every lane pulls its next unit from a global ticket counter the moment it finishes one, so a
-    // warp never idles on its slowest stream and the grid is exactly the resident capacity (no partial last wave).
-    int status = SWC_OK, state = ST_DONE;
-    bool have_unit = false, exhausted = false;
-    u64 unit = 0;
-    BitReader br;
-    Emitter em;
-    BlockCtx bc;
-    i64 total_bits = 0;
-    u64 cap64 = 0;
-    u32 pend_len = 0;
-    br.avail = 0;
-    em.op = 0; em.nrec = 0; em.dirty = false; em.acc = 0; em.last_end = 0; em.cap = 0;
-    for (;;) {
-        if (state == ST_DONE) {
-            if (have_unit) {                                                             // retire the finished unit
-                em.finish();
-                if (status == SWC_OK && (u64)em.op > cap64) status = SWC_ERR_OUTPUT_OVERFLOW;
-                a.consumed_bits[unit] = (u64)(total_bits - br.avail);
-                a.out_len[unit] = em.op;
-                a.status[unit] = status;
-                a.rec_count[unit] = em.nrec;
-                have_unit = false;
-            }
-            if (!exhausted) {
-                unit = atomicAdd(a.ticket, 1ull);
-                if (unit >= a.n) {
-                    exhausted = true;
-                } else {
-                    have_unit = true;
-                    status = SWC_OK;
-                    const u64 in_len = a.in_len[unit];
-                    cap64 = a.out_cap[unit];
-                    em.out = a.out_base + a.out_off[unit];
-                    em.rec = a.rec_base + rec_start(a.out_off[unit]);
-                    em.cap = cap64 > 0xFFFFFFF0ull ? 0xFFFFFFF0u : (u32)cap64;
-                    em.op = 0; em.nrec = 0; em.dirty = false; em.acc = 0; em.last_end = 0;
-                    total_bits = 0; br.avail = 0;
-                    if (in_len >= (1ull << 32)) {
-                        status = SWC_ERR_UNSUPPORTED;
-                    } else {
-                        br.init(a.in_base, a.in_off[unit], in_len, a.start_bits ? a.start_bits[unit] : 0);
-                        total_bits = br.avail;
-                        if (br.avail < 10) status = SWC_DEFLATE_WRONG_BLOCK_TYPE;        // Deflate.swift:36
-                        else state = ST_HEADER;
-                    }
-                }
-            }
-        }
-        if (!__any_sync(SWC_FULL, state != ST_DONE || have_unit || !exhausted)) break;
-#pragma unroll 1
-        for (int k = 0; k < KLIT; k++) {
-            if (state == ST_SYMBOLS) {
-                const int r = litlen_step(br, em, S, bc, state, pend_len);
-                if (r) { status = r; state = ST_DONE; }
-            }
-        }
-        if (state == ST_MATCH) {
-            const int r = dist_step(br, em, S, bc, lut, state, pend_len);
-            if (r) { status = r; state = ST_DONE; }
-            else if (state == ST_MATCH) state = ST_SYMBOLS;
-        } else if (state == ST_HEADER) {
-            int next = ST_DONE;
-            const int r = begin_block(br, em, S, bc, next);
-            if (r) { status = r; state = ST_DONE; }
-            else state = next;
-        }
-    }
-}
 
 // ------------------------------------------------------------------------------------------------ K2
 // One warp per unit: replay the match records in order.  Lane j holds record j of a 32-record group; an inclusive warp
@@ -521,18 +42,15 @@ lz_resolve_kernel(BatchArgs a) {
     u8 *out = a.out_base + a.out_off[unit];
     u32 base = 0;
     for (u32 g = 0; g < nrec; g += 32) {
-        const u32 r = (g + lane < nrec) ? rec[g + lane] : 0x8000u;     // padding = escape with skip 0
-        const bool esc = (r & 0x8000u) != 0;
-        const u32 len = esc ? 0 : ((r >> 16) & 0xFF) + 3;
-        const u32 adv = esc ? ((r & 0x7FFFu) | ((r >> 16) << 15)) : (r >> 24) + len;
-        u32 end = adv;
+        const Match m = get_match((g + lane < nrec) ? rec[g + lane] : REC_ESC);
+        u32 end = m.adv;
 #pragma unroll
         for (int d = 1; d < 32; d <<= 1) {
             const u32 v = __shfl_up_sync(SWC_FULL, end, d);
             if (lane >= (u32)d) end += v;
         }
         // a sub-group fetches its record with one 16-byte shared-memory load instead of three shuffles
-        st[lane] = make_uint4(base + end - len, len, (r & 0x7FFFu) + 1, 0u);
+        st[lane] = make_uint4(base + end - m.len, m.len, m.dist, 0u);
         base += __shfl_sync(SWC_FULL, end, 31);
         __syncwarp();
 #pragma unroll 1
@@ -580,34 +98,20 @@ lz_resolve_kernel(BatchArgs a) {
 // ------------------------------------------------------------------------------------------------ host
 int launch(const BatchArgs &a, cudaStream_t stream) {
     if (a.n == 0) return SWC_OK;
-    // Path selection.
-    //   large batches : K1L (inflate_lut.cu) — one lane per stream, table-lookup decode — then K2.
+    // Huffman stage.
+    //   large batches : K1L (inflate_lut.cu) — one lane per stream, table-lookup decode.
     //   small batches (and the single-stream API calls) cannot fill the chip with one lane per stream, so they take the
-    //                   warp-per-unit decoder K1w (32 lanes on every stream, ~10 x lower latency per stream) + K2.
-    //   SWC_DEFLATE_K1 = lut | warp | thread forces K1L / K1w / the round-1 limit-compare K1 (kept for A/B runs).
-    static const int forced = [] { const char *e = getenv("SWC_DEFLATE_K1"); return !e ? -1 : (e[0] == 'w' ? 1 : (e[0] == 't' ? 2 : 0)); }();
-    const int path = forced >= 0 ? forced : (a.n < 20000 ? 1 : 0);
+    //                   warp-per-unit decoder K1w (32 lanes on every stream, ~10 x lower latency per stream).
+    //   SWC_DEFLATE_K1 = lut | warp forces K1L / K1w; any other value keeps the choice by batch size.
+    static const int forced = [] {
+        const char *e = getenv("SWC_DEFLATE_K1");
+        return !e ? -1 : !strcmp(e, "lut") ? 0 : !strcmp(e, "warp") ? 1 : -1;
+    }();
+    const bool use_lut = forced >= 0 ? forced == 0 : a.n >= 20000;
     SWC_CUDA_TRY(cudaMemsetAsync(a.ticket, 0, 16, stream));
     timing_mark(stream);
-    if (path == 0) {
-        int st = launch_lut(a, stream);
-        if (st) return st;
-    } else if (path == 1) {
-        int st = launch_warp(a, stream);
-        if (st) return st;
-    } else {
-        int st = configure_once(CFG_INFLATE_K1, [](DeviceCtx &) {
-            SWC_CUDA_TRY(cudaFuncSetAttribute(inflate_huffman_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-            return (int)SWC_OK;
-        });
-        if (st) return st;
-        const u64 per_cta = WARPS_PER_CTA * 32;
-        u64 g1 = (a.n + per_cta - 1) / per_cta;
-        const u64 resident = (u64)device_ctx().num_sms * CTAS_PER_SM;       // persistent lanes: one CTA per resident slot
-        if (g1 > resident) g1 = resident;
-        inflate_huffman_kernel<<<(unsigned)g1, WARPS_PER_CTA * 32, SMEM_BYTES, stream>>>(a);
-        count_launch();
-    }
+    const int st = use_lut ? launch_lut(a, stream) : launch_warp(a, stream);
+    if (st) return st;
     timing_mark(stream);
     launch_slow(a, stream);          // no-op unless a Huffman stage flagged a unit (over-subscribed code set)
     timing_mark(stream);

@@ -1,8 +1,7 @@
 // inflate_lut.cu — K1L: Deflate Huffman stage for large batches, table-lookup decode (one thread per unit).
 // Replaces the walk of Deflate.decompress(_: LsbBitReader) (reference Sources/Deflate/Deflate.swift:30-249) and
 // DecodingTree.findNextSymbol (Sources/Common/CodingTree/DecodingTree.swift:36-50) for the batched hot path.
-// Same contract as inflate_huffman_kernel (inflate.cu): literals land at their final output position, every match
-// becomes a 4-byte record {dist-1:15 | esc:1 | len-3:8 | literal-run:8} for lz_resolve_kernel.
+// Literals land at their final output position, every match becomes a record for lz_resolve_kernel (format in inflate.cuh).
 //
 // 32 different streams per warp, persistent lanes.  Units are handed out 32 at a time to a warp whose lanes are all idle, so the
 // lanes of a warp run in phase (see the hand-out comment in the kernel).  A warp works in rounds that start with a full-mask vote:
@@ -22,9 +21,10 @@
 //            (LUTs, 18 long-code base words, ring): 16 resident warps per SM.
 // Input availability (the reference's bitsLeft guards) is checked lazily against an absolute bit position: reads past the
 // unit return zero bits and the first field that crosses the end reports symbolNotFound exactly as the reference does.
-// Code sets with Kraft sum > 1 go to inflate_slow_kernel via SWC_INTERNAL_NEEDS_SLOW (same contract as K1).
+// Code sets with Kraft sum > 1 go to inflate_slow_kernel via SWC_INTERNAL_NEEDS_SLOW.
 // Variants that fused the LZ77 copy into this kernel were slower than this kernel followed by lz_resolve_kernel.
 #include "common.cuh"
+#include "deflate_tables.cuh"
 #include "inflate.cuh"
 #include "host_util.h"
 
@@ -32,14 +32,8 @@ namespace swc {
 namespace inflate {
 namespace k1l {
 
-#ifndef SWC_LB
-#define SWC_LB 7
-#endif
-#ifndef SWC_DB
-#define SWC_DB 5
-#endif
-constexpr int LB = SWC_LB;                  // lit/len LUT index bits
-constexpr int DB = SWC_DB;                  // distance LUT index bits
+constexpr int LB = 7;                       // lit/len LUT index bits
+constexpr int DB = 5;                       // distance LUT index bits
 // ---- per-lane shared memory: halfword area (entry h of lane l at H[h*32+l]), byte area (D[h*32+l]), word area (W[w*32+l]) ----
 constexpr int H_LIT = 0;
 constexpr int H_TOTAL = 1 << LB;            // lit/len LUT, 16-bit entries
@@ -55,57 +49,20 @@ constexpr int W_CL_SYM = 8;                 // 19 x u8
 static_assert(W_CL_SYM + 5 <= W_TOTAL, "code-length tables must fit the long-code words they alias");
 constexpr int RING_BYTES = 8 * 32 * 4;      // per warp: 8 words of compressed input per lane; 1 KiB, 1 KiB-aligned (address wrap by mask)
 constexpr int WARP_BYTES = H_TOTAL * 32 * 2 + D_TOTAL * 32 + W_TOTAL * 32 * 4;
-#ifndef SWC_K1L_WARPS
-#define SWC_K1L_WARPS 4
-#define SWC_K1L_CTAS 4
-#endif
-constexpr int WARPS_PER_CTA = SWC_K1L_WARPS;
-constexpr int CTAS_PER_SM = SWC_K1L_CTAS;   // 16 warps per SM with a 2^7-entry LUT (12.3 KB per warp)
+constexpr int WARPS_PER_CTA = 4;
+constexpr int CTAS_PER_SM = 4;              // 16 warps per SM with a 2^7-entry LUT (12.3 KB per warp)
 constexpr int LUT_WORDS = 64;               // CTA-shared length / distance base+extra tables
 // CTA layout: [rings: WARPS x 1 KiB][LUT_WORDS x 4][per-warp tables]
 constexpr size_t SMEM_BYTES = (size_t)WARPS_PER_CTA * RING_BYTES + LUT_WORDS * 4 + (size_t)WARPS_PER_CTA * WARP_BYTES;
 
-#ifndef SWC_KLIT2
-#define SWC_KLIT2 8
-#endif
-constexpr int KLIT = SWC_KLIT2;             // lookups a lane may do per round (<= 56 bits) before parked symbols are serviced
-static_assert(SWC_KLIT2 <= 8, "at most one 8-byte literal word may fill up per round (deferred store)");
+constexpr int KLIT = 8;                     // lookups a lane may do per round (<= 56 bits) before parked symbols are serviced
+static_assert(KLIT <= 8, "at most one 8-byte literal word may fill up per round (deferred store)");
 
-#ifndef SWC_PATIENCE_SHIFT
-#define SWC_PATIENCE_SHIFT 3
-#endif
-#ifndef SWC_HDR_BATCH
-#define SWC_HDR_BATCH 6
-#endif
-constexpr int HDR_BATCH = SWC_HDR_BATCH;    // lanes that gather at a block boundary before the warp parses their headers
+constexpr int PATIENCE_SHIFT = 3;           // an idle lane waits for its warp for at most 1/2^PATIENCE_SHIFT of its last unit's rounds
+constexpr int HDR_BATCH = 6;                // lanes that gather at a block boundary before the warp parses their headers
 
 constexpr u32 E_NONLIT = 0x8000u;           // LUT entry: bit15 = not a literal; [11:8] code length (0 = long / no code)
 constexpr u32 CODE_EOB = 31;                //   non-literal low byte: 0..28 length symbol 257+k, 29/30 = 286/287, 31 = end of block
-
-// RFC 1951 3.2.5 tables as {base | extra_bits << 16}; Deflate+Constants.swift:179-186 + Deflate.swift:188-189,206
-__constant__ u32 c_len_tab[32] = {
-    3, 4, 5, 6, 7, 8, 9, 10, 11 | 1 << 16, 13 | 1 << 16, 15 | 1 << 16, 17 | 1 << 16, 19 | 2 << 16, 23 | 2 << 16, 27 | 2 << 16,
-    31 | 2 << 16, 35 | 3 << 16, 43 | 3 << 16, 51 | 3 << 16, 59 | 3 << 16, 67 | 4 << 16, 83 | 4 << 16, 99 | 4 << 16,
-    115 | 4 << 16, 131 | 5 << 16, 163 | 5 << 16, 195 | 5 << 16, 227 | 5 << 16, 258, 0, 0, 0};
-__constant__ u32 c_dist_tab[32] = {
-    1, 2, 3, 4, 5 | 1 << 16, 7 | 1 << 16, 9 | 2 << 16, 13 | 2 << 16, 17 | 3 << 16, 25 | 3 << 16, 33 | 4 << 16, 49 | 4 << 16,
-    65 | 5 << 16, 97 | 5 << 16, 129 | 6 << 16, 193 | 6 << 16, 257 | 7 << 16, 385 | 7 << 16, 513 | 8 << 16, 769 | 8 << 16,
-    1025 | 9 << 16, 1537 | 9 << 16, 2049 | 10 << 16, 3073 | 10 << 16, 4097 | 11 << 16, 6145 | 11 << 16, 8193 | 12 << 16,
-    12289 | 12 << 16, 16385 | 13 << 16, 24577 | 13 << 16, 0, 0};
-__constant__ u8 c_cl_order[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
-
-struct Limits { u32 p[8]; };   // p[k] = limit[2k+1] | limit[2k+2] << 16 ; limit[L] = left-justified end of the length-L code range
-
-__device__ __forceinline__ int code_length(u32 r15, const Limits &lim) {
-    const u32 X = (r15 | (r15 << 16)) + 0x80008000u;
-    u32 t[8];
-#pragma unroll
-    for (int k = 0; k < 8; k++) t[k] = X - lim.p[k];
-    u32 a = __byte_perm(t[0], t[1], 0x7531), b = __byte_perm(t[2], t[3], 0x7531);
-    u32 c = __byte_perm(t[4], t[5], 0x7531), d = __byte_perm(t[6], t[7], 0x7531);
-    u32 v = (a & 0x80808080u) | ((b & 0x80808080u) >> 1) | ((c & 0x80808080u) >> 2) | ((d & 0x80808080u) >> 3);
-    return 1 + __popc(v);                                    // 16 => no code matches (incomplete set)
-}
 
 // The unit as seen by both readers: bit positions count from `origin`, the 16-byte aligned address at or below the unit's
 // first byte.  Bytes outside [ubeg, uend) read as zero.
@@ -274,15 +231,7 @@ struct Emit {
     }
     __device__ __forceinline__ void match(u32 len, u32 dist) {
         const u32 nop = op + len;
-        if (nop <= cap) {
-            u32 run = op - last_end;
-            if (run > 255) {                       // escape record: skip (run & ~255) literal bytes
-                const u32 skip = run & ~255u;
-                rec[nrec++] = 0x8000u | (skip & 0x7FFFu) | ((skip >> 15) << 16);
-                run &= 255u;
-            }
-            rec[nrec++] = (dist - 1) | ((len - 3) << 16) | (run << 24);
-        }
+        if (nop <= cap) put_match(rec, nrec, op - last_end, len, dist);
         last_end = nop;
         if ((op >> 3) != (nop >> 3)) {             // the match leaves the current word
             if (dirty) flush_partial();
@@ -332,10 +281,6 @@ __device__ __forceinline__ void rewind_tables(u32 *bo, int maxlen) {
             prev = w;
         }
     }
-}
-
-__device__ __forceinline__ int static_len(int i) {   // i < 288: lit/len, else distance (32 symbols of 5 bits)
-    return i < 144 ? 8 : i < 256 ? 9 : i < 280 ? 7 : i < 288 ? 8 : 5;
 }
 
 struct LaneMem {
@@ -612,7 +557,7 @@ inflate_lut_kernel(BatchArgs a) {
             a.status[unit] = status;
             a.rec_count[unit] = em.nrec;
             have_unit = false;
-            patience = rounds >> SWC_PATIENCE_SHIFT;
+            patience = rounds >> PATIENCE_SHIFT;
         }
         // Unit hand-out.  A unit keeps a lane busy for thousands of rounds, so WHEN lanes start matters: lanes that run in phase
         // share the header code (one pass serves all 32), finish together, and leave no tail of half-empty warps at the end of

@@ -3,8 +3,9 @@
 // validates (Sources/Common/CodingTree/Code.swift:15-39), DecodingTree.init overwrites heap slots
 // (DecodingTree.swift:22-32) and findNextSymbol returns at the first leaf on the path (:36-50) — so "shortest prefix
 // wins, and among equal paths the code assigned last wins".  That rule is emulated here directly on the sorted code
-// list (no 2^16-slot heap per tree).  Only units K1 flagged SWC_INTERNAL_NEEDS_SLOW are touched.
+// list (no 2^16-slot heap per tree).  Only units the Huffman stage (K1L / K1w) flagged SWC_INTERNAL_NEEDS_SLOW are touched.
 #include "common.cuh"
+#include "deflate_tables.cuh"
 #include "inflate.cuh"
 
 namespace swc {
@@ -60,11 +61,6 @@ struct SlowTree {
     }
 };
 
-__constant__ u8 s_cl_order[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
-__constant__ u16 s_len_base[29] = {3, 4, 5, 6, 7, 8, 9, 10, 11, 13, 15, 17, 19, 23, 27, 31, 35, 43, 51, 59, 67, 83, 99, 115, 131, 163, 195, 227, 258};
-__constant__ u16 s_dist_base[30] = {1, 2, 3, 4, 5, 7, 9, 13, 17, 25, 33, 49, 65, 97, 129, 193, 257, 385, 513, 769, 1025, 1537, 2049, 3073,
-                                    4097, 6145, 8193, 12289, 16385, 24577};
-
 __global__ void __launch_bounds__(64) inflate_slow_kernel(BatchArgs a) {
     const u64 unit = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (unit >= a.n) return;
@@ -100,8 +96,7 @@ __global__ void __launch_bounds__(64) inflate_slow_kernel(BatchArgs a) {
         } else {
             int hlit = 288, hdist = 32;
             if (btype == 1) {
-                for (int i = 0; i < 288; i++) lens[i] = i < 144 ? 8 : i < 256 ? 9 : i < 280 ? 7 : 8;
-                for (int i = 0; i < 32; i++) lens[288 + i] = 5;
+                for (int i = 0; i < 320; i++) lens[i] = (u8)static_len(i);
             } else {
                 if (r.left() < 14) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
                 hlit = (int)r.bits(5) + 257;
@@ -111,7 +106,7 @@ __global__ void __launch_bounds__(64) inflate_slow_kernel(BatchArgs a) {
                 if (r.left() < (u64)(3 * hclen)) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
                 u8 cll[19];
                 for (int i = 0; i < 19; i++) cll[i] = 0;
-                for (int i = 0; i < hclen; i++) cll[s_cl_order[i]] = (u8)r.bits(3);
+                for (int i = 0; i < hclen; i++) cll[c_cl_order[i]] = (u8)r.bits(3);
                 cl.build(cll, 19);
                 const int count = hlit + hdist;
                 for (int i = 0; i < count; i++) lens[i] = 0;
@@ -144,15 +139,17 @@ __global__ void __launch_bounds__(64) inflate_slow_kernel(BatchArgs a) {
                 if (s < 256) { if (op < cap) out[op] = (u8)s; op++; continue; }
                 if (s == 256) break;
                 if (s > 285) FAIL(SWC_DEFLATE_WRONG_SYMBOL);
-                const int eb = (s <= 260 || s == 285) ? 0 : (((s - 257) >> 2) - 1);
+                const u32 le = c_len_tab[s - 257];
+                const int eb = (int)(le >> 16);
                 if (r.left() < (u64)eb) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
-                const u32 length = s_len_base[s - 257] + r.bits(eb);
+                const u32 length = (le & 0xFFFFu) + r.bits(eb);
                 const int dc = dist.next(r);
                 if (dc < 0) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
                 if (dc > 29) FAIL(SWC_DEFLATE_WRONG_SYMBOL);
-                const int db = dc < 2 ? 0 : (dc >> 1) - 1;
+                const u32 de = c_dist_tab[dc];
+                const int db = (int)(de >> 16);
                 if (r.left() < (u64)db) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
-                const u64 d = (u64)s_dist_base[dc] + r.bits(db);
+                const u64 d = (u64)(de & 0xFFFFu) + r.bits(db);
                 if (d > op) FAIL(SWC_ERR_REFERENCE_TRAP);
                 for (u32 i = 0; i < length; i++) { if (op < cap) out[op] = out[op - d]; op++; }
             }

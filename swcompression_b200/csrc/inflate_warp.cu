@@ -1,6 +1,6 @@
 // inflate_warp.cu — K1w: Deflate Huffman stage, ONE WARP PER UNIT with speculative sub-stream decoding.
-// Same contract as inflate_huffman_kernel (inflate.cu): literals land at their final output position, matches become
-// 4-byte records for lz_resolve_kernel, every reference error / trap case is reproduced (Deflate.swift:30-249).
+// Literals land at their final output position, matches become records for lz_resolve_kernel (format in inflate.cuh),
+// every reference error / trap case is reproduced (Deflate.swift:30-249).
 //
 // Why: with one thread per stream every lane needs private decode tables (536 B) and ~10 issue slots per symbol.  With
 // one warp per stream the tables are shared, so a flat 2^11-entry lit/len LUT + 2^9-entry distance LUT fit in shared
@@ -12,8 +12,9 @@
 //   scan : exclusive prefix sums of bytes and records over the valid lanes give every lane its output offsets.
 //   pass B: every lane decodes its window once more from the now-proven start and emits literals + records.
 // Block headers (code lengths, table build) and stored blocks are handled warp-uniformly / cooperatively.
-// Code sets with Kraft sum > 1 are routed to inflate_slow_kernel exactly like in K1.
+// Code sets with Kraft sum > 1 are routed to inflate_slow_kernel exactly like in K1L.
 #include "common.cuh"
+#include "deflate_tables.cuh"
 #include "inflate.cuh"
 #include "host_util.h"
 
@@ -22,10 +23,7 @@ namespace inflate {
 
 namespace w {
 
-#ifndef SWC_WIN_WORDS
-#define SWC_WIN_WORDS 19
-#endif
-constexpr int WIN_WORDS = SWC_WIN_WORDS;     // window per lane in 32-bit words; odd stride = conflict-free initial reads
+constexpr int WIN_WORDS = 19;                // window per lane in 32-bit words; odd stride = conflict-free initial reads
 constexpr int WIN_BITS = WIN_WORDS * 32;
 constexpr int STAGE_WORDS = 32 * WIN_WORDS + 8;
 constexpr int LIT_BITS = 11, DST_BITS = 9;
@@ -47,30 +45,6 @@ struct Smem {
     u8 lens[320];
     u8 cl_lut[128];              // code-length alphabet: sym << 3 | len (0 = no code)
 };
-
-__constant__ u32 k_len_tab[32] = {
-    3, 4, 5, 6, 7, 8, 9, 10, 11 | 1 << 16, 13 | 1 << 16, 15 | 1 << 16, 17 | 1 << 16, 19 | 2 << 16, 23 | 2 << 16, 27 | 2 << 16,
-    31 | 2 << 16, 35 | 3 << 16, 43 | 3 << 16, 51 | 3 << 16, 59 | 3 << 16, 67 | 4 << 16, 83 | 4 << 16, 99 | 4 << 16,
-    115 | 4 << 16, 131 | 5 << 16, 163 | 5 << 16, 195 | 5 << 16, 227 | 5 << 16, 258, 0, 0, 0};
-__constant__ u32 k_dist_tab[32] = {
-    1, 2, 3, 4, 5 | 1 << 16, 7 | 1 << 16, 9 | 2 << 16, 13 | 2 << 16, 17 | 3 << 16, 25 | 3 << 16, 33 | 4 << 16, 49 | 4 << 16,
-    65 | 5 << 16, 97 | 5 << 16, 129 | 6 << 16, 193 | 6 << 16, 257 | 7 << 16, 385 | 7 << 16, 513 | 8 << 16, 769 | 8 << 16,
-    1025 | 9 << 16, 1537 | 9 << 16, 2049 | 10 << 16, 3073 | 10 << 16, 4097 | 11 << 16, 6145 | 11 << 16, 8193 | 12 << 16,
-    12289 | 12 << 16, 16385 | 13 << 16, 24577 | 13 << 16, 0, 0};
-__constant__ u8 k_cl_order[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
-
-struct Limits { u32 p[8]; };
-
-__device__ __forceinline__ int code_length(u32 r15, const Limits &lim) {
-    const u32 X = (r15 | (r15 << 16)) + 0x80008000u;
-    u32 t[8];
-#pragma unroll
-    for (int k = 0; k < 8; k++) t[k] = X - lim.p[k];
-    u32 a = __byte_perm(t[0], t[1], 0x7531), b = __byte_perm(t[2], t[3], 0x7531);
-    u32 c = __byte_perm(t[4], t[5], 0x7531), d = __byte_perm(t[6], t[7], 0x7531);
-    u32 v = (a & 0x80808080u) | ((b & 0x80808080u) >> 1) | ((c & 0x80808080u) >> 2) | ((d & 0x80808080u) >> 3);
-    return 1 + __popc(v);
-}
 
 // ---- warp-uniform view of the unit's bitstream (header parsing): positions are bits from `wbase` ----
 struct Stream {
@@ -149,11 +123,7 @@ struct Emit {
     }
     __device__ __forceinline__ void match(u32 len, u32 dist) {
         const u32 nop = op + len;
-        if (nop <= cap) {
-            u32 run = op - last_end;
-            if (run > 255) { const u32 skip = run & ~255u; rec[ri++] = 0x8000u | (skip & 0x7FFFu) | ((skip >> 15) << 16); run &= 255u; }
-            rec[ri++] = (dist - 1) | ((len - 3) << 16) | (run << 24);
-        }
+        if (nop <= cap) put_match(rec, ri, op - last_end, len, dist);
         last_end = nop;
         if ((op >> 3) != (nop >> 3)) {
             if (dirty) {
@@ -173,10 +143,7 @@ struct Emit {
 };
 
 // One match: length extra bits + distance symbol + distance extra bits (Deflate.swift:186-232). Returns an error or 0.
-#ifndef SWC_KW_LIT
-#define SWC_KW_LIT 4
-#endif
-constexpr int KW_LIT = SWC_KW_LIT;      // lit/len steps per round before pending matches are serviced
+constexpr int KW_LIT = 4;               // lit/len steps per round before pending matches are serviced
 
 template <bool EMIT>
 __device__ __forceinline__ int window_match(const Smem &S, const Tables &T, const u32 *lens_tab, Cursor &c, u32 &p, u64 left,
@@ -227,7 +194,7 @@ __device__ __forceinline__ WinResult decode_window(const Smem &S, const Tables &
     bool active = enable;
     if (enable) { r.nbytes = 0; r.nrec = 0; r.head = 0; r.tail = 0; r.flags = 0; c.init(S.stage, start + stage_bit0); }
     // A round = up to KW_LIT lit/len symbols per lane, then ONE pass of the (long, rare) match path for every lane that
-    // parked a length symbol — the same scheme as the thread-per-unit kernel (inflate.cu): the match path used to run inside
+    // parked a length symbol — the same scheme as K1L's parked phase (inflate_lut.cu): the match path used to run inside
     // every step with ~4 of 32 lanes (22 % of the issued instructions, ncu source view).
     bool pend = false;
     u32 pvalue = 0; int peb = 0;
@@ -297,7 +264,7 @@ __global__ void __launch_bounds__(WARPS * 32)
 inflate_warp_kernel(BatchArgs a) {
     extern __shared__ __align__(16) u8 smem_raw[];
     __shared__ u32 lens_tab[64];
-    if (threadIdx.x < 32) { lens_tab[threadIdx.x] = k_len_tab[threadIdx.x]; lens_tab[32 + threadIdx.x] = k_dist_tab[threadIdx.x]; }
+    if (threadIdx.x < 32) { lens_tab[threadIdx.x] = c_len_tab[threadIdx.x]; lens_tab[32 + threadIdx.x] = c_dist_tab[threadIdx.x]; }
     __syncthreads();
     const u32 lane = lane_id(), warp = threadIdx.x >> 5;
     Smem &S = *reinterpret_cast<Smem *>(smem_raw + (size_t)warp * sizeof(Smem));
@@ -357,7 +324,7 @@ inflate_warp_kernel(BatchArgs a) {
             // ---- code lengths -> S.lens[0..hlit+hdist)
             int hlit = 288, hdist = 32;
             if (btype == 1) {
-                for (int i = lane; i < 320; i += 32) S.lens[i] = i < 144 ? 8 : i < 256 ? 9 : i < 280 ? 7 : i < 288 ? 8 : 5;
+                for (int i = lane; i < 320; i += 32) S.lens[i] = static_len(i);
             } else {
                 if (st.total - pos < 14) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
                 const u32 h = st.peek32(pos); pos += 14;
@@ -367,7 +334,7 @@ inflate_warp_kernel(BatchArgs a) {
                 const int hclen = (int)((h >> 10) & 15) + 4;
                 if (st.total - pos < (u64)(3 * hclen)) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
                 u64 cl = 0;
-                for (int i = 0; i < hclen; i++) { cl |= (u64)(st.peek32(pos) & 7) << (3 * k_cl_order[i]); pos += 3; }
+                for (int i = 0; i < hclen; i++) { cl |= (u64)(st.peek32(pos) & 7) << (3 * c_cl_order[i]); pos += 3; }
                 // canonical code of the 19-symbol alphabet -> 7-bit LUT (lane s handles symbol s)
                 u32 cnt8[8];
 #pragma unroll

@@ -192,8 +192,9 @@ def test_batch_host_pipelined(oracle):
 
 
 def test_large_batch_thread_kernel(oracle):
-    """>= 20000 units take the thread-per-unit K1 (persistent lanes, ticket counter; inflate.cu launch()): valid,
-    stored, truncated, corrupted, over-subscribed (slow kernel) and empty units side by side, all equal to the oracle."""
+    """>= 20000 units take K1L, the thread-per-unit table-lookup decoder (inflate_lut.cu; persistent lanes, ticket
+    counter): valid, stored, truncated, corrupted, over-subscribed (slow kernel) and empty units side by side, all equal
+    to the oracle."""
     rng = random.Random(17)
     distinct = []
     for i in range(40):

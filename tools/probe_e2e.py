@@ -25,7 +25,7 @@ if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "pcie":
         pcie(); sys.exit(0)
     subprocess.run([sys.executable, __file__, "pcie"])
-    for k1 in ("", "thread"):
+    for k1 in ("", "lut"):
         for S in (8, 16, 32):
             env = dict(os.environ, SWC_HOST_SLICES=str(S))
             if k1: env["SWC_DEFLATE_K1"] = k1
