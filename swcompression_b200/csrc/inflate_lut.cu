@@ -1,7 +1,7 @@
 // inflate_lut.cu — K1L: Deflate Huffman stage for large batches, table-lookup decode (one thread per unit).
 // Replaces the walk of Deflate.decompress(_: LsbBitReader) (reference Sources/Deflate/Deflate.swift:30-249) and
 // DecodingTree.findNextSymbol (Sources/Common/CodingTree/DecodingTree.swift:36-50) for the batched hot path.
-// Literals land at their final output position, every match becomes a record for lz_resolve_kernel (format in inflate.cuh).
+// Literals go to a packed stream, every match becomes a record for lz_resolve_kernel (format in inflate.cuh).
 //
 // 32 different streams per warp, persistent lanes.  Units are handed out 32 at a time to a warp whose lanes are all idle, so the
 // lanes of a warp run in phase (see the hand-out comment in the kernel).  A warp works in rounds that start with a full-mask vote:
@@ -10,8 +10,8 @@
 //            load — the only place global input is touched, so the load latency never sits on the decode chain.
 //   fast   : up to KLIT table lookups per lane: peek (funnel shift of a 64-bit register window, refilled without a branch, the
 //            next ring word already in a register) -> 2^7-entry 16-bit LUT in shared memory, halfword-interleaved across the
-//            warp (entry h of lane l at halfword h*32+l: conflict-free) -> literal: shifted into the 8-byte word of its final
-//            position (the word that fills up is stored once, after the loop); anything else (length, end of block, code
+//            warp (entry h of lane l at halfword h*32+l: conflict-free) -> literal: shifted into the next 8-byte word of the
+//            packed literal stream (the word that fills up is stored once, after the loop); anything else (length, end of block, code
 //            longer than 7 bits) parks the lane, which leaves the loop.
 //   parked : all parked lanes together: length extra bits, distance code (2^5-entry 8-bit LUT, canonical limit-compare decoder
 //            for longer codes), reference checks (Deflate.swift:199-232), one record per match.
@@ -177,74 +177,61 @@ struct HeaderBits {
 };
 
 // ------------------------------------------------------------------------------------------------ output side
-// `acc` is a shift register of the last 8 OUTPUT bytes, newest in the top byte, with zero standing in for every byte a match
-// produces (lz_resolve_kernel writes those later).  Whenever `op` reaches a multiple of 8 the register is exactly the aligned
-// word [op-8, op), so a literal costs two funnel shifts and the store needs no alignment arithmetic.
+// `acc` is a shift register of the last 8 literals, newest in the top byte.  Whenever `nlit` reaches a multiple of 8 the
+// register is exactly the word [nlit-8, nlit) of the packed literal stream (inflate.cuh), so a literal costs two funnel
+// shifts and the store needs no alignment arithmetic.  Literal words are stored as two 4-byte halves: the stream is only
+// 4-byte aligned.
 struct Emit {
-    u8 *out;        // unit output base (16-byte aligned)
-    u32 *rec;       // unit record stream
+    u8 *lits;       // unit literal stream
+    u32 *rec;       // end of the unit's scratch region (records grow downward from here)
     u32 op;         // bytes produced so far
+    u32 nlit;       // literals produced so far
     u32 cap;
     u32 last_end;   // end of the previous match (start of the current literal run)
     u32 nrec;
     u32 acc_lo, acc_hi;
-    bool dirty;     // the current word holds at least one literal
 
+    __device__ __forceinline__ void store_word(u32 lo, u32 hi) {          // the word that ends at nlit & ~7
+        u32 *p = (u32 *)(lits + (nlit & ~7u) - 8);
+        p[0] = lo; p[1] = hi;
+    }
     __device__ __forceinline__ void literal(u32 e) {           // low byte of e
         acc_lo = __funnelshift_r(acc_lo, acc_hi, 8);
         acc_hi = __funnelshift_r(acc_hi, e, 8);
-        dirty = true;
         op++;
-        if ((op & 7) == 0) {
-            if (op <= cap) *(uint2 *)(out + op - 8) = make_uint2(acc_lo, acc_hi);
-            dirty = false;
-        }
+        nlit++;
+        if ((nlit & 7) == 0 && op <= cap) store_word(acc_lo, acc_hi);
     }
     // fast-loop form: the word that fills up (at most one per round, KLIT <= 8) is parked in (f_lo, f_hi) and stored after the
-    // loop at a convergent point, at [(op & ~7) - 8, op & ~7)
+    // loop at a convergent point.  Only literals follow it in the round, so its last literal sat at output byte op - (nlit & 7) - 1.
     __device__ __forceinline__ void literal_deferred(u32 e, u32 &f_lo, u32 &f_hi, bool &full) {
         acc_lo = __funnelshift_r(acc_lo, acc_hi, 8);
         acc_hi = __funnelshift_r(acc_hi, e, 8);
         op++;
-        const bool fill = (op & 7) == 0;
+        nlit++;
+        const bool fill = (nlit & 7) == 0;
         f_lo = fill ? acc_lo : f_lo;
         f_hi = fill ? acc_hi : f_hi;
         full = full || fill;
-        dirty = !fill;
     }
     __device__ __forceinline__ void store_deferred(u32 f_lo, u32 f_hi) {
-        const u32 p = op & ~7u;                                // the filled word ends here
-        if (p <= cap) *(uint2 *)(out + p - 8) = make_uint2(f_lo, f_hi);
-    }
-    // the k = op & 7 bytes of the unfinished word, moved down to byte 0 (bytes above k are zero)
-    __device__ __forceinline__ uint2 partial_word() const {
-        const u32 sh = 8 * (8 - (op & 7));                     // 8..56
-        if (sh >= 32) return make_uint2(acc_hi >> (sh - 32), 0u);
-        return make_uint2(__funnelshift_r(acc_lo, acc_hi, sh), acc_hi >> sh);
-    }
-    __device__ __forceinline__ void flush_partial() {          // requires dirty (hence op & 7 != 0)
-        const uint2 w = partial_word();
-        if ((op | 7) < cap) { *(uint2 *)(out + (op & ~7u)) = w; return; }
-        const u64 v = ((u64)w.y << 32) | w.x;                  // last, partial word of the capacity: stay inside it
-        for (u32 i = op & ~7u; i < op; i++)
-            if (i < cap) out[i] = (u8)(v >> ((i & 7) * 8));
+        if (op - (nlit & 7) <= cap) store_word(f_lo, f_hi);
     }
     __device__ __forceinline__ void match(u32 len, u32 dist) {
         const u32 nop = op + len;
         if (nop <= cap) put_match(rec, nrec, op - last_end, len, dist);
         last_end = nop;
-        if ((op >> 3) != (nop >> 3)) {             // the match leaves the current word
-            if (dirty) flush_partial();
-            dirty = false;
-            acc_lo = 0; acc_hi = 0;                // the new word starts with (nop & 7) match bytes = zeros
-        } else {                                   // it stays inside: shift `len` (< 8) zero bytes in
-            const u32 sh = 8 * len;
-            if (sh >= 32) { acc_lo = acc_hi >> (sh - 32); acc_hi = 0; }
-            else { acc_lo = __funnelshift_r(acc_lo, acc_hi, sh); acc_hi >>= sh; }
-        }
         op = nop;
     }
-    __device__ __forceinline__ void finish() { if (dirty) flush_partial(); }
+    // stores the last, partial literal word when it fits below the records (inflate.cuh); false when it does not
+    __device__ __forceinline__ bool finish(u64 region) {
+        if (op > cap) return true;                             // overflow: K2 skips the unit, nothing to hand over
+        if ((u64)nlit + 4ull * nrec > region) return false;
+        const u32 k = nlit & 7;
+        const u64 v = ((u64)acc_hi << 32) | acc_lo;
+        for (u32 i = 0; i < k; i++) lits[(nlit & ~7u) + i] = (u8)(v >> (8 * (8 - k + i)));
+        return true;
+    }
     __device__ __forceinline__ void stored_byte(u32 b) { literal(b); }
 };
 
@@ -546,12 +533,13 @@ inflate_lut_kernel(BatchArgs a) {
     sp.origin = sp.ubeg = sp.uend = nullptr; sp.pos0 = sp.end = 0;
     br.lo = br.hi = br.nxt = 0;
     br.pos = 0; br.wend = 32; br.rptr = 0; br.wr = 0; br.nextc = 0; br.pre = make_uint4(0, 0, 0, 0);
-    em.out = nullptr; em.rec = nullptr; em.op = 0; em.cap = 0; em.last_end = 0; em.nrec = 0; em.acc_lo = em.acc_hi = 0; em.dirty = false;
+    em.lits = nullptr; em.rec = nullptr; em.op = 0; em.nlit = 0; em.cap = 0; em.last_end = 0; em.nrec = 0; em.acc_lo = em.acc_hi = 0;
     u32 rounds = 0, patience = 0;     // rounds spent on the current unit / rounds an idle lane still waits for its warp
     for (;;) {
         if (state == ST_DONE && have_unit) {                                             // retire the finished unit
-            em.finish();
+            const bool fits = em.finish(region_bytes(a.out_off[unit], cap64));
             if (status == SWC_OK && (u64)em.op > cap64) status = SWC_ERR_OUTPUT_OVERFLOW;
+            if (status == SWC_OK && !fits) status = SWC_INTERNAL_NEEDS_SLOW;
             a.consumed_bits[unit] = br.pos - sp.pos0;
             a.out_len[unit] = em.op;
             a.status[unit] = status;
@@ -587,10 +575,10 @@ inflate_lut_kernel(BatchArgs a) {
                         status = SWC_OK;
                         const u64 in_len = a.in_len[unit];
                         cap64 = a.out_cap[unit];
-                        em.out = a.out_base + a.out_off[unit];
-                        em.rec = a.rec_base + rec_start(a.out_off[unit]);
+                        em.lits = (u8 *)(a.rec_base + rec_start(a.out_off[unit]));
+                        em.rec = a.rec_base + rec_start(a.out_off[unit] + cap64);
                         em.cap = cap64 > 0xFFFFFFF0ull ? 0xFFFFFFF0u : (u32)cap64;
-                        em.op = 0; em.last_end = 0; em.nrec = 0; em.acc_lo = em.acc_hi = 0; em.dirty = false;
+                        em.op = 0; em.nlit = 0; em.last_end = 0; em.nrec = 0; em.acc_lo = em.acc_hi = 0;
                         const u32 bitskip = a.start_bits ? a.start_bits[unit] : 0;
                         sp.ubeg = a.in_base + a.in_off[unit];
                         sp.uend = sp.ubeg + in_len;

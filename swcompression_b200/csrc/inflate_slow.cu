@@ -162,7 +162,7 @@ done:
     a.out_len[unit] = op;
     a.consumed_bits[unit] = r.pos - skip;
     a.status[unit] = status;
-    a.rec_count[unit] = 0;      // K2 has nothing to replay for this unit
+    a.rec_count[unit] = REC_DIRECT;      // the output is written: K2 leaves the unit alone
 }
 
 void launch_slow(const BatchArgs &a, cudaStream_t stream) {

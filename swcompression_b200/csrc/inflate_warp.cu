@@ -1,5 +1,5 @@
 // inflate_warp.cu — K1w: Deflate Huffman stage, ONE WARP PER UNIT with speculative sub-stream decoding.
-// Literals land at their final output position, matches become records for lz_resolve_kernel (format in inflate.cuh),
+// Literals go to a packed stream, matches become records for lz_resolve_kernel (format in inflate.cuh),
 // every reference error / trap case is reproduced (Deflate.swift:30-249).
 //
 // Why: with one thread per stream every lane needs private decode tables (536 B) and ~10 issue slots per symbol.  With
@@ -7,9 +7,9 @@
 // memory (one LDS per symbol), and the 32 lanes decode DIFFERENT 288-bit windows of the SAME block concurrently:
 //   chunk = 32 windows.  Lane 0 starts at the known symbol boundary; lanes 1..31 guess their window start.
 //   pass A (repeat until nothing changes): each lane whose start changed decodes its window and reports where its last
-//          symbol ended (= the next lane's true start), plus byte / record counts.  Huffman streams self-synchronise
+//          symbol ended (= the next lane's true start), plus byte / literal / record counts.  Huffman streams self-synchronise
 //          within a few symbols, so a wrong start almost always yields the right end: typically 2 rounds.
-//   scan : exclusive prefix sums of bytes and records over the valid lanes give every lane its output offsets.
+//   scan : exclusive prefix sums of bytes, literals and records over the valid lanes give every lane its offsets.
 //   pass B: every lane decodes its window once more from the now-proven start and emits literals + records.
 // Block headers (code lengths, table build) and stored blocks are handled warp-uniformly / cooperatively.
 // Code sets with Kraft sum > 1 are routed to inflate_slow_kernel exactly like in K1L.
@@ -96,6 +96,7 @@ __device__ __forceinline__ int canon_decode(const Smem &S, const Limits &lim, u3
 struct WinResult {
     u32 end;        // bit position (relative to chunk base) after the last symbol decoded
     u32 nbytes;     // output bytes produced
+    u32 nlit;       // literal bytes produced
     u32 nrec;       // records produced EXCLUDING a possible escape in front of the first match
     u32 head;       // literal bytes before the first match (== nbytes when no match)
     u32 tail;       // literal bytes after the last match
@@ -104,41 +105,23 @@ struct WinResult {
 
 // Emission state of one lane in pass B
 struct Emit {
-    u8 *out; u32 *rec;
+    u8 *lits;        // unit literal stream
+    u32 *rec;        // end of the unit's scratch region (records grow downward from here)
     u32 cap;
-    u32 lo;          // first byte this lane owns (words below it are shared with the previous lane)
     u32 op;          // next output byte (absolute in unit)
+    u32 li;          // next literal index (absolute in unit)
     u32 last_end;    // end of the previous match (absolute), for the literal-run field
     u32 ri;          // next record index (absolute in unit)
-    u64 acc; bool dirty;
-    __device__ __forceinline__ void store_word(u32 wstart, u32 upto) {      // bytes [wstart, upto) of acc are ours
-        if (wstart >= lo && (upto & 7) == 0 && upto <= cap) { *(u64 *)(out + wstart) = acc; return; }
-        for (u32 i = wstart < lo ? lo : wstart; i < upto; i++) if (i < cap) out[i] = (u8)(acc >> ((i & 7) * 8));
-    }
     __device__ __forceinline__ void literal(u32 byte) {
-        acc |= (u64)byte << ((op & 7) * 8);
-        dirty = true;
+        if (op < cap) lits[li] = (u8)byte;
+        li++;
         op++;
-        if ((op & 7) == 0) { store_word(op - 8, op); acc = 0; dirty = false; }
     }
     __device__ __forceinline__ void match(u32 len, u32 dist) {
         const u32 nop = op + len;
         if (nop <= cap) put_match(rec, ri, op - last_end, len, dist);
         last_end = nop;
-        if ((op >> 3) != (nop >> 3)) {
-            if (dirty) {
-                // bytes [op&~7, op) hold literals; the rest of the word belongs to the match (K2 fills it)
-                const u32 ws = op & ~7u;
-                if (ws >= lo && ws + 8 <= cap) *(u64 *)(out + ws) = acc;
-                else for (u32 i = ws < lo ? lo : ws; i < op; i++) if (i < cap) out[i] = (u8)(acc >> ((i & 7) * 8));
-            }
-            acc = 0; dirty = false;
-        }
         op = nop;
-    }
-    __device__ __forceinline__ void finish() {
-        if (dirty) { const u32 ws = op & ~7u; for (u32 i = ws < lo ? lo : ws; i < op; i++) if (i < cap) out[i] = (u8)(acc >> ((i & 7) * 8)); }
-        dirty = false; acc = 0;
     }
 };
 
@@ -192,7 +175,7 @@ __device__ __forceinline__ WinResult decode_window(const Smem &S, const Tables &
     int err = 0;
     bool eob = false;
     bool active = enable;
-    if (enable) { r.nbytes = 0; r.nrec = 0; r.head = 0; r.tail = 0; r.flags = 0; c.init(S.stage, start + stage_bit0); }
+    if (enable) { r.nbytes = 0; r.nlit = 0; r.nrec = 0; r.head = 0; r.tail = 0; r.flags = 0; c.init(S.stage, start + stage_bit0); }
     // A round = up to KW_LIT lit/len symbols per lane, then ONE pass of the (long, rare) match path for every lane that
     // parked a length symbol — the same scheme as K1L's parked phase (inflate_lut.cu): the match path used to run inside
     // every step with ~4 of 32 lanes (22 % of the issued instructions, ncu source view).
@@ -221,7 +204,7 @@ __device__ __forceinline__ WinResult decode_window(const Smem &S, const Tables &
                     c.skip(L); p += (u32)L;
                     if (kind == 0) {
                         if (EMIT) em->literal(value);
-                        r.nbytes++; run++;
+                        r.nbytes++; r.nlit++; run++;
                     } else if (kind == 1) {
                         eob = true;
                     } else if (kind == 3) {
@@ -278,12 +261,13 @@ inflate_warp_kernel(BatchArgs a) {
         const u64 in_len = a.in_len[unit];
         const u64 cap64 = a.out_cap[unit];
         const u32 cap = cap64 > 0xFFFFFFF0ull ? 0xFFFFFFF0u : (u32)cap64;
-        u8 *out = a.out_base + a.out_off[unit];
-        u32 *rec = a.rec_base + rec_start(a.out_off[unit]);
+        u8 *lits = (u8 *)(a.rec_base + rec_start(a.out_off[unit]));
+        u32 *rec = a.rec_base + rec_start(a.out_off[unit] + cap64);
         const u32 bitskip = a.start_bits ? a.start_bits[unit] : 0;
         int status = SWC_OK;
         u64 pos = 0;                 // bits consumed from the unit start (true chain)
         u64 op = 0;                  // bytes produced
+        u32 nlit = 0;                // literals produced
         u32 nrec = 0;
         u32 run_carry = 0;           // literal bytes since the last match
         Stream st;
@@ -314,8 +298,8 @@ inflate_warp_kernel(BatchArgs a) {
                 if (((st.total - pos) >> 3) < length) FAIL(SWC_DEFLATE_WRONG_UNCOMPRESSED_BLOCK_LENGTHS);
                 const u8 *src = (const u8 *)st.wbase + ((pos + st.bit0) >> 3);
                 if (op + length > 0xFFFFFFF0ull) FAIL(SWC_ERR_UNSUPPORTED);
-                if (op + length <= cap) for (u32 i = lane; i < length; i += 32) out[op + i] = src[i];
-                op += length; run_carry += length;
+                if (op + length <= cap) for (u32 i = lane; i < length; i += 32) lits[nlit + i] = src[i];
+                op += length; nlit += length; run_carry += length;
                 pos += (u64)length * 8;
                 __syncwarp();
                 if (is_last) break;
@@ -463,7 +447,7 @@ inflate_warp_kernel(BatchArgs a) {
                 const u32 hi = (lane + 1) * WIN_BITS;
                 u32 start = lane * WIN_BITS;
                 bool dirty = true, valid = true;
-                WinResult r; r.end = 0; r.nbytes = 0; r.nrec = 0; r.head = 0; r.tail = 0; r.flags = 0;
+                WinResult r; r.end = 0; r.nbytes = 0; r.nlit = 0; r.nrec = 0; r.head = 0; r.tail = 0; r.flags = 0;
                 // pass A: iterate until every window starts where its predecessor ended
                 for (int round = 0; round < 33; round++) {
                     r = decode_window<false>(S, T, lens_tab, dirty && valid, start, hi, left, stage_bit0, nullptr, r);
@@ -498,32 +482,33 @@ inflate_warp_kernel(BatchArgs a) {
                 u32 myrec = contrib ? r.nrec : 0;
                 if (contrib && (r.flags & 1) && my_carry + r.head > 255) myrec++;
                 u32 mybytes = contrib ? r.nbytes : 0;
-                u32 ib = mybytes, ir = myrec;
+                u32 mylit = contrib ? r.nlit : 0;
+                u32 ib = mybytes, il = mylit, ir = myrec;
 #pragma unroll
                 for (int d = 1; d < 32; d <<= 1) {
-                    const u32 vb = __shfl_up_sync(SWC_FULL, ib, d), vr = __shfl_up_sync(SWC_FULL, ir, d);
-                    if (lane >= (u32)d) { ib += vb; ir += vr; }
+                    const u32 vb = __shfl_up_sync(SWC_FULL, ib, d), vl = __shfl_up_sync(SWC_FULL, il, d), vr = __shfl_up_sync(SWC_FULL, ir, d);
+                    if (lane >= (u32)d) { ib += vb; il += vl; ir += vr; }
                 }
-                const u32 tot_b = __shfl_sync(SWC_FULL, ib, 31), tot_r = __shfl_sync(SWC_FULL, ir, 31);
+                const u32 tot_b = __shfl_sync(SWC_FULL, ib, 31), tot_l = __shfl_sync(SWC_FULL, il, 31), tot_r = __shfl_sync(SWC_FULL, ir, 31);
                 if (op + tot_b > 0xFFFFFFF0ull) FAIL(SWC_ERR_UNSUPPORTED);
                 // pass B: emit
                 int my_err = 0;
                 {
                     Emit em;
-                    em.out = out; em.rec = rec; em.cap = cap;
-                    em.op = (u32)op + (ib - mybytes); em.lo = em.op;
+                    em.lits = lits; em.rec = rec; em.cap = cap;
+                    em.op = (u32)op + (ib - mybytes);
+                    em.li = nlit + (il - mylit);
                     em.last_end = em.op - my_carry;
                     em.ri = nrec + (ir - myrec);
-                    em.acc = 0; em.dirty = false;
                     const WinResult rb = decode_window<true>(S, T, lens_tab, contrib, start, hi, left, stage_bit0, &em, r);
-                    if (contrib) { em.finish(); my_err = (int)(rb.flags >> 8); }
+                    if (contrib) my_err = (int)(rb.flags >> 8);
                 }
                 const u32 emask = __ballot_sync(SWC_FULL, my_err != 0);
                 if (emask) FAIL(__shfl_sync(SWC_FULL, my_err, __ffs(emask) - 1));                 // earliest error in stream order
                 // advance the true chain
                 const u32 endbits = __shfl_sync(SWC_FULL, r.end, last);
                 const u32 lflags = __shfl_sync(SWC_FULL, r.flags, last);
-                op += tot_b; nrec += tot_r; run_carry = carry;
+                op += tot_b; nlit += tot_l; nrec += tot_r; run_carry = carry;
                 pos += endbits;
                 __syncwarp();
                 if (lflags & 2) block_done = true;
@@ -535,6 +520,8 @@ inflate_warp_kernel(BatchArgs a) {
         __syncwarp();
         if (lane == 0) {
             if (status == SWC_OK && op > cap64) status = SWC_ERR_OUTPUT_OVERFLOW;
+            // a unit of fewer than 8 literals may not fit its literals below its records (inflate.cuh)
+            if (status == SWC_OK && (u64)nlit + 4ull * nrec > region_bytes(a.out_off[unit], cap64)) status = SWC_INTERNAL_NEEDS_SLOW;
             a.consumed_bits[unit] = pos;
             a.out_len[unit] = op;
             a.status[unit] = status;
