@@ -24,34 +24,49 @@ namespace inflate {
 // One warp per unit, the only writer of the unit's output, which it builds in order in a per-warp ring of RING bytes of
 // shared memory (output byte p lives at ring[(p + phase) % RING], phase = the output's address mod 16, so that aligned
 // 16-byte chunks of the output are aligned 16-byte chunks of the ring).  A batch is a run of consecutive records whose
-// output ends at most SPAN bytes past the batch start; lane j holds record j.  Per batch:
+// output ends at most SPAN bytes past the batch start; lane j holds record j, loaded one batch ahead.  Per batch:
 //   scan     : inclusive warp scans of (literal run + length) and of the literal run give every record its position and
 //              the offset of its literals in the batch's part of the literal stream;
-//   literals : the batch's literals are copied from the packed stream into shared memory with 16-byte loads, then every
-//              lane places literals: a binary search over the records' literal offsets (shuffles) finds each one's position;
-//   matches  : replayed 8 at a time by 4-lane sub-groups.  A record is READY when everything it reads is final: its source
-//              ends at or before the start of the oldest still-pending record of the 8 (bytes before that point are literals,
-//              older matches or earlier batches) — or it IS that oldest record.  Far matches therefore run 8-wide in one
-//              pass, chains of near matches (RLE-like data) degrade to in-order execution.  Overlapping copies (dist < len)
-//              replicate the period: every source byte lies in [start-dist, start), never in what the match itself writes.
-//              A source byte less than RING bytes behind the batch end is still in the ring; an older one has been written
-//              to the output by this warp and is read back from there;
+//   gather   : one round of 16-byte cp.async copies brings in the batch's literals from the packed stream and the sources
+//              of its FAR matches from the output.  A match is far when its first source byte is more than RING bytes behind
+//              the batch end (bend): with len <= 258 and bend - RING <= done - SPAN, its whole source then lies in output this
+//              warp has already flushed, and dist > RING - SPAN >= len.  Every other match reads only bytes that are still
+//              in the ring.  A far source takes at most len/16 + 2 aligned chunks, so a batch (<= 32 records, their lengths
+//              summing to <= SPAN) needs at most 128 of them, which a warp-wide scan packs into a 2 KiB staging buffer;
+//              the part of the output's first chunk that lies before out[0] is never read (that chunk is copied byte by
+//              byte);
+//   literals : every lane places literals: a binary search over the records' literal offsets (shuffles) finds each
+//              one's position;
+//   matches  : replayed 8 at a time by 4-lane sub-groups, reading shared memory only (far ones from the staging buffer,
+//              the others from the ring).  A record is READY when everything it reads is final: its source ends at or
+//              before the start of the oldest still-pending record of the 8 (bytes before that point are literals, older
+//              matches or earlier batches) — or it IS that oldest record.  Far matches therefore run 8-wide in one pass,
+//              chains of near matches (RLE-like data) degrade to in-order execution.  Overlapping copies (dist < len)
+//              replicate the period: every source byte lies in [start-dist, start), never in what the match itself writes;
 //   flush    : every whole 16-byte chunk of the output below the batch end goes out with one 16-byte store; the output's
 //              first and last partial chunks are written byte by byte, so no byte outside [0, out_len) is touched.
 // A batch stays within SPAN + 15 bytes of the first unflushed byte, so nothing is overwritten in the ring before it is
 // flushed.  A literal run too long for one batch (an escape of more than SPAN bytes, or the literals after the last match)
-// is placed in pieces of SPAN bytes.
+// is placed in pieces of SPAN bytes.  So a batch waits on global memory once: its records were loaded during the batch
+// before, its literals and far sources arrive together.
 namespace k2 {
 constexpr int WARPS = 8;
 constexpr int CTAS_PER_SM = 4;
 constexpr u32 RING = 2048;
 constexpr u32 SPAN = RING / 2;       // >= 255 + 258: one record of any kind but an escape fits a batch
 constexpr u32 LITBUF = SPAN + 32;    // a batch's literals plus the 16-byte alignment slack at both ends
+constexpr u32 FARBUF = 128 * 16;     // the far sources of a batch: at most 32 * 2 + SPAN / 16 chunks
+constexpr u32 NEAR = 0xFFFFFFFFu;    // staging offset of a match that reads the ring
 struct __align__(16) WarpSmem {
-    uint4 stage[32];                 // {start, length, distance} of the batch's records
+    uint4 stage[32];                 // {start, length, distance, staging offset of the first source byte | NEAR}
     u8 ring[RING];
     u8 lit[LITBUF];
+    u8 far[FARBUF];
 };
+__device__ __forceinline__ void cp_async16(void *dst, const void *src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"((u32)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
 }  // namespace k2
 
 __global__ void __launch_bounds__(k2::WARPS * 32, k2::CTAS_PER_SM)
@@ -92,11 +107,10 @@ lz_resolve_kernel(BatchArgs a) {
         }
         flushed = to;
     };
+    u32 rv = lane < nrec ? __ldg(rec - 1 - lane) : REC_ESC;              // record g + lane
     for (;;) {
         // ---- the batch: records g.. whose output ends within SPAN bytes of `done`
         const bool real = g + lane < nrec;
-        u32 rv = REC_ESC;
-        if (real) rv = *(rec - 1 - (g + lane));
         const Match m = get_match(rv);
         const u32 adv = m.adv - (lane == 0 ? part : 0u);
         const u32 run = adv - m.len;
@@ -126,13 +140,37 @@ lz_resolve_kernel(BatchArgs a) {
             delta = done;
             lend = lane == 0 ? nl : 0xFFFFFFFFu;
         }
-        S.stage[lane] = make_uint4(done + end - m.len, lane < k ? m.len : 0u, m.dist, 0u);
-        // ---- literals: packed stream -> shared memory (16-byte loads) -> their positions in the ring
+        if (k > 0) rv = g + lane < nrec ? __ldg(rec - 1 - (g + lane)) : REC_ESC;   // the next batch's records
+        const u32 bend = done + span;                            // batch end
+        // ---- gather: the literals (packed stream) and the far match sources (flushed output) -> shared memory
         const uintptr_t lsrc = (uintptr_t)(lits + lit);
-        const uint4 *lchunk = (const uint4 *)(lsrc & ~(uintptr_t)15);
+        const u8 *lchunk = (const u8 *)(lsrc & ~(uintptr_t)15);
         const u32 lofs = (u32)(lsrc & 15), nch = (lofs + nl + 15) >> 4;
-        for (u32 c = lane; c < nch; c += 32) ((uint4 *)S.lit)[c] = __ldg(lchunk + c);
+        for (u32 c = lane; c < nch; c += 32) cp_async16(S.lit + c * 16, lchunk + c * 16);
+        const u32 ms = done + end - m.len, mq = ms - m.dist;      // the lane's match: start, first source byte
+        const bool far = lane < k && m.len != 0 && mq + RING < bend;
+        const u32 c0 = (mq + ph) >> 4;                           // first source chunk (output chunk index)
+        const u32 fch = far ? ((mq + m.len - 1 + ph) >> 4) - c0 + 1 : 0u;
+        u32 fend = fch;                                          // inclusive scan: staging chunks up to this record
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const u32 v = __shfl_up_sync(SWC_FULL, fend, d);
+            if (lane >= (u32)d) fend += v;
+        }
+        const u32 fbeg = fend - fch;
+        const u8 *outa = out - ph;                               // 16-byte aligned: output chunk c starts at outa + 16 c
+        for (u32 c = 0; c < fch; c++) {
+            u8 *dst = S.far + (fbeg + c) * 16;
+            if (c0 + c > 0 || ph == 0) {
+                cp_async16(dst, outa + (c0 + c) * 16);
+            } else {
+                for (u32 b = ph; b < 16; b++) dst[b] = outa[b];  // the output's first chunk starts before out[0]
+            }
+        }
+        S.stage[lane] = make_uint4(ms, lane < k ? m.len : 0u, m.dist, far ? fbeg * 16 + ((mq + ph) & 15) : NEAR);
+        cp_async_wait_all();
         __syncwarp();
+        // ---- literals -> their positions in the ring
         for (u32 j0 = 0; j0 < nl; j0 += 32) {
             const u32 j = j0 + lane;
             u32 r = 0;                                           // records whose literals all precede literal j
@@ -143,15 +181,19 @@ lz_resolve_kernel(BatchArgs a) {
             if (j < nl) S.ring[(p + ph) & M] = S.lit[lofs + j];
         }
         lit += nl;
-        const u32 bend = done + span;                            // batch end
         __syncwarp();
         // ---- matches
-        auto src_byte = [&](u32 q) -> u8 { return q + RING >= bend ? S.ring[(q + ph) & M] : out[q]; };
 #pragma unroll 1
         for (u32 b0 = 0; b0 < k; b0 += 8) {
             const uint4 rc = S.stage[b0 + sub];                  // this sub-group's record
             const u32 s = rc.x, l = rc.y, d = rc.z;
             const u32 src_end = s - d + (l < d ? l : d);
+            // source byte i of the match: a far one from the staging buffer, a near one from the ring
+            const bool fr = rc.w != NEAR;
+            const u8 *sb = fr ? S.far : S.ring;
+            const u32 s0 = fr ? rc.w : s - d + ph, sm = fr ? 0xFFFFFFFFu : M;
+            const u32 alim = fr ? FARBUF : M - 3;               // source index of 4 bytes that do not wrap around
+            auto src_byte = [&](u32 i) -> u8 { return sb[(s0 + i) & sm]; };
             bool pend = l != 0;
             u32 pmask = __ballot_sync(SWC_FULL, pend && t == 0); // bit 4*sub per pending record
             while (pmask) {
@@ -159,23 +201,37 @@ lz_resolve_kernel(BatchArgs a) {
                 const u32 frontier = S.stage[b0 + oldest].x;
                 const bool ready = pend && (sub == oldest || src_end <= frontier);
                 if (ready) {
-                    const u32 q0 = s - d;
                     if (d >= l) {
-                        // four bytes per lane and trip, all four loads issued before the first store
-                        for (u32 i = t; i < l; i += 16) {
-                            const bool p1 = i + 4 < l, p2 = i + 8 < l, p3 = i + 12 < l;
-                            const u8 v0 = src_byte(q0 + i);
-                            u8 v1 = 0, v2 = 0, v3 = 0;
-                            if (p1) v1 = src_byte(q0 + i + 4);
-                            if (p2) v2 = src_byte(q0 + i + 8);
-                            if (p3) v3 = src_byte(q0 + i + 12);
-                            S.ring[(s + i + ph) & M] = v0;
-                            if (p1) S.ring[(s + i + 4 + ph) & M] = v1;
-                            if (p2) S.ring[(s + i + 8 + ph) & M] = v2;
-                            if (p3) S.ring[(s + i + 12 + ph) & M] = v3;
+                        // four consecutive bytes per lane and trip, all four loads issued before the first store; one
+                        // source and one ring address per trip unless the four bytes wrap around the ring
+                        for (u32 i = 4 * t; i < l; i += 16) {
+                            const bool p1 = i + 1 < l, p2 = i + 2 < l, p3 = i + 3 < l;
+                            const u32 a = (s0 + i) & sm, b = (s + i + ph) & M;
+                            u32 v0, v1 = 0, v2 = 0, v3 = 0;
+                            if (a <= alim && b <= M - 3) {
+                                const u8 *src = sb + a;
+                                u8 *dst = S.ring + b;
+                                v0 = src[0];
+                                if (p1) v1 = src[1];
+                                if (p2) v2 = src[2];
+                                if (p3) v3 = src[3];
+                                dst[0] = v0;
+                                if (p1) dst[1] = v1;
+                                if (p2) dst[2] = v2;
+                                if (p3) dst[3] = v3;
+                            } else {
+                                v0 = src_byte(i);
+                                if (p1) v1 = src_byte(i + 1);
+                                if (p2) v2 = src_byte(i + 2);
+                                if (p3) v3 = src_byte(i + 3);
+                                S.ring[b] = v0;
+                                if (p1) S.ring[(b + 1) & M] = v1;
+                                if (p2) S.ring[(b + 2) & M] = v2;
+                                if (p3) S.ring[(b + 3) & M] = v3;
+                            }
                         }
                     } else {
-                        for (u32 i = t; i < l; i += 4) S.ring[(s + i + ph) & M] = src_byte(q0 + i % d);
+                        for (u32 i = t; i < l; i += 4) S.ring[(s + i + ph) & M] = src_byte(i % d);
                     }
                     pend = false;
                 }
