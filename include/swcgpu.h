@@ -101,7 +101,37 @@ int32_t swc_lz4_block_decompress_batch_host(const uint8_t *in_base, const uint64
                                             uint64_t out_capacity_total,
                                             uint64_t *out_len, int32_t *status, uint64_t n);
 
-/* ---- BZip2 --------------------------------------------------------------------------------------------------
+/* ---- LZ4 compression ----------------------------------------------------------------------------------------
+ * LZ4.compress(data:)                                                     Sources/LZ4/LZ4+Compress.swift:16-19
+ * LZ4.compress(data:independentBlocks:blockChecksums:contentChecksum:contentSize:blockSize:dictionary:dictionaryID:)
+ *                                                                          Sources/LZ4/LZ4+Compress.swift:47-154
+ * LZ4.compress(block:_:) (private raw-block compressor)                   Sources/LZ4/LZ4+Compress.swift:156-298 -> *_batch
+ * The output bytes equal the reference's for every option combination (its greedy parse, not liblz4's).  The reference
+ * cannot fail; where it traps (block_size outside 1 ... 4 MiB, a 1-3 byte dictionary, a dependent frame of blocks of
+ * 1-3 bytes) these calls return SWC_ERR_REFERENCE_TRAP.
+ * swc_lz4_compress: one frame from host memory; dict == NULL is `dictionary: nil`, has_dict_id == 0 `dictionaryID: nil`. */
+int32_t swc_lz4_compress(const uint8_t *in, size_t in_len, int32_t independent_blocks, int32_t block_checksums,
+                         int32_t content_checksum, int32_t content_size, int64_t block_size,
+                         const uint8_t *dict, size_t dict_len, int32_t has_dict_id, uint32_t dict_id,
+                         uint8_t **out, size_t *out_len);
+/* Raw blocks, device memory, asynchronous on `cuda_stream` (the unit sizes are read back first, which synchronises).
+ * Unit i compresses in_base[in_off[i] ..+ in_len[i]) with the dictionary window in_base[dict_off[i] ..+ dict_len[i])
+ * (dict_off == dict_len == NULL: no dictionary).  The window expresses both frame modes: the user's dictionary, or the
+ * last <= 64 KiB of the previous block.  Windows longer than 64 KiB act as their last 64 KiB, as in the reference.
+ * out_len[i] is the exact size of the raw block compress(block:_:) returns, even when it is longer than the input; if it
+ * exceeds out_cap[i] the unit reports SWC_ERR_OUTPUT_OVERFLOW and writes nothing.  Any input or output alignment; an empty
+ * unit encodes to the single token 0x00 (the reference's release build; its assert at :261 is compiled out).  Units longer
+ * than 4 MiB report SWC_ERR_UNSUPPORTED.  scratch may be NULL (library pool); a caller's scratch of
+ * swc_lz4_compress_batch_scratch_bytes(n, sum of in_len[i] + min(dict_len[i], 65536)) bytes runs the batch in one
+ * slice, a smaller one in several (it must hold the largest unit). */
+size_t  swc_lz4_compress_batch_scratch_bytes(uint64_t n, uint64_t window_bytes_total);
+int32_t swc_lz4_block_compress_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                                     const uint64_t *dict_off /* NULL = none */, const uint64_t *dict_len,
+                                     uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                     uint64_t *out_len, int32_t *status, uint64_t n,
+                                     void *scratch, size_t scratch_bytes, void *cuda_stream);
+
+/* ---- BZip2--------------------------------------------------------------------------------------------------
  * BZip2.decompress(data:)            Sources/BZip2/BZip2.swift:22-26
  * BZip2.multiDecompress(data:)       Sources/BZip2/BZip2.swift:40-48
  * BZip2.decompress(_: MsbBitReader)  Sources/BZip2/BZip2.swift:50-95 */

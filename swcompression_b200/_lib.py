@@ -61,6 +61,10 @@ def lib():
         L.swc_lz4_multi_decompress.argtypes = [vp, sz, vp, sz, i32, u32, C.POINTER(vp), szp, C.POINTER(vp), szp]
         L.swc_lz4_block_decompress_batch.argtypes = [vp, vp, vp, vp, u64, vp, vp, vp, vp, vp, u64, vp]
         L.swc_lz4_block_decompress_batch_host.argtypes = [vp, vp, vp, u64, vp, vp, vp, u64, vp, vp, u64]
+        L.swc_lz4_compress.argtypes = [vp, sz, i32, i32, i32, i32, C.c_int64, vp, sz, i32, u32, C.POINTER(vp), szp]
+        L.swc_lz4_compress_batch_scratch_bytes.restype = C.c_size_t
+        L.swc_lz4_compress_batch_scratch_bytes.argtypes = [C.c_uint64, C.c_uint64]
+        L.swc_lz4_block_compress_batch.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, u64, vp, sz, vp]
         L.swc_bzip2_decompress.argtypes = [vp, sz, sz, C.POINTER(vp), szp, szp]
         L.swc_bzip2_multi_decompress.argtypes = [vp, sz, C.POINTER(vp), szp, C.POINTER(vp), szp]
         L.swc_bzip2_decompress_batch.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, u64, vp]

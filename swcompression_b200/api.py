@@ -8,6 +8,7 @@ meaning, same error cases), routed through the C ABI of libswcgpu.so.
     LZMA2.decompress(data:)                             LZMA2.decompress(data)
     LZ4.decompress(data:[dictionary:dictionaryID:])     LZ4.decompress(data[, dictionary, dictionaryID])
     LZ4.multiDecompress(data:dictionary:dictionaryID:)  LZ4.multiDecompress(...)
+    LZ4.compress(data:[independentBlocks:...])          LZ4.compress(data[, independentBlocks, ...])
     GzipArchive.unarchive / multiUnarchive -> [Member]  GzipArchive.unarchive / multiUnarchive -> [GzipArchive.Member]
     GzipHeader(archive:) / ZlibHeader(archive:)         GzipHeader(archive) / ZlibHeader(archive)
     ZlibArchive.unarchive                               ZlibArchive.unarchive
@@ -117,7 +118,28 @@ def _dict_args(dictionary, dictionaryID):
 
 
 class LZ4:
-    """Sources/LZ4/LZ4.swift:33-146"""
+    """Sources/LZ4/LZ4.swift:33-146, Sources/LZ4/LZ4+Compress.swift:16-154"""
+
+    @staticmethod
+    def compress(data, independentBlocks=True, blockChecksums=False, contentChecksum=True, contentSize=False,
+                 blockSize=4 * 1024 * 1024, dictionary=None, dictionaryID=None):
+        """LZ4.compress(data:) with the defaults, or the overload with every option; the frame equals the reference's byte
+        for byte.  The reference cannot throw; where it traps (blockSize outside 1 ... 4 MiB, a 1-3 byte dictionary) this
+        raises the engine's referenceTrap error."""
+        L = _lib.lib()
+        buf, n = _lib.inbuf(data)
+        if dictionary is None:
+            dp, dn = None, 0
+        else:
+            dp, dn = _lib.inbuf(dictionary)
+        out, out_len = C.c_void_p(), C.c_size_t(0)
+        st = L.swc_lz4_compress(buf, n, int(bool(independentBlocks)), int(bool(blockChecksums)), int(bool(contentChecksum)),
+                                int(bool(contentSize)), int(blockSize), dp, dn, 0 if dictionaryID is None else 1,
+                                int(dictionaryID or 0), C.byref(out), C.byref(out_len))
+        payload = _lib.take(out, out_len)
+        if st != 0:
+            raise error_for(st, None)
+        return payload
 
     @staticmethod
     def decompress(data, dictionary=None, dictionaryID=None):

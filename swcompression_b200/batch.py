@@ -30,7 +30,10 @@ def pack_units(units, align=16):
 
 
 class Batch:
-    """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'lzma2')."""
+    """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'lzma2', 'lz4_block_compress').
+
+    'lz4_block_compress' compresses each unit into a raw LZ4 block (LZ4+Compress.swift:156-277); `aux` is then an optional
+    (dict_off, dict_len) pair of u64 arrays placing each unit's dictionary window inside `in_buf`."""
 
     def __init__(self, codec, in_buf, in_off, in_len, out_cap, device="cuda:0", aux=None):
         self.codec = codec
@@ -54,7 +57,19 @@ class Batch:
         self.d_consumed = torch.zeros(self.n, dtype=torch.int64, device=self.device)
         self.d_status = torch.full((self.n,), -1, dtype=torch.int32, device=self.device)
         self.d_scratch = None
-        self.d_aux = None if aux is None else torch.from_numpy(np.frombuffer(bytes(aux), dtype=np.uint8).copy()).to(self.device)
+        self.d_dict_off = self.d_dict_len = None
+        if codec == "lz4_block_compress":
+            self.d_aux = None
+            dl = np.zeros(self.n, dtype=np.uint64)
+            if aux is not None:
+                self.d_dict_off, self.d_dict_len = t(np.asarray(aux[0], dtype=np.uint64)), t(np.asarray(aux[1], dtype=np.uint64))
+                dl = np.asarray(aux[1], dtype=np.uint64)
+            window = int(np.asarray(in_len, dtype=np.uint64).sum()) + int(np.minimum(dl, np.uint64(65536)).sum())
+            # past 16 GiB of scratch the library runs the batch in slices that fit
+            nbytes = min(_lib.lib().swc_lz4_compress_batch_scratch_bytes(self.n, window), 16 << 30)
+            self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        else:
+            self.d_aux = None if aux is None else torch.from_numpy(np.frombuffer(bytes(aux), dtype=np.uint8).copy()).to(self.device)
         if codec == "deflate":
             nbytes = _lib.lib().swc_deflate_batch_scratch_bytes(self.n, self.out_total)
             self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
@@ -77,6 +92,12 @@ class Batch:
             st = L.swc_lz4_block_decompress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), None, 0, p(self.d_out),
                                                   p(self.d_out_off), p(self.d_out_cap), p(self.d_out_len), p(self.d_status),
                                                   self.n, stream)
+        elif self.codec == "lz4_block_compress":
+            opt = lambda t: None if t is None else p(t)
+            st = L.swc_lz4_block_compress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), opt(self.d_dict_off),
+                                                opt(self.d_dict_len), p(self.d_out), p(self.d_out_off), p(self.d_out_cap),
+                                                p(self.d_out_len), p(self.d_status), self.n, p(self.d_scratch),
+                                                self.d_scratch.numel(), stream)
         elif self.codec == "bzip2":
             st = L.swc_bzip2_decompress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out), p(self.d_out_off),
                                               p(self.d_out_cap), p(self.d_out_len), p(self.d_consumed), p(self.d_status), self.n, stream)

@@ -2,11 +2,15 @@
 // LZ4.decompress / LZ4.multiDecompress (reference Sources/LZ4/LZ4.swift:73-330).  Frame descriptors and block marks
 // are walked on the host (a few bytes per block); block decode, block checksums and the content checksum run on the
 // device.  Errors are reported in the order the reference's sequential loop would meet them.
+// The compress half (LZ4.compress, LZ4+Compress.swift:16-154) writes its frame the other way round: every block is
+// compressed on the device, the host lays out the frame from the compressed sizes, the device writes the payloads and
+// checksums in place, and the host adds the header, block marks and EndMark.
 #include <cstring>
 #include <vector>
 #include "../../include/swcgpu.h"
 #include "host_util.h"
 #include "lz4.cuh"
+#include "lz4_compress.cuh"
 #include "checks.cuh"
 
 using namespace swc;
@@ -417,6 +421,220 @@ int32_t swc_lz4_multi_decompress(const uint8_t *in, size_t in_len, const uint8_t
     for (size_t i = 0; i < ends.size(); i++) (*frame_ends)[i] = ends[i];
     *n_frames = ends.size();
     return result;
+}
+
+}  // extern "C"
+
+// ---- compression ----------------------------------------------------------------------------------------------------
+
+namespace {
+
+constexpr u64 kCompressPoolLimit = 16ull << 30;      // library-pool scratch per slice of a compress batch
+
+inline u64 window_of(u64 in_len, u64 dict_len) {
+    if (in_len > lz4c::MAX_BLOCK || (dict_len >= 1 && dict_len <= 3)) return 0;       // rejected units need no scratch
+    return in_len + (dict_len > lz4c::MAX_DICT ? lz4c::MAX_DICT : dict_len);
+}
+inline u64 need_of(u64 in_len, u64 dict_len) {
+    const u64 w = window_of(in_len, dict_len);
+    return lz4c::unit_scratch(w, w ? in_len : 0);
+}
+inline u64 meta_bytes(u64 count) { return (count * 8 + 255) & ~(u64)255; }
+
+inline void put32(uint8_t *p, uint32_t v) { p[0] = (uint8_t)v; p[1] = (uint8_t)(v >> 8); p[2] = (uint8_t)(v >> 16); p[3] = (uint8_t)(v >> 24); }
+
+}  // namespace
+
+extern "C" {
+
+size_t swc_lz4_compress_batch_scratch_bytes(uint64_t n, uint64_t window_bytes_total) {
+    // unit_scratch(w, l) <= 33 w / 8 + 795 for l <= w, plus 8 bytes of offsets per unit and the alignment of that table
+    return (size_t)(window_bytes_total / 8 * 33 + 33 + n * 1040 + 4096);
+}
+
+int32_t swc_lz4_block_compress_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                                     const uint64_t *dict_off, const uint64_t *dict_len,
+                                     uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                     uint64_t *out_len, int32_t *status, uint64_t n,
+                                     void *scratch, size_t scratch_bytes, void *cuda_stream) {
+    if (ensure_device()) return SWC_ERR_NO_DEVICE;
+    ApiLock api_lock;
+    if (n == 0) return SWC_OK;
+    if (!in_base || !in_off || !in_len || !out_base || !out_off || !out_cap || !out_len || !status) return SWC_ERR_INVALID_ARG;
+    if ((dict_off == nullptr) != (dict_len == nullptr)) return SWC_ERR_INVALID_ARG;
+    const cudaStream_t s = (cudaStream_t)cuda_stream;
+    // the scratch layout is planned on the host from the unit sizes (n x 16 bytes)
+    std::vector<uint64_t> lens(n), dlens(n, 0), offs(n);
+    SWC_CUDA_TRY(cudaMemcpyAsync(lens.data(), in_len, n * 8, cudaMemcpyDeviceToHost, s));
+    if (dict_len) SWC_CUDA_TRY(cudaMemcpyAsync(dlens.data(), dict_len, n * 8, cudaMemcpyDeviceToHost, s));
+    SWC_CUDA_TRY(cudaStreamSynchronize(s));
+    u64 total = meta_bytes(n), biggest = 0;
+    for (uint64_t i = 0; i < n; i++) {
+        const u64 need = need_of(lens[i], dlens[i]);
+        total += need;
+        if (need > biggest) biggest = need;
+    }
+    size_t cap = scratch_bytes;
+    if (!scratch) {
+        cap = (size_t)(total < kCompressPoolLimit ? total : kCompressPoolLimit);
+        if (cap < meta_bytes(1) + biggest) cap = (size_t)(meta_bytes(1) + biggest);
+        int st = scratch_get(cap, &scratch, s);
+        if (st) return st;
+    }
+    lz4c::Args a;
+    a.in_base = in_base; a.in_off = in_off; a.in_len = in_len; a.dict_off = dict_off; a.dict_len = dict_len;
+    a.out_base = out_base; a.out_off = out_off; a.out_cap = out_cap; a.out_len = out_len; a.status = status;
+    a.stored = nullptr; a.n = n;
+    u8 *scr = (u8 *)scratch;
+    // units go in slices whose scratch fits: a slice's table of offsets first, then each unit's region
+    for (uint64_t first = 0; first < n;) {
+        uint64_t count = 0;
+        u64 used = 0;
+        while (first + count < n) {
+            const u64 need = need_of(lens[first + count], dlens[first + count]);
+            if (meta_bytes(count + 1) + used + need > cap) break;
+            offs[first + count] = used;
+            used += need;
+            count++;
+        }
+        if (count == 0) return SWC_ERR_INVALID_ARG;                       // caller scratch smaller than one unit needs
+        const u64 mb = meta_bytes(count);
+        for (uint64_t j = 0; j < count; j++) offs[first + j] += mb;
+        SWC_CUDA_TRY(cudaMemcpyAsync(scr, offs.data() + first, count * 8, cudaMemcpyHostToDevice, s));
+        int st = lz4c::parse(a, first, count, scr, (const u64 *)scr, s);
+        if (!st) st = lz4c::emit(a, first, count, scr, (const u64 *)scr, s);
+        if (st) return st;
+        first += count;
+    }
+    return SWC_OK;
+}
+
+// LZ4.compress(data:independentBlocks:blockChecksums:contentChecksum:contentSize:blockSize:dictionary:dictionaryID:)
+// LZ4+Compress.swift:47-154
+int32_t swc_lz4_compress(const uint8_t *in, size_t in_len, int32_t independent_blocks, int32_t block_checksums,
+                         int32_t content_checksum, int32_t content_size, int64_t block_size,
+                         const uint8_t *dict, size_t dict_len, int32_t has_dict_id, uint32_t dict_id,
+                         uint8_t **out, size_t *out_len) {
+    if (!out || !out_len || (!in && in_len)) return SWC_ERR_INVALID_ARG;
+    *out = nullptr; *out_len = 0;
+    if (!(block_size <= (int64_t)lz4c::MAX_BLOCK && block_size > 0)) return SWC_ERR_REFERENCE_TRAP;     // :51
+    const u64 bs = (u64)block_size;
+    const u64 nb = (in_len + bs - 1) / bs;
+    const u64 D = dict ? (dict_len > lz4c::MAX_DICT ? lz4c::MAX_DICT : dict_len) : 0;                    // :95-101
+    // compress(block:_:) traps on a 1-3 byte dictionary (:283): the user's, or a short previous block (:106-110)
+    if (nb > 0 && D >= 1 && D <= 3) return SWC_ERR_REFERENCE_TRAP;
+    if (nb > 1 && !independent_blocks && bs <= 3) return SWC_ERR_REFERENCE_TRAP;
+    if (ensure_device()) return SWC_ERR_NO_DEVICE;
+    ApiLock api_lock;
+
+    uint8_t hdr[19];                                                                                     // :54-93
+    size_t h = 0;
+    hdr[h++] = 0x04; hdr[h++] = 0x22; hdr[h++] = 0x4D; hdr[h++] = 0x18;
+    hdr[h++] = (uint8_t)(0x40 | (independent_blocks ? 0x20 : 0) | (block_checksums ? 0x10 : 0) | (content_size ? 0x8 : 0) |
+                         (content_checksum ? 0x4 : 0) | (has_dict_id ? 0x1 : 0));
+    hdr[h++] = bs <= (64u << 10) ? 0x40 : bs <= (256u << 10) ? 0x50 : bs <= (1u << 20) ? 0x60 : 0x70;
+    if (content_size) for (int k = 0; k < 8; k++) hdr[h++] = (uint8_t)((uint64_t)in_len >> (8 * k));
+    if (has_dict_id) for (int k = 0; k < 4; k++) hdr[h++] = (uint8_t)(dict_id >> (8 * k));
+    hdr[h] = (uint8_t)((xxh32_descriptor(hdr + 4, h - 4) >> 8) & 0xFF);
+    h++;
+
+    int st;
+    // device input: the dictionary window, then the data
+    DevBuf d_in;
+    if ((st = d_in.alloc(D + in_len + 16))) return st;
+    if (D) SWC_CUDA_TRY(cudaMemcpy(d_in.p, dict + (dict_len - D), D, cudaMemcpyHostToDevice));
+    if (in_len) { int cst = copy_pageable(d_in.as<u8>() + D, in, in_len, true); if (cst) return cst; }
+
+    // per block: in_off, in_len, dict_off, dict_len, out_off, out_cap, then out_len, status, payload length, stored flag
+    std::vector<uint64_t> meta(nb * 6);
+    uint64_t *h_in_off = meta.data(), *h_in_len = h_in_off + nb, *h_doff = h_in_len + nb, *h_dlen = h_doff + nb;
+    uint64_t *h_out_off = h_dlen + nb, *h_out_cap = h_out_off + nb;
+    std::vector<uint64_t> scr_off(nb);
+    u64 scr_total = 0;
+    for (u64 k = 0; k < nb; k++) {
+        const u64 o = k * bs, l = in_len - o < bs ? in_len - o : bs;
+        h_in_off[k] = D + o; h_in_len[k] = l;
+        if (independent_blocks || k == 0) { h_doff[k] = 0; h_dlen[k] = D; }                               // :105
+        else { const u64 pl = bs < lz4c::MAX_DICT ? bs : lz4c::MAX_DICT; h_doff[k] = D + o - pl; h_dlen[k] = pl; }   // :106-110
+        h_out_off[k] = 0; h_out_cap[k] = ~0ull;
+        scr_off[k] = scr_total;
+        scr_total += need_of(l, h_dlen[k]);
+    }
+    DevBuf d_meta, d_scr;
+    const size_t mb = nb * 8;
+    if ((st = d_meta.alloc(mb * 10 + 64))) return st;
+    u8 *m = d_meta.as<u8>();
+    u64 *d_res_len = (u64 *)(m + 6 * mb), *d_scr_off = (u64 *)(m + 7 * mb);
+    int32_t *d_status = (int32_t *)(m + 8 * mb);
+    u8 *d_stored = m + 9 * mb;
+    u32 *d_ck = (u32 *)(m + 9 * mb + ((nb + 15) & ~(u64)15));
+    if ((st = d_scr.alloc(scr_total + 256))) return st;
+    std::vector<uint64_t> res_len(nb);
+    std::vector<int32_t> res_st(nb);
+    std::vector<uint8_t> stored(nb);
+    std::vector<uint32_t> cks(nb);
+    u64 frame_len = h;
+    std::vector<u64> pay_off(nb), pay_len(nb);
+    lz4c::Args a;
+    if (nb) {
+        SWC_CUDA_TRY(cudaMemcpy(m, meta.data(), 6 * mb, cudaMemcpyHostToDevice));
+        SWC_CUDA_TRY(cudaMemcpy(d_scr_off, scr_off.data(), mb, cudaMemcpyHostToDevice));
+        a.in_base = d_in.as<u8>(); a.in_off = (u64 *)m; a.in_len = (u64 *)(m + mb);
+        a.dict_off = (u64 *)(m + 2 * mb); a.dict_len = (u64 *)(m + 3 * mb);
+        a.out_base = nullptr; a.out_off = (u64 *)(m + 4 * mb); a.out_cap = (u64 *)(m + 5 * mb);
+        a.out_len = d_res_len; a.status = d_status; a.stored = nullptr; a.n = nb;
+        if ((st = lz4c::parse(a, 0, nb, d_scr.as<u8>(), d_scr_off, 0))) return st;
+        SWC_CUDA_TRY(cudaMemcpy(res_len.data(), d_res_len, mb, cudaMemcpyDeviceToHost));
+        SWC_CUDA_TRY(cudaMemcpy(res_st.data(), d_status, nb * 4, cudaMemcpyDeviceToHost));
+        for (u64 k = 0; k < nb; k++) {
+            if (res_st[k] != SWC_OK) return res_st[k];
+            stored[k] = res_len[k] > h_in_len[k];                                                        // :112
+            pay_len[k] = stored[k] ? h_in_len[k] : res_len[k];
+            pay_off[k] = frame_len + 4;
+            frame_len += 4 + pay_len[k] + (block_checksums ? 4 : 0);
+        }
+    }
+    const u64 payload_end = frame_len;
+    frame_len += 4 + (content_checksum ? 4 : 0);                                                         // :143-151
+    DevBuf d_frame;
+    if ((st = d_frame.alloc(frame_len + 16))) return st;
+    if (nb) {
+        // the payloads go straight to their frame offsets; out_cap keeps the parse's "unbounded" fence
+        memcpy(h_out_off, pay_off.data(), mb);
+        SWC_CUDA_TRY(cudaMemcpy(m + 4 * mb, h_out_off, mb, cudaMemcpyHostToDevice));
+        SWC_CUDA_TRY(cudaMemcpy(d_stored, stored.data(), nb, cudaMemcpyHostToDevice));
+        a.out_base = d_frame.as<u8>(); a.stored = d_stored;
+        if ((st = lz4c::emit(a, 0, nb, d_scr.as<u8>(), d_scr_off, 0))) return st;
+        if (block_checksums) {                                                                           // :120-125, :133-138
+            SWC_CUDA_TRY(cudaMemcpy(d_res_len, pay_len.data(), mb, cudaMemcpyHostToDevice));
+            if ((st = checks::xxh32_batch(d_frame.as<u8>(), a.out_off, d_res_len, d_ck, nb, 0))) return st;
+            SWC_CUDA_TRY(cudaMemcpy(cks.data(), d_ck, nb * 4, cudaMemcpyDeviceToHost));
+        }
+    }
+    uint32_t content_ck = xxh32_descriptor(nullptr, 0);
+    if (content_checksum && in_len) {                                                                    // :146-151
+        DevBuf d_res;
+        if ((st = d_res.alloc(16))) return st;
+        const u64 len64 = in_len;
+        SWC_CUDA_TRY(cudaMemcpy(d_res.p, &len64, 8, cudaMemcpyHostToDevice));
+        if ((st = checks::xxh32_batch(d_in.as<u8>() + D, nullptr, d_res.as<u64>(), (u32 *)(d_res.as<u8>() + 8), 1, 0))) return st;
+        SWC_CUDA_TRY(cudaMemcpy(&content_ck, d_res.as<u8>() + 8, 4, cudaMemcpyDeviceToHost));
+    }
+    uint8_t *host = (uint8_t *)swc_alloc(frame_len);
+    if (!host) return SWC_ERR_OUTPUT_OVERFLOW;
+    if (payload_end > h) {
+        int cst = copy_pageable(host + h, d_frame.as<u8>() + h, payload_end - h, false);
+        if (cst) { swc_free(host); return cst; }
+    }
+    memcpy(host, hdr, h);
+    for (u64 k = 0; k < nb; k++) {                                                                       // :113-139
+        put32(host + pay_off[k] - 4, (stored[k] ? 0x80000000u : 0u) | (uint32_t)pay_len[k]);
+        if (block_checksums) put32(host + pay_off[k] + pay_len[k], cks[k]);
+    }
+    put32(host + payload_end, 0);
+    if (content_checksum) put32(host + payload_end + 4, content_ck);
+    *out = host; *out_len = frame_len;
+    return SWC_OK;
 }
 
 }  // extern "C"

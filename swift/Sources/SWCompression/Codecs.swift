@@ -1,11 +1,13 @@
 // Public decode API of the reference, bodies routed through libswcgpu (include/swcgpu.h).
 //   DecompressionAlgorithm  Sources/Common/DecompressionAlgorithm.swift:9-14
 //   Archive                 Sources/Common/Archive.swift:9-14
+//   CompressionAlgorithm    Sources/Common/CompressionAlgorithm.swift (LZ4 is its only GPU-backed conformer here)
 import CSWCGPU
 import Foundation
 
 public protocol DecompressionAlgorithm { static func decompress(data: Data) throws -> Data }
 public protocol Archive { static func unarchive(archive: Data) throws -> Data }
+public protocol CompressionAlgorithm { static func compress(data: Data) -> Data }
 
 private let payloadCodes: Set<Int32> = [210, 503, 605, 705, 807]
 
@@ -95,7 +97,34 @@ public enum LZ4: DecompressionAlgorithm {                            // Sources/
             try multi(data) { p, n, o, ol, e, c in swc_lz4_multi_decompress(p, n, dp, dn, dictionaryID == nil ? 0 : 1, dictionaryID ?? 0, o, ol, e, c) }
         }
     }
-    private static func withDictionary<T>(_ d: Data?, _ body: (UnsafePointer<UInt8>?, Int) throws -> T) rethrows -> T {
+}
+
+extension LZ4: CompressionAlgorithm {                                // Sources/LZ4/LZ4+Compress.swift:8-154
+    public static func compress(data: Data) -> Data {
+        compress(data: data, independentBlocks: true, blockChecksums: false, contentChecksum: true, contentSize: false,
+                 blockSize: 4 * 1024 * 1024, dictionary: nil, dictionaryID: nil)
+    }
+    /// Non-throwing as in the reference: an engine status (a trap of the reference, no device, CUDA failure) stops the program.
+    public static func compress(data: Data, independentBlocks: Bool, blockChecksums: Bool, contentChecksum: Bool,
+                                contentSize: Bool, blockSize: Int = 4 * 1024 * 1024, dictionary: Data? = nil,
+                                dictionaryID: UInt32? = nil) -> Data {
+        var out: UnsafeMutablePointer<UInt8>? = nil
+        var outLen = 0
+        let status: Int32 = withDictionary(dictionary) { dp, dn in
+            data.withUnsafeBytes { raw in
+                swc_lz4_compress(raw.bindMemory(to: UInt8.self).baseAddress, raw.count, independentBlocks ? 1 : 0,
+                                 blockChecksums ? 1 : 0, contentChecksum ? 1 : 0, contentSize ? 1 : 0, Int64(blockSize),
+                                 dp, dn, dictionaryID == nil ? 0 : 1, dictionaryID ?? 0, &out, &outLen)
+            }
+        }
+        defer { swc_free(out) }
+        guard status == 0 else { fatalError("LZ4.compress: \(String(cString: swc_status_name(status)))") }
+        return out.map { Data(bytes: $0, count: outLen) } ?? Data()
+    }
+}
+
+extension LZ4 {
+    fileprivate static func withDictionary<T>(_ d: Data?, _ body: (UnsafePointer<UInt8>?, Int) throws -> T) rethrows -> T {
         guard let d = d else { return try body(nil, 0) }
         var one: UInt8 = 0     // a non-nil pointer distinguishes an EMPTY dictionary from `nil`
         return try d.withUnsafeBytes { raw in
