@@ -68,11 +68,13 @@ int bzip2_stream_by_blocks(const uint8_t *in, const u8 *d_in, size_t in_len, siz
     if (!have_end || pos.size() < 2 || pos[0] != (u64)(start + 4) * 8) return SWC_OK;
     const size_t nb = pos.size();
     const size_t cap = round16(level * 100000 * 2 + 65536);          // RLE1 can expand a block further: then the sequential path takes over
-    std::vector<u64> h(nb * 4);
-    std::vector<u8> h_sb(nb);
+    UnitTable t;
+    UnitCols c(t, nb);
+    const Col<u8> sb = t.in<u8>(nb);
     for (size_t k = 0; k < nb; k++) {
-        h[k] = pos[k] >> 3; h[nb + k] = in_len - (pos[k] >> 3); h[2 * nb + k] = k * cap; h[3 * nb + k] = cap;
-        h_sb[k] = (u8)(pos[k] & 7);
+        t.host(c.in_off)[k] = pos[k] >> 3; t.host(c.in_len)[k] = in_len - (pos[k] >> 3);
+        t.host(c.out_off)[k] = k * cap; t.host(c.out_cap)[k] = cap;
+        t.host(sb)[k] = (u8)(pos[k] & 7);
     }
     // the block-parallel attempt needs nb x (cap + ~6 x cap of scratch); when that does not fit, the sequential decoder (which
     // holds one block at a time) takes over instead of failing the call
@@ -82,14 +84,10 @@ int bzip2_stream_by_blocks(const uint8_t *in, const u8 *d_in, size_t in_len, siz
         const size_t need = nb * (cap + bzip2::scratch_per_unit(cap)) + ((size_t)64 << 20);
         if (need > free_b / 2) return SWC_OK;
     }
-    DevBuf d_out, d_meta;
+    DevBuf d_out;
     if (d_out.alloc(nb * cap + 64)) return SWC_OK;
-    if (d_meta.alloc(nb * 8 * 7 + nb * 4 + nb + 64)) return SWC_OK;
-    u64 *m = d_meta.as<u64>();
-    int32_t *d_status = (int32_t *)(m + 7 * nb);
-    u8 *d_sb = (u8 *)(d_status + nb);
-    SWC_CUDA_TRY(cudaMemcpy(m, h.data(), nb * 32, cudaMemcpyHostToDevice));
-    SWC_CUDA_TRY(cudaMemcpy(d_sb, h_sb.data(), nb, cudaMemcpyHostToDevice));
+    if (t.alloc()) return SWC_OK;
+    if ((st = t.upload())) return st;
     {
         size_t total = (nb * 8 + 255) & ~(size_t)255;
         std::vector<u64> soff(nb);
@@ -98,21 +96,21 @@ int bzip2_stream_by_blocks(const uint8_t *in, const u8 *d_in, size_t in_len, siz
         if (scratch_get(total, &scratch, 0)) return SWC_OK;
         SWC_CUDA_TRY(cudaMemcpy(scratch, soff.data(), nb * 8, cudaMemcpyHostToDevice));
         bzip2::Args a;
-        a.in_base = d_in; a.in_off = m; a.in_len = m + nb;
-        a.out_base = d_out.as<u8>(); a.out_off = m + 2 * nb; a.out_cap = m + 3 * nb;
-        a.out_len = m + 4 * nb; a.consumed_bits = m + 5 * nb; a.status = d_status; a.n = nb;
+        a.in_base = d_in; a.in_off = t.dev(c.in_off); a.in_len = t.dev(c.in_len);
+        a.out_base = d_out.as<u8>(); a.out_off = t.dev(c.out_off); a.out_cap = t.dev(c.out_cap);
+        a.out_len = t.dev(c.out_len); a.consumed_bits = t.dev(c.consumed); a.status = t.dev(c.status); a.n = nb;
         a.scratch = (u8 *)scratch; a.scr_off = (const u64 *)scratch;
-        a.start_bits = d_sb; a.block_mode = 1;
+        a.start_bits = t.dev(sb); a.block_mode = 1;
         if ((st = bzip2::launch(a, 0))) return st;
     }
-    std::vector<u64> r_len(nb), r_used(nb);
-    std::vector<int32_t> r_st(nb);
-    SWC_CUDA_TRY(cudaMemcpy(r_len.data(), m + 4 * nb, nb * 8, cudaMemcpyDeviceToHost));
-    SWC_CUDA_TRY(cudaMemcpy(r_used.data(), m + 5 * nb, nb * 8, cudaMemcpyDeviceToHost));
-    SWC_CUDA_TRY(cudaMemcpy(r_st.data(), d_status, nb * 4, cudaMemcpyDeviceToHost));
+    std::vector<u64> r_len, r_used;
+    std::vector<int32_t> r_st;
+    if ((st = t.fetch(c.out_len, r_len)) || (st = t.fetch(c.consumed, r_used)) || (st = t.fetch(c.status, r_st))) return st;
     // the in-order walk: every block must end where the next magic starts, the last one at the end-of-stream magic
     uint32_t total_crc = 0;
-    std::vector<u64> g_dst(nb);
+    UnitTable g;
+    const Col<u64> dst = g.in<u64>(nb);
+    u64 *g_dst = g.host(dst);
     u64 out_total = 0;
     for (size_t k = 0; k < nb; k++) {
         const u64 ends_at = (pos[k] & ~7ull) + r_used[k];            // consumed is counted from the unit's first byte
@@ -127,10 +125,8 @@ int bzip2_stream_by_blocks(const uint8_t *in, const u8 *d_in, size_t in_len, siz
     if (bits32_at(in, in_len, end_pos + 48) != total_crc) return SWC_OK;   // the sequential path reports wrongCRC with its payload
     // contiguous result
     if ((st = r.out.alloc(round16((size_t)out_total) + 64))) return st;
-    DevBuf d_g;
-    if ((st = d_g.alloc(nb * 8 + 64))) return st;
-    SWC_CUDA_TRY(cudaMemcpy(d_g.p, g_dst.data(), nb * 8, cudaMemcpyHostToDevice));
-    if ((st = checks::gather_units(d_out.as<u8>(), m + 2 * nb, m + 4 * nb, r.out.as<u8>(), d_g.as<u64>(), nb, 0))) return st;
+    if ((st = g.alloc()) || (st = g.upload())) return st;
+    if ((st = checks::gather_units(d_out.as<u8>(), t.dev(c.out_off), t.dev(c.out_len), r.out.as<u8>(), g.dev(dst), nb, 0))) return st;
     SWC_CUDA_TRY(cudaStreamSynchronize(0));
     r.out_len = (size_t)out_total;
     r.consumed = (size_t)(end_pos + 80 - (u64)start * 8);
@@ -148,35 +144,14 @@ int bzip2_unit_device(const u8 *d_in, size_t in_len, size_t start, UnitResult &r
         if (bst) return bst;
         if (done) return SWC_OK;
     }
-    size_t cap = (in_len - start) * 16 + (1u << 20);
-    DevBuf meta;
-    int st = meta.alloc(256);
-    if (st) return st;
-    for (int attempt = 0; attempt < 8; attempt++) {
-        cap = round16(cap);
-        if ((st = r.out.alloc(cap))) return st;
-        u64 h[6] = {start, in_len - start, 0, cap, 0, 0};
-        SWC_CUDA_TRY(cudaMemcpy(meta.p, h, sizeof(h), cudaMemcpyHostToDevice));
-        u64 *m = meta.as<u64>();
-        if ((st = bzip2_batch_impl(d_in, m + 0, m + 1, r.out.as<u8>(), m + 2, m + 3, m + 4, m + 5, (int32_t *)((u8 *)meta.p + 48), 1, 0))) return st;
-        SWC_CUDA_TRY(cudaStreamSynchronize(0));
-        u64 res[7];
-        SWC_CUDA_TRY(cudaMemcpy(res, meta.p, 56, cudaMemcpyDeviceToHost));
-        r.out_len = (size_t)res[4];
-        r.consumed = (size_t)res[5];
-        int32_t st32; memcpy(&st32, &res[6], 4);
-        r.status = st32;
-        if (r.status != SWC_ERR_OUTPUT_OVERFLOW || cap >= ((size_t)1 << 32)) break;
-        cap *= 4;                     // BZip2 cannot report the final size before it has decoded everything
-    }
-    return SWC_OK;
-}
-
-int upload(DevBuf &d, const uint8_t *in, size_t n) {
-    int st = d.alloc(round16(n) + 256);
-    if (st) return st;
-    { int cst = copy_pageable(d.p, in, n, true); if (cst) return cst; }
-    return SWC_OK;
+    UnitTable t;
+    UnitCols c(t, 1);
+    // BZip2 cannot report the final size before it has decoded everything: x4 per attempt
+    return decode_unit(t, c, start, in_len, (in_len - start) * 16 + (1u << 20), 8,
+                       [](size_t cap, size_t) { return cap >= ((size_t)1 << 32) ? 0 : cap * 4; }, [&](u8 *out, size_t) {
+        return bzip2_batch_impl(d_in, t.dev(c.in_off), t.dev(c.in_len), out, t.dev(c.out_off), t.dev(c.out_cap), t.dev(c.out_len),
+                                t.dev(c.consumed), t.dev(c.status), 1, 0);
+    }, r);
 }
 
 }  // namespace
@@ -202,7 +177,7 @@ int32_t swc_bzip2_decompress(const uint8_t *in, size_t in_len, size_t start_bit,
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
     DevBuf d_in;
-    int st = upload(d_in, in, in_len);
+    int st = upload_input(d_in, in, in_len);
     if (st) return st;
     UnitResult r;
     if ((st = bzip2_unit_device(d_in.as<u8>(), in_len, start_bit >> 3, r, in))) return st;
@@ -220,9 +195,9 @@ int32_t swc_bzip2_multi_decompress(const uint8_t *in, size_t in_len,
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
     DevBuf d_in;
-    int st = upload(d_in, in, in_len);
+    int st = upload_input(d_in, in, in_len);
     if (st) return st;
-    std::vector<uint8_t> o;
+    HostOut o;
     std::vector<size_t> ends;
     size_t off = 0;
     int result = SWC_OK;
@@ -241,45 +216,45 @@ int32_t swc_bzip2_multi_decompress(const uint8_t *in, size_t in_len,
         }
         if (cand.size() >= 2 && cand[0] == 0) {
             const size_t n = cand.size();
-            std::vector<uint64_t> h_off(n), h_len(n), h_ooff(n), h_cap(n), r_len(n), r_used(n);
-            std::vector<int32_t> r_st(n);
+            auto len_of = [&](size_t k) { return (k + 1 < n ? cand[k + 1] : in_len) - cand[k]; };
+            auto cap_of = [&](size_t k) { return round16(len_of(k) * 12 + (1u << 20)); };
             // groups bounded by a scratch budget (the BWT working set is ~6x the output capacity of a unit)
             const size_t budget = (size_t)24 << 30;
             size_t k0 = 0;
             bool handed_over = false;
             while (k0 < n && !handed_over) {
-                size_t k1 = k0, need = 0, out_total = 0;
+                size_t k1 = k0, need = 0;
                 while (k1 < n) {
-                    const size_t len = (k1 + 1 < n ? cand[k1 + 1] : in_len) - cand[k1];
-                    const size_t cap = round16(len * 12 + (1u << 20));
-                    const size_t add = bzip2::scratch_per_unit(cap) + cap;
+                    const size_t add = bzip2::scratch_per_unit(cap_of(k1)) + cap_of(k1);
                     if (k1 > k0 && need + add > budget) break;
-                    h_off[k1] = cand[k1]; h_len[k1] = len; h_ooff[k1] = out_total; h_cap[k1] = cap;
-                    need += add; out_total += cap; k1++;
+                    need += add; k1++;
                 }
                 const size_t g = k1 - k0;
-                DevBuf d_out, d_meta;
+                UnitTable t;
+                UnitCols c(t, g);
+                u64 *h_len = t.host(c.in_len), *h_ooff = t.host(c.out_off);
+                size_t out_total = 0;
+                for (size_t j = 0; j < g; j++) {
+                    t.host(c.in_off)[j] = cand[k0 + j]; h_len[j] = len_of(k0 + j);
+                    h_ooff[j] = out_total; t.host(c.out_cap)[j] = cap_of(k0 + j);
+                    out_total += cap_of(k0 + j);
+                }
+                DevBuf d_out;
                 if ((st = d_out.alloc(out_total + 64))) return st;
-                if ((st = d_meta.alloc(g * 8 * 6 + g * 4 + 64))) return st;
-                u64 *m = d_meta.as<u64>();
-                SWC_CUDA_TRY(cudaMemcpy(m + 0 * g, h_off.data() + k0, g * 8, cudaMemcpyHostToDevice));
-                SWC_CUDA_TRY(cudaMemcpy(m + 1 * g, h_len.data() + k0, g * 8, cudaMemcpyHostToDevice));
-                SWC_CUDA_TRY(cudaMemcpy(m + 2 * g, h_ooff.data() + k0, g * 8, cudaMemcpyHostToDevice));
-                SWC_CUDA_TRY(cudaMemcpy(m + 3 * g, h_cap.data() + k0, g * 8, cudaMemcpyHostToDevice));
-                if ((st = bzip2_batch_impl(d_in.as<u8>(), m + 0 * g, m + 1 * g, d_out.as<u8>(), m + 2 * g, m + 3 * g, m + 4 * g, m + 5 * g,
-                                           (int32_t *)(m + 6 * g), g, 0))) return st;
-                SWC_CUDA_TRY(cudaStreamSynchronize(0));
-                SWC_CUDA_TRY(cudaMemcpy(r_len.data() + k0, m + 4 * g, g * 8, cudaMemcpyDeviceToHost));
-                SWC_CUDA_TRY(cudaMemcpy(r_used.data() + k0, m + 5 * g, g * 8, cudaMemcpyDeviceToHost));
-                SWC_CUDA_TRY(cudaMemcpy(r_st.data() + k0, m + 6 * g, g * 4, cudaMemcpyDeviceToHost));
-                for (size_t k = k0; k < k1; k++) {
-                    const bool ok = r_st[k] == SWC_OK && (r_used[k] + 7) / 8 == h_len[k];
-                    if (!ok) { off = cand[k]; handed_over = true; break; }        // sequential loop re-decodes this stream
-                    const size_t base = o.size();
-                    o.resize(base + r_len[k]);
-                    if (r_len[k]) SWC_CUDA_TRY(cudaMemcpy(o.data() + base, d_out.as<u8>() + h_ooff[k], r_len[k], cudaMemcpyDeviceToHost));
-                    ends.push_back(o.size());
-                    off = cand[k] + h_len[k];
+                if ((st = t.alloc()) || (st = t.upload())) return st;
+                if ((st = bzip2_batch_impl(d_in.as<u8>(), t.dev(c.in_off), t.dev(c.in_len), d_out.as<u8>(), t.dev(c.out_off), t.dev(c.out_cap),
+                                           t.dev(c.out_len), t.dev(c.consumed), t.dev(c.status), g, 0))) return st;
+                std::vector<u64> r_len, r_used;
+                std::vector<int32_t> r_st;
+                if ((st = t.fetch(c.out_len, r_len)) || (st = t.fetch(c.consumed, r_used)) || (st = t.fetch(c.status, r_st))) return st;
+                for (size_t j = 0; j < g; j++) {
+                    const bool ok = r_st[j] == SWC_OK && (r_used[j] + 7) / 8 == h_len[j];
+                    if (!ok) { off = cand[k0 + j]; handed_over = true; break; }   // sequential loop re-decodes this stream
+                    uint8_t *dst = o.grow(r_len[j]);
+                    if (!dst) return SWC_ERR_OUTPUT_OVERFLOW;
+                    if (r_len[j]) SWC_CUDA_TRY(cudaMemcpy(dst, d_out.as<u8>() + h_ooff[j], r_len[j], cudaMemcpyDeviceToHost));
+                    ends.push_back(o.len);
+                    off = cand[k0 + j] + h_len[j];
                 }
                 k0 = k1;
             }
@@ -289,20 +264,15 @@ int32_t swc_bzip2_multi_decompress(const uint8_t *in, size_t in_len,
         UnitResult r;
         if ((st = bzip2_unit_device(d_in.as<u8>(), in_len, off, r, in))) return st;
         if (r.status != SWC_OK && r.status != SWC_BZIP2_WRONG_CRC) return r.status;
-        size_t base = o.size();
-        if (r.status == SWC_BZIP2_WRONG_CRC) { o.clear(); ends.clear(); base = 0; }   // payload = the failing archive only
-        o.resize(base + r.out_len);
-        if (r.out_len) SWC_CUDA_TRY(cudaMemcpy(o.data() + base, r.out.p, r.out_len, cudaMemcpyDeviceToHost));
-        ends.push_back(o.size());
+        if (r.status == SWC_BZIP2_WRONG_CRC) { o.len = 0; ends.clear(); }   // payload = the failing archive only
+        uint8_t *dst = o.grow(r.out_len);
+        if (!dst) return SWC_ERR_OUTPUT_OVERFLOW;
+        if (r.out_len) SWC_CUDA_TRY(cudaMemcpy(dst, r.out.p, r.out_len, cudaMemcpyDeviceToHost));
+        ends.push_back(o.len);
         if (r.status) { result = r.status; break; }
         off += (r.consumed + 7) / 8;                     // reader.align()
     }
-    uint8_t *h = (uint8_t *)swc_alloc(o.size());
-    if (!h) return SWC_ERR_OUTPUT_OVERFLOW;
-    if (!o.empty()) memcpy(h, o.data(), o.size());
-    *out = h; *out_len = o.size();
-    *stream_ends = (size_t *)swc_alloc(sizeof(size_t) * (ends.size() + 1));
-    for (size_t i = 0; i < ends.size(); i++) (*stream_ends)[i] = ends[i];
+    if ((st = o.release_to(out, out_len)) || (st = give_sizes(ends, stream_ends, out, out_len))) return st;
     *n_streams = ends.size();
     return result;
 }

@@ -7,18 +7,6 @@
 
 namespace swc {
 
-int to_host_alloc(const void *d, size_t n, uint8_t **out, size_t *out_len) {
-    uint8_t *h = (uint8_t *)swc_alloc(n);
-    if (!h) return SWC_ERR_OUTPUT_OVERFLOW;
-    if (n) {
-        int st = copy_pageable(h, d, n, false);
-        if (st) { swc_free(h); return st; }
-    }
-    *out = h;
-    *out_len = n;
-    return SWC_OK;
-}
-
 int deflate_batch_impl(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, const uint8_t *start_bits,
                               uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t out_total,
                               uint64_t *out_len, uint64_t *consumed_bits, int32_t *status, uint64_t n,
@@ -37,42 +25,24 @@ int deflate_batch_impl(const uint8_t *in_base, const uint64_t *in_off, const uin
     a.in_base = in_base; a.in_off = in_off; a.in_len = in_len; a.start_bits = start_bits;
     a.out_base = out_base; a.out_off = out_off; a.out_cap = out_cap;
     a.out_len = out_len; a.consumed_bits = consumed_bits; a.status = status; a.n = n;
-    a.ticket = (unsigned long long *)scratch;                       // 8 bytes (256 reserved)
-    a.rec_count = (u32 *)((u8 *)scratch + 256);                     // n entries
-    a.rec_base = (u32 *)((u8 *)scratch + 256 + ((n * 4 + 255) & ~(size_t)255));
+    inflate::seat_scratch(a, scratch, n, 0, 1, 0);
     return inflate::launch(a, stream);
 }
 
-// Decode one Deflate stream that already sits on the device; grows the output buffer until it fits.
+// Decode one Deflate stream that already sits on the device; retries once more at the exact size the counting pass reports.
 int deflate_unit_device(const u8 *d_in, size_t in_len, size_t start_bit_abs, UnitResult &r, size_t hint) {
     size_t start_byte = start_bit_abs >> 3;
     if (start_byte > in_len) start_byte = in_len;
-    u8 sb = (u8)(start_bit_abs & 7);
-    size_t cap = hint ? hint : (in_len - start_byte) * 4 + 65536;
-    DevBuf meta;
-    int st = meta.alloc(256);
+    UnitTable t;
+    UnitCols c(t, 1);
+    const Col<u8> sb = t.in<u8>(1);
+    *t.host(sb) = (u8)(start_bit_abs & 7);
+    const size_t first_cap = hint ? hint : (in_len - start_byte) * 4 + 65536;
+    int st = decode_unit(t, c, start_byte, in_len, first_cap, 3, [](size_t, size_t need) { return need; }, [&](u8 *out, size_t cap) {
+        return deflate_batch_impl(d_in, t.dev(c.in_off), t.dev(c.in_len), t.dev(sb), out, t.dev(c.out_off), t.dev(c.out_cap), cap,
+                                  t.dev(c.out_len), t.dev(c.consumed), t.dev(c.status), 1, nullptr, 0, 0);
+    }, r);
     if (st) return st;
-    for (int attempt = 0; attempt < 3; attempt++) {
-        cap = round16(cap);
-        if ((st = r.out.alloc(cap))) return st;
-        // meta layout: in_off, in_len, out_off, out_cap, out_len, consumed (u64 each) | status (i32) | start_bits (u8)
-        u64 h[6] = {start_byte, in_len - start_byte, 0, cap, 0, 0};
-        SWC_CUDA_TRY(cudaMemcpy(meta.p, h, sizeof(h), cudaMemcpyHostToDevice));
-        SWC_CUDA_TRY(cudaMemcpy((u8 *)meta.p + 64, &sb, 1, cudaMemcpyHostToDevice));
-        u64 *m = meta.as<u64>();
-        st = deflate_batch_impl(d_in, m + 0, m + 1, (u8 *)meta.p + 64, r.out.as<u8>(), m + 2, m + 3, cap, m + 4, m + 5,
-                                (int32_t *)((u8 *)meta.p + 48), 1, nullptr, 0, 0);
-        if (st) return st;
-        SWC_CUDA_TRY(cudaStreamSynchronize(0));
-        u64 res[7];
-        SWC_CUDA_TRY(cudaMemcpy(res, meta.p, 56, cudaMemcpyDeviceToHost));
-        r.out_len = (size_t)res[4];
-        r.consumed = (size_t)res[5];
-        int32_t st32; memcpy(&st32, &res[6], 4);
-        r.status = st32;
-        if (r.status != SWC_ERR_OUTPUT_OVERFLOW) break;
-        cap = r.out_len;          // exact size reported by the counting pass
-    }
     if (r.status == SWC_INTERNAL_NEEDS_SLOW) r.status = SWC_ERR_UNSUPPORTED;
     return SWC_OK;
 }
@@ -118,28 +88,28 @@ int32_t swc_deflate_decompress_batch_host(const uint8_t *in_base, const uint64_t
         SWC_CUDA_TRY(cudaEventCreateWithFlags(&ctx.tables_ready, cudaEventDisableTiming));
     }
     cudaEvent_t tables_ready = ctx.tables_ready;
-    // every unit must lie inside the two arenas (checked for ALL units, without overflowing sums); slices additionally need
-    // monotone offsets so that a slice is one contiguous byte range on both sides
+    // slices additionally need monotone offsets so that a slice is one contiguous byte range on both sides
     bool monotone = true;
-    for (uint64_t i = 0; i < n; i++) {
-        if (in_off[i] > in_total || in_len[i] > in_total - in_off[i] || out_off[i] > out_total || out_cap[i] > out_total - out_off[i])
-            return SWC_ERR_INVALID_ARG;
-        if (out_off[i] & 15) return SWC_ERR_INVALID_ARG;
-        if (i && (in_off[i] < in_off[i - 1] + in_len[i - 1] || out_off[i] < out_off[i - 1] + out_cap[i - 1])) monotone = false;
-    }
+    int st = check_host_units(in_off, in_len, in_total, out_off, out_cap, out_total, n, &monotone);
+    if (st) return st;
     static const int s_env = [] { const char *e = getenv("SWC_HOST_SLICES"); return e ? atoi(e) : 0; }();
     // slice count: ~2048 units per slice keeps the warp-per-unit decoder's grid full while the first device->host copy can
     // start after 1/32 of the batch
     uint64_t S = 1;
     if (monotone && n >= 4096) { S = s_env > 0 ? (uint64_t)s_env : n / 2048; if (S > 32) S = 32; if (S > 64) S = 64; }
+    // the unit table lives in an arena; its columns are filled straight from the caller's arrays
+    UnitTable t;
+    const Col<u64> d_in_off = t.out<u64>(n), d_in_len = t.out<u64>(n), d_out_off = t.out<u64>(n), d_out_cap = t.out<u64>(n);
+    const Col<u64> d_out_len = t.out<u64>(n), d_cons = t.out<u64>(n);
+    const Col<int32_t> d_status = t.out<int32_t>(n);
     void *p_in = nullptr, *p_out = nullptr, *p_meta = nullptr, *p_scr = nullptr;
-    int st;
     const size_t tb = n * 8;
-    const size_t hdr = 256 * 64 + ((n * 4 + 255) & ~(size_t)255);      // up to 64 slices, one ticket block each
+    const int tickets = 64;                                              // up to 64 slices, one ticket block each
     if ((st = arena_get(1, round16(in_total) + 64, &p_in, 0))) return st;
     if ((st = arena_get(2, round16(out_total) + 64, &p_out, 0))) return st;
-    if ((st = arena_get(3, tb * 6 + n * 4 + 256, &p_meta, 0))) return st;
-    if ((st = arena_get(0, hdr + (out_total / 3 + 2) * 4 + 256, &p_scr, 0))) return st;
+    if ((st = arena_get(3, t.bytes(), &p_meta, 0))) return st;
+    if ((st = arena_get(0, inflate::scratch_header(n, tickets) + (out_total / 3 + 2) * 4 + 256, &p_scr, 0))) return st;
+    t.place(p_meta);
     // result tables come back through a library-owned pinned buffer: a D2H into pageable caller memory would block the
     // host thread inside the slice loop and serialise the whole pipeline
     const size_t res_bytes = n * 20;
@@ -152,14 +122,10 @@ int32_t swc_deflate_decompress_batch_host(const uint8_t *in_base, const uint64_t
     u8 *h_res = ctx.h_res;
     u64 *h_out_len = (u64 *)h_res, *h_cons = h_out_len + n;
     int32_t *h_status = (int32_t *)(h_cons + n);
-    u8 *m = (u8 *)p_meta;
-    u64 *d_in_off = (u64 *)(m + 0 * tb), *d_in_len = (u64 *)(m + 1 * tb), *d_out_off = (u64 *)(m + 2 * tb), *d_out_cap = (u64 *)(m + 3 * tb);
-    u64 *d_out_len = (u64 *)(m + 4 * tb), *d_cons = (u64 *)(m + 5 * tb);
-    int32_t *d_status = (int32_t *)(m + 6 * tb);
-    SWC_CUDA_TRY(cudaMemcpyAsync(d_in_off, in_off, tb, cudaMemcpyHostToDevice, streams[0]));
-    SWC_CUDA_TRY(cudaMemcpyAsync(d_in_len, in_len, tb, cudaMemcpyHostToDevice, streams[0]));
-    SWC_CUDA_TRY(cudaMemcpyAsync(d_out_off, out_off, tb, cudaMemcpyHostToDevice, streams[0]));
-    SWC_CUDA_TRY(cudaMemcpyAsync(d_out_cap, out_cap, tb, cudaMemcpyHostToDevice, streams[0]));
+    SWC_CUDA_TRY(cudaMemcpyAsync(t.dev(d_in_off), in_off, tb, cudaMemcpyHostToDevice, streams[0]));
+    SWC_CUDA_TRY(cudaMemcpyAsync(t.dev(d_in_len), in_len, tb, cudaMemcpyHostToDevice, streams[0]));
+    SWC_CUDA_TRY(cudaMemcpyAsync(t.dev(d_out_off), out_off, tb, cudaMemcpyHostToDevice, streams[0]));
+    SWC_CUDA_TRY(cudaMemcpyAsync(t.dev(d_out_cap), out_cap, tb, cudaMemcpyHostToDevice, streams[0]));
     SWC_CUDA_TRY(cudaEventRecord(tables_ready, streams[0]));
     for (uint64_t k = 0; k < S; k++) {
         const uint64_t b = n * k / S, e = n * (k + 1) / S;
@@ -169,24 +135,15 @@ int32_t swc_deflate_decompress_batch_host(const uint8_t *in_base, const uint64_t
         const uint64_t i0 = S == 1 ? 0 : in_off[b], i1 = S == 1 ? in_total : in_off[e - 1] + in_len[e - 1];
         SWC_CUDA_TRY(cudaMemcpyAsync((u8 *)p_in + i0, in_base + i0, i1 - i0, cudaMemcpyHostToDevice, s));
         inflate::BatchArgs a;
-        a.in_base = (const u8 *)p_in; a.in_off = d_in_off + b; a.in_len = d_in_len + b; a.start_bits = nullptr;
-        a.out_base = (u8 *)p_out; a.out_off = d_out_off + b; a.out_cap = d_out_cap + b;
-        a.out_len = d_out_len + b; a.consumed_bits = d_cons + b; a.status = d_status + b; a.n = e - b;
-        a.ticket = (unsigned long long *)((u8 *)p_scr + 256 * k);
-        a.rec_count = (u32 *)((u8 *)p_scr + 256 * 64) + b;
-        a.rec_base = (u32 *)((u8 *)p_scr + hdr);
+        a.in_base = (const u8 *)p_in; a.in_off = t.dev(d_in_off) + b; a.in_len = t.dev(d_in_len) + b; a.start_bits = nullptr;
+        a.out_base = (u8 *)p_out; a.out_off = t.dev(d_out_off) + b; a.out_cap = t.dev(d_out_cap) + b;
+        a.out_len = t.dev(d_out_len) + b; a.consumed_bits = t.dev(d_cons) + b; a.status = t.dev(d_status) + b; a.n = e - b;
+        inflate::seat_scratch(a, p_scr, n, b, tickets, (int)k);
         if ((st = inflate::launch(a, s))) return st;
-        // only the output regions come back: the caller's bytes between and around them are not ours to overwrite
-        // (regions that touch are merged, so a densely packed slice is still one copy)
-        for (uint64_t i = b; i < e;) {
-            const uint64_t r0 = out_off[i];
-            uint64_t r1 = r0 + out_cap[i++];
-            while (i < e && out_off[i] == r1) r1 += out_cap[i++];
-            if (r1 > r0) SWC_CUDA_TRY(cudaMemcpyAsync(out_base + r0, (u8 *)p_out + r0, r1 - r0, cudaMemcpyDeviceToHost, s));
-        }
-        SWC_CUDA_TRY(cudaMemcpyAsync(h_out_len + b, d_out_len + b, (e - b) * 8, cudaMemcpyDeviceToHost, s));
-        SWC_CUDA_TRY(cudaMemcpyAsync(h_cons + b, d_cons + b, (e - b) * 8, cudaMemcpyDeviceToHost, s));
-        SWC_CUDA_TRY(cudaMemcpyAsync(h_status + b, d_status + b, (e - b) * 4, cudaMemcpyDeviceToHost, s));
+        if ((st = copy_back_regions(out_base, (const u8 *)p_out, out_off, out_cap, b, e, s))) return st;
+        SWC_CUDA_TRY(cudaMemcpyAsync(h_out_len + b, t.dev(d_out_len) + b, (e - b) * 8, cudaMemcpyDeviceToHost, s));
+        SWC_CUDA_TRY(cudaMemcpyAsync(h_cons + b, t.dev(d_cons) + b, (e - b) * 8, cudaMemcpyDeviceToHost, s));
+        SWC_CUDA_TRY(cudaMemcpyAsync(h_status + b, t.dev(d_status) + b, (e - b) * 4, cudaMemcpyDeviceToHost, s));
     }
     for (int i = 0; i < 3; i++) SWC_CUDA_TRY(cudaStreamSynchronize(streams[i]));
     memcpy(out_len, h_out_len, n * 8);
@@ -203,9 +160,8 @@ int32_t swc_deflate_decompress(const uint8_t *in, size_t in_len, size_t start_bi
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
     DevBuf d_in;
-    int st = d_in.alloc(round16(in_len) + 16);
+    int st = upload_input(d_in, in, in_len);
     if (st) return st;
-    { int cst = copy_pageable(d_in.p, in, in_len, true); if (cst) return cst; }
     UnitResult r;
     if ((st = deflate_unit_device(d_in.as<u8>(), in_len, start_bit, r))) return st;
     if (consumed_bits) *consumed_bits = r.consumed;

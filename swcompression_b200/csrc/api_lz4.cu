@@ -17,8 +17,7 @@ using namespace swc;
 
 namespace {
 
-inline uint32_t rd32(const uint8_t *p) { return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24; }
-inline uint64_t rd64(const uint8_t *p) { return (uint64_t)rd32(p) | (uint64_t)rd32(p + 4) << 32; }
+inline uint64_t rd64(const uint8_t *p) { return (uint64_t)le32(p) | (uint64_t)le32(p + 4) << 32; }
 inline bool is_magic(uint32_t v) { return v == 0x184D2204u || v == 0x184C2102u || (v >= 0x184D2A50u && v <= 0x184D2A5Fu); }
 
 // xxHash32 of the <= 14-byte frame descriptor (framing, not payload) — XxHash32.swift:24-83 with n < 16
@@ -26,7 +25,7 @@ uint32_t xxh32_descriptor(const uint8_t *p, size_t n) {
     auto rotl = [](uint32_t v, int s) { return (v << s) | (v >> (32 - s)); };
     uint32_t acc = 0x165667B1u + (uint32_t)n;
     size_t i = 0;
-    for (; n - i >= 4; i += 4) acc = rotl(acc + rd32(p + i) * 0xC2B2AE3Du, 17) * 0x27D4EB2Fu;
+    for (; n - i >= 4; i += 4) acc = rotl(acc + le32(p + i) * 0xC2B2AE3Du, 17) * 0x27D4EB2Fu;
     for (; n - i >= 1; i += 1) acc = rotl(acc + (uint32_t)p[i] * 0x165667B1u, 11) * 0x9E3779B1u;
     acc ^= acc >> 15; acc *= 0x85EBCA77u; acc ^= acc >> 13; acc *= 0xC2B2AE3Du; acc ^= acc >> 16;
     return acc;
@@ -44,14 +43,21 @@ struct DeviceInput {      // compressed input + optional dictionary, resident on
 // mode: 0 = every block is its own unit (independent / legacy), 1 = one chain (dependent blocks).
 // `pending_error` is the framing error the host scan stopped at (0 if it reached the EndMark).
 int run_blocks(DeviceInput &dev, const std::vector<Block> &blocks, int mode, bool use_dict, size_t max_block,
-               bool check_blocks, int pending_error, std::vector<uint8_t> &host_out, DevBuf &d_out_keep, size_t &d_out_len) {
+               bool check_blocks, int pending_error, HostOut &host_out, DevBuf &d_out_keep, size_t &d_out_len) {
     const size_t nb = blocks.size();
     d_out_len = 0;
     if (nb == 0) return pending_error;
     const size_t nunits = mode == 0 ? nb : 1;
-    std::vector<uint64_t> h_off(nb), h_len(nb), u_off(nunits), u_cap(nunits);
-    std::vector<uint32_t> h_first(nunits), h_cnt(nunits);
-    for (size_t i = 0; i < nb; i++) { h_off[i] = blocks[i].off; h_len[i] = blocks[i].len | (blocks[i].stored ? 1ull << 63 : 0); }
+    // block columns, then unit columns (a unit is one block, or the whole chain of a dependent frame)
+    UnitTable t;
+    const Col<u64> blk_off = t.in<u64>(nb), blk_len = t.in<u64>(nb), unit_off = t.in<u64>(nunits), unit_cap = t.in<u64>(nunits);
+    const Col<uint32_t> first = t.in<uint32_t>(nunits), count = t.in<uint32_t>(nunits);
+    const Col<u64> unit_len = t.out<u64>(nunits);
+    const Col<int32_t> status = t.out<int32_t>(nunits);
+    const Col<uint32_t> ck = t.out<uint32_t>(nb);
+    u64 *u_off = t.host(unit_off), *u_cap = t.host(unit_cap);
+    uint32_t *h_first = t.host(first), *h_cnt = t.host(count);
+    for (size_t i = 0; i < nb; i++) { t.host(blk_off)[i] = blocks[i].off; t.host(blk_len)[i] = blocks[i].len | (blocks[i].stored ? 1ull << 63 : 0); }
     // first-attempt capacity: the frame's block size, but never more than an LZ4 block of that many bytes can expand to
     // (each input byte adds at most 255 output bytes) — frames made of many tiny flushed blocks would otherwise ask for
     // nb x 4 MiB; a block that decodes to more than this reports the size it needs and is redone (overflow retry below)
@@ -67,31 +73,21 @@ int run_blocks(DeviceInput &dev, const std::vector<Block> &blocks, int mode, boo
         for (size_t i = 0; i < nb; i++) total += cap_of(i);
         u_off[0] = 0; u_cap[0] = total; h_first[0] = 0; h_cnt[0] = (uint32_t)nb;
     }
-    DevBuf d_meta, d_ck;
-    std::vector<uint64_t> r_len(nunits);
-    std::vector<int32_t> r_st(nunits);
-    std::vector<uint32_t> r_ck(nb);
-    int st;
+    std::vector<uint64_t> r_len;
+    std::vector<int32_t> r_st;
+    std::vector<uint32_t> r_ck;
+    int st = t.alloc();
+    if (st) return st;
     for (int attempt = 0; attempt < 2; attempt++) {
         if ((st = d_out_keep.alloc(total))) return st;
-        const size_t mbytes = nb * 16 + nunits * (8 * 3 + 4 * 3) + 64;
-        if ((st = d_meta.alloc(mbytes))) return st;
-        uint8_t *m = d_meta.as<uint8_t>();
-        uint64_t *d_boff = (uint64_t *)m, *d_blen = d_boff + nb, *d_uoff = d_blen + nb, *d_ucap = d_uoff + nunits, *d_ulen = d_ucap + nunits;
-        uint32_t *d_first = (uint32_t *)(d_ulen + nunits), *d_cnt = d_first + nunits;
-        int32_t *d_st = (int32_t *)(d_cnt + nunits);
-        SWC_CUDA_TRY(cudaMemcpy(d_boff, h_off.data(), nb * 8, cudaMemcpyHostToDevice));
-        SWC_CUDA_TRY(cudaMemcpy(d_blen, h_len.data(), nb * 8, cudaMemcpyHostToDevice));
-        SWC_CUDA_TRY(cudaMemcpy(d_uoff, u_off.data(), nunits * 8, cudaMemcpyHostToDevice));
-        SWC_CUDA_TRY(cudaMemcpy(d_ucap, u_cap.data(), nunits * 8, cudaMemcpyHostToDevice));
-        SWC_CUDA_TRY(cudaMemcpy(d_first, h_first.data(), nunits * 4, cudaMemcpyHostToDevice));
-        SWC_CUDA_TRY(cudaMemcpy(d_cnt, h_cnt.data(), nunits * 4, cudaMemcpyHostToDevice));
+        if ((st = t.upload())) return st;
         lz4::Args a;
-        a.in_base = dev.in.as<u8>(); a.blk_off = d_boff; a.blk_len = d_blen; a.first_blk = d_first; a.n_blk = d_cnt;
+        a.in_base = dev.in.as<u8>(); a.blk_off = t.dev(blk_off); a.blk_len = t.dev(blk_len); a.first_blk = t.dev(first); a.n_blk = t.dev(count);
         a.dict = use_dict && dev.have_dict ? dev.dict.as<u8>() : nullptr;
         a.dict_len = use_dict && dev.have_dict ? dev.dict_len : 0;
         if (mode == 1 && a.dict_len > 65536) { a.dict += a.dict_len - 65536; a.dict_len = 65536; }    // LZ4.swift:309
-        a.out_base = d_out_keep.as<u8>(); a.out_off = d_uoff; a.out_cap = d_ucap; a.out_len = d_ulen; a.status = d_st; a.n = nunits;
+        a.out_base = d_out_keep.as<u8>(); a.out_off = t.dev(unit_off); a.out_cap = t.dev(unit_cap); a.out_len = t.dev(unit_len);
+        a.status = t.dev(status); a.n = nunits;
         a.scratch = nullptr;
         if (mode == 0) {               // one block per unit: take the two-phase (parse + 8-wide execute) path
             uint64_t tot = 0;
@@ -102,12 +98,10 @@ int run_blocks(DeviceInput &dev, const std::vector<Block> &blocks, int mode, boo
         }
         if ((st = lz4::launch(a, 0))) return st;
         if (check_blocks && attempt == 0) {
-            if ((st = d_ck.alloc(nb * 4))) return st;
-            if ((st = checks::xxh32_batch(dev.in.as<u8>(), d_boff, d_blen, d_ck.as<u32>(), nb, 0))) return st;
-            SWC_CUDA_TRY(cudaMemcpy(r_ck.data(), d_ck.p, nb * 4, cudaMemcpyDeviceToHost));
+            if ((st = checks::xxh32_batch(dev.in.as<u8>(), t.dev(blk_off), t.dev(blk_len), t.dev(ck), nb, 0))) return st;
+            if ((st = t.fetch(ck, r_ck))) return st;
         }
-        SWC_CUDA_TRY(cudaMemcpy(r_len.data(), d_ulen, nunits * 8, cudaMemcpyDeviceToHost));
-        SWC_CUDA_TRY(cudaMemcpy(r_st.data(), d_st, nunits * 4, cudaMemcpyDeviceToHost));
+        if ((st = t.fetch(unit_len, r_len)) || (st = t.fetch(status, r_st))) return st;
         bool overflow = false;
         for (size_t u = 0; u < nunits; u++) if (r_st[u] == SWC_ERR_OUTPUT_OVERFLOW) overflow = true;
         if (!overflow) break;
@@ -136,17 +130,16 @@ int run_blocks(DeviceInput &dev, const std::vector<Block> &blocks, int mode, boo
     // gather
     size_t produced = 0;
     for (size_t u = 0; u < nunits; u++) produced += (size_t)r_len[u];
-    size_t base = host_out.size();
-    host_out.resize(base + produced);
+    uint8_t *dst = host_out.grow(produced);
+    if (!dst) return SWC_ERR_OUTPUT_OVERFLOW;
     bool contiguous = true;
     { size_t run = 0; for (size_t u = 0; u < nunits; u++) { if (u_off[u] != run) contiguous = false; run += (size_t)r_len[u]; } }
     if (contiguous) {
-        if (produced) SWC_CUDA_TRY(cudaMemcpy(host_out.data() + base, d_out_keep.p, produced, cudaMemcpyDeviceToHost));
+        if (produced) SWC_CUDA_TRY(cudaMemcpy(dst, d_out_keep.p, produced, cudaMemcpyDeviceToHost));
     } else {
-        size_t w = base;
         for (size_t u = 0; u < nunits; u++) {
-            if (r_len[u]) SWC_CUDA_TRY(cudaMemcpy(host_out.data() + w, d_out_keep.as<u8>() + u_off[u], (size_t)r_len[u], cudaMemcpyDeviceToHost));
-            w += (size_t)r_len[u];
+            if (r_len[u]) SWC_CUDA_TRY(cudaMemcpy(dst, d_out_keep.as<u8>() + u_off[u], (size_t)r_len[u], cudaMemcpyDeviceToHost));
+            dst += (size_t)r_len[u];
         }
     }
     d_out_len = contiguous ? produced : 0;     // 0 = the device copy is not one contiguous run
@@ -155,7 +148,7 @@ int run_blocks(DeviceInput &dev, const std::vector<Block> &blocks, int mode, boo
 
 // process(frame:) LZ4.swift:188-330; `p` is the whole input, `pos` points right after the magic.
 int frame(DeviceInput &dev, const uint8_t *p, size_t n_total, size_t pos, bool have_dict, bool has_ext_id, uint32_t ext_id,
-          std::vector<uint8_t> &out, size_t *next) {
+          HostOut &out, size_t *next) {
     const uint8_t *in = p + pos;
     const size_t n = n_total - pos;
     if (n < 7) return SWC_DATA_TRUNCATED;
@@ -181,7 +174,7 @@ int frame(DeviceInput &dev, const uint8_t *p, size_t n_total, size_t pos, bool h
     if (dictid_p) {
         if (!have_dict) return SWC_DATA_CORRUPTED;
         if (n - off < 9) return SWC_DATA_TRUNCATED;
-        uint32_t id = rd32(in + off); off += 4;
+        uint32_t id = le32(in + off); off += 4;
         if (has_ext_id && ext_id != id) return SWC_DATA_CORRUPTED;
     }
     const uint8_t hc = (uint8_t)((xxh32_descriptor(in, off) >> 8) & 0xFF);
@@ -192,53 +185,50 @@ int frame(DeviceInput &dev, const uint8_t *p, size_t n_total, size_t pos, bool h
     int pending = SWC_OK;
     for (;;) {                                                     // LZ4.swift:278-318 framing only
         if (n - off < 4) { pending = SWC_DATA_TRUNCATED; break; }
-        uint32_t mark = rd32(in + off); off += 4;
+        uint32_t mark = le32(in + off); off += 4;
         if (mark == 0) break;
         size_t bs = mark & 0x7FFFFFFFu;
         if (bs > max_block) { pending = SWC_DATA_CORRUPTED; break; }
         if (n - off < bs + (block_ck ? 4 : 0) + 4) { pending = SWC_DATA_TRUNCATED; break; }
         Block b; b.off = pos + off; b.len = bs; b.stored = (mark & 0x80000000u) != 0; b.has_ck = block_ck; b.stored_ck = 0;
         off += bs;
-        if (block_ck) { b.stored_ck = rd32(in + off); off += 4; }
+        if (block_ck) { b.stored_ck = le32(in + off); off += 4; }
         blocks.push_back(b);
     }
-    const size_t fstart = out.size();
+    const size_t fstart = out.len;
     DevBuf d_out; size_t d_out_len = 0;
     int st = run_blocks(dev, blocks, independent ? 0 : 1, have_dict, max_block, block_ck, pending, out, d_out, d_out_len);
     if (st) return st;
-    if (csize_p && (uint64_t)(out.size() - fstart) != content_size) return SWC_DATA_CORRUPTED;
+    const size_t flen = out.len - fstart;
+    if (csize_p && (uint64_t)flen != content_size) return SWC_DATA_CORRUPTED;
     if (cck) {                                                     // :323-328
         if (n - off < 4) return SWC_DATA_TRUNCATED;
-        uint32_t stored = rd32(in + off); off += 4;
+        uint32_t stored = le32(in + off); off += 4;
         // content checksum over the decoded frame, on the device
-        DevBuf d_res; uint64_t len64 = d_out_len; uint32_t got = 0;
-        bool whole = (d_out_len == out.size() - fstart);
         DevBuf d_tmp;
         const u8 *d_data = d_out.as<u8>();
-        if (!whole || d_out_len == 0) {        // output was gathered from non-contiguous regions (or is empty): re-upload
-            if ((st = d_tmp.alloc(out.size() - fstart + 16))) return st;
-            if (out.size() > fstart) SWC_CUDA_TRY(cudaMemcpy(d_tmp.p, out.data() + fstart, out.size() - fstart, cudaMemcpyHostToDevice));
-            d_data = d_tmp.as<u8>(); len64 = out.size() - fstart;
+        if (d_out_len != flen || d_out_len == 0) {  // output was gathered from non-contiguous regions (or is empty): re-upload
+            if ((st = d_tmp.alloc(flen + 16))) return st;
+            if (flen) SWC_CUDA_TRY(cudaMemcpy(d_tmp.p, out.p + fstart, flen, cudaMemcpyHostToDevice));
+            d_data = d_tmp.as<u8>();
         }
-        if ((st = d_res.alloc(16))) return st;
-        SWC_CUDA_TRY(cudaMemcpy(d_res.p, &len64, 8, cudaMemcpyHostToDevice));
-        if ((st = checks::xxh32_batch(d_data, nullptr, d_res.as<u64>(), (u32 *)(d_res.as<u8>() + 8), 1, 0))) return st;
-        SWC_CUDA_TRY(cudaMemcpy(&got, d_res.as<u8>() + 8, 4, cudaMemcpyDeviceToHost));
+        u64 got = 0;
+        if ((st = checks::check_device(checks::XXH32, d_data, flen, &got))) return st;
         *next = pos + off;
-        if (got != stored) return SWC_DATA_CHECKSUM_MISMATCH;
+        if ((uint32_t)got != stored) return SWC_DATA_CHECKSUM_MISMATCH;
     }
     *next = pos + off;
     return SWC_OK;
 }
 
 // process(legacyFrame:) LZ4.swift:160-186
-int legacy_frame(DeviceInput &dev, const uint8_t *p, size_t n_total, size_t pos, std::vector<uint8_t> &out, size_t *next) {
+int legacy_frame(DeviceInput &dev, const uint8_t *p, size_t n_total, size_t pos, HostOut &out, size_t *next) {
     size_t off = pos;
     std::vector<Block> blocks;
     int pending = SWC_OK;
     while (off < n_total) {
         if (n_total - off < 4) { pending = SWC_DATA_TRUNCATED; break; }
-        uint32_t raw = rd32(p + off); off += 4;
+        uint32_t raw = le32(p + off); off += 4;
         if (is_magic(raw)) { off -= 4; break; }
         if (n_total - off < raw) { pending = SWC_DATA_TRUNCATED; break; }
         Block b; b.off = off; b.len = raw; b.stored = false; b.has_ck = false; b.stored_ck = 0;
@@ -254,23 +244,11 @@ int legacy_frame(DeviceInput &dev, const uint8_t *p, size_t n_total, size_t pos,
 
 int upload(DeviceInput &dev, const uint8_t *in, size_t in_len, const uint8_t *dict, size_t dict_len) {
     int st;
-    if ((st = dev.in.alloc(round16(in_len) + 32))) return st;
-    { int cst = copy_pageable(dev.in.p, in, in_len, true); if (cst) return cst; }
+    if ((st = upload_input(dev.in, in, in_len))) return st;
     dev.in_len = in_len;
     dev.have_dict = dict != nullptr;
     dev.dict_len = dict ? dict_len : 0;
-    if (dict && dict_len) {
-        if ((st = dev.dict.alloc(dict_len))) return st;
-        SWC_CUDA_TRY(cudaMemcpy(dev.dict.p, dict, dict_len, cudaMemcpyHostToDevice));
-    }
-    return SWC_OK;
-}
-
-int give(const std::vector<uint8_t> &v, uint8_t **out, size_t *out_len) {
-    uint8_t *h = (uint8_t *)swc_alloc(v.size());
-    if (!h) return SWC_ERR_OUTPUT_OVERFLOW;
-    if (!v.empty()) memcpy(h, v.data(), v.size());
-    *out = h; *out_len = v.size();
+    if (dict && dict_len && (st = upload_input(dev.dict, dict, dict_len))) return st;
     return SWC_OK;
 }
 
@@ -314,33 +292,31 @@ int32_t swc_lz4_block_decompress_batch_host(const uint8_t *in_base, const uint64
     ApiLock api_lock;
     if (n == 0) return SWC_OK;
     if (!in_base || !in_off || !in_len || !out_base || !out_off || !out_cap || !out_len || !status) return SWC_ERR_INVALID_ARG;
-    for (uint64_t i = 0; i < n; i++)                                       // every unit inside the two arenas, overflow-safe
-        if (in_off[i] > in_total || in_len[i] > in_total - in_off[i] || out_off[i] > out_total || out_cap[i] > out_total - out_off[i] || (out_off[i] & 15))
-            return SWC_ERR_INVALID_ARG;
-    DevBuf d_in, d_out, d_meta;
-    int st;
+    bool monotone;
+    int st = check_host_units(in_off, in_len, in_total, out_off, out_cap, out_total, n, &monotone);
+    if (st) return st;
+    // the unit table's columns are filled straight from the caller's arrays
+    UnitTable t;
+    const Col<u64> d_in_off = t.out<u64>(n), d_in_len = t.out<u64>(n), d_out_off = t.out<u64>(n), d_out_cap = t.out<u64>(n);
+    const Col<u64> d_out_len = t.out<u64>(n);
+    const Col<int32_t> d_status = t.out<int32_t>(n);
+    DevBuf d_in, d_out;
     if ((st = d_in.alloc(round16(in_total) + 32))) return st;
     if ((st = d_out.alloc(round16(out_total)))) return st;
+    if ((st = t.alloc())) return st;
     const size_t tb = n * 8;
-    if ((st = d_meta.alloc(tb * 5 + n * 4))) return st;
-    u8 *m = d_meta.as<u8>();
     cudaStream_t s = 0;
     SWC_CUDA_TRY(cudaMemcpyAsync(d_in.p, in_base, in_total, cudaMemcpyHostToDevice, s));
-    SWC_CUDA_TRY(cudaMemcpyAsync(m + 0 * tb, in_off, tb, cudaMemcpyHostToDevice, s));
-    SWC_CUDA_TRY(cudaMemcpyAsync(m + 1 * tb, in_len, tb, cudaMemcpyHostToDevice, s));
-    SWC_CUDA_TRY(cudaMemcpyAsync(m + 2 * tb, out_off, tb, cudaMemcpyHostToDevice, s));
-    SWC_CUDA_TRY(cudaMemcpyAsync(m + 3 * tb, out_cap, tb, cudaMemcpyHostToDevice, s));
-    st = swc_lz4_block_decompress_batch(d_in.as<u8>(), (u64 *)(m + 0 * tb), (u64 *)(m + 1 * tb), nullptr, 0, d_out.as<u8>(),
-                                        (u64 *)(m + 2 * tb), (u64 *)(m + 3 * tb), (u64 *)(m + 4 * tb), (int32_t *)(m + 5 * tb), n, s);
+    SWC_CUDA_TRY(cudaMemcpyAsync(t.dev(d_in_off), in_off, tb, cudaMemcpyHostToDevice, s));
+    SWC_CUDA_TRY(cudaMemcpyAsync(t.dev(d_in_len), in_len, tb, cudaMemcpyHostToDevice, s));
+    SWC_CUDA_TRY(cudaMemcpyAsync(t.dev(d_out_off), out_off, tb, cudaMemcpyHostToDevice, s));
+    SWC_CUDA_TRY(cudaMemcpyAsync(t.dev(d_out_cap), out_cap, tb, cudaMemcpyHostToDevice, s));
+    st = swc_lz4_block_decompress_batch(d_in.as<u8>(), t.dev(d_in_off), t.dev(d_in_len), nullptr, 0, d_out.as<u8>(), t.dev(d_out_off),
+                                        t.dev(d_out_cap), t.dev(d_out_len), t.dev(d_status), n, s);
     if (st) return st;
-    for (uint64_t i = 0; i < n;) {                         // only the output regions come back (touching ones as one copy)
-        const uint64_t r0 = out_off[i];
-        uint64_t r1 = r0 + out_cap[i++];
-        while (i < n && out_off[i] == r1) r1 += out_cap[i++];
-        if (r1 > r0) SWC_CUDA_TRY(cudaMemcpyAsync(out_base + r0, d_out.as<u8>() + r0, r1 - r0, cudaMemcpyDeviceToHost, s));
-    }
-    SWC_CUDA_TRY(cudaMemcpyAsync(out_len, m + 4 * tb, tb, cudaMemcpyDeviceToHost, s));
-    SWC_CUDA_TRY(cudaMemcpyAsync(status, m + 5 * tb, n * 4, cudaMemcpyDeviceToHost, s));
+    if ((st = copy_back_regions(out_base, d_out.as<u8>(), out_off, out_cap, 0, n, s))) return st;
+    SWC_CUDA_TRY(cudaMemcpyAsync(out_len, t.dev(d_out_len), tb, cudaMemcpyDeviceToHost, s));
+    SWC_CUDA_TRY(cudaMemcpyAsync(status, t.dev(d_status), n * 4, cudaMemcpyDeviceToHost, s));
     SWC_CUDA_TRY(cudaStreamSynchronize(s));
     return SWC_OK;
 }
@@ -357,10 +333,10 @@ int32_t swc_lz4_decompress(const uint8_t *in, size_t in_len, const uint8_t *dict
     bool have_dict = dict != nullptr;
     for (;;) {
         if (in_len - base < 4) return SWC_DATA_TRUNCATED;
-        const uint32_t magic = rd32(in + base);
+        const uint32_t magic = le32(in + base);
         if (magic >= 0x184D2A50u && magic <= 0x184D2A5Fu) {           // :148-155, then recursion without dictionary (:85)
             if (in_len - base - 4 < 4) return SWC_DATA_TRUNCATED;
-            size_t size = rd32(in + base + 4);
+            size_t size = le32(in + base + 4);
             if (in_len - base - 4 < size + 4) return SWC_DATA_TRUNCATED;
             base += 4 + size + 4;
             have_dict = false; has_dict_id = 0;
@@ -370,13 +346,13 @@ int32_t swc_lz4_decompress(const uint8_t *in, size_t in_len, const uint8_t *dict
         DeviceInput dev;
         int st = upload(dev, in, in_len, have_dict ? dict : nullptr, dict_len);
         if (st) return st;
-        std::vector<uint8_t> o;
+        HostOut o;
         size_t next = base + 4;
         if (magic == 0x184D2204u) st = frame(dev, in, in_len, base + 4, have_dict, has_dict_id != 0, dict_id, o, &next);
         else st = legacy_frame(dev, in, in_len, base + 4, o, &next);
         if (consumed_bytes) *consumed_bytes = next;
         if (st != SWC_OK && st != SWC_DATA_CHECKSUM_MISMATCH) return st;
-        int g = give(o, out, out_len);
+        int g = o.release_to(out, out_len);
         return g ? g : st;
     }
 }
@@ -391,13 +367,13 @@ int32_t swc_lz4_multi_decompress(const uint8_t *in, size_t in_len, const uint8_t
     ApiLock api_lock;
     DeviceInput dev;
     bool uploaded = false;
-    std::vector<uint8_t> o;
+    HostOut o;
     std::vector<size_t> ends;
     size_t next = 0;
     int result = SWC_OK;
     do {
         if (next + 4 > in_len) { result = SWC_DATA_TRUNCATED; break; }
-        const uint32_t magic = rd32(in + next); next += 4;
+        const uint32_t magic = le32(in + next); next += 4;
         int st = SWC_OK; bool produced = false;
         if (magic == 0x184D2204u || magic == 0x184C2102u) {
             if (!uploaded) { if ((st = upload(dev, in, in_len, dict, dict_len))) return st; uploaded = true; }
@@ -407,18 +383,16 @@ int32_t swc_lz4_multi_decompress(const uint8_t *in, size_t in_len, const uint8_t
             next = nn; produced = true;
         } else if (magic >= 0x184D2A50u && magic <= 0x184D2A5Fu) {
             if (in_len - next < 4) { result = SWC_DATA_TRUNCATED; break; }
-            size_t size = rd32(in + next);
+            size_t size = le32(in + next);
             if (in_len - next < size + 4) { result = SWC_DATA_TRUNCATED; break; }
             next += size + 4;
         } else { result = SWC_DATA_CORRUPTED; break; }
-        if (produced && (st == SWC_OK || st == SWC_DATA_CHECKSUM_MISMATCH)) ends.push_back(o.size());
+        if (produced && (st == SWC_OK || st == SWC_DATA_CHECKSUM_MISMATCH)) ends.push_back(o.len);
         if (st) { result = st; break; }
     } while (next < in_len);
     if (result != SWC_OK && result != SWC_DATA_CHECKSUM_MISMATCH) return result;
-    int g = give(o, out, out_len);
-    if (g) return g;
-    *frame_ends = (size_t *)swc_alloc(sizeof(size_t) * (ends.size() + 1));
-    for (size_t i = 0; i < ends.size(); i++) (*frame_ends)[i] = ends[i];
+    int g;
+    if ((g = o.release_to(out, out_len)) || (g = give_sizes(ends, frame_ends, out, out_len))) return g;
     *n_frames = ends.size();
     return result;
 }
@@ -545,47 +519,42 @@ int32_t swc_lz4_compress(const uint8_t *in, size_t in_len, int32_t independent_b
     if (D) SWC_CUDA_TRY(cudaMemcpy(d_in.p, dict + (dict_len - D), D, cudaMemcpyHostToDevice));
     if (in_len) { int cst = copy_pageable(d_in.as<u8>() + D, in, in_len, true); if (cst) return cst; }
 
-    // per block: in_off, in_len, dict_off, dict_len, out_off, out_cap, then out_len, status, payload length, stored flag
-    std::vector<uint64_t> meta(nb * 6);
-    uint64_t *h_in_off = meta.data(), *h_in_len = h_in_off + nb, *h_doff = h_in_len + nb, *h_dlen = h_doff + nb;
-    uint64_t *h_out_off = h_dlen + nb, *h_out_cap = h_out_off + nb;
-    std::vector<uint64_t> scr_off(nb);
+    // per block: where it is read from and which window precedes it; after the parse, where its payload goes in the frame
+    UnitTable t;
+    const Col<u64> in_off = t.in<u64>(nb), in_len_c = t.in<u64>(nb), dict_off = t.in<u64>(nb), dict_len_c = t.in<u64>(nb);
+    const Col<u64> out_off = t.in<u64>(nb), out_cap = t.in<u64>(nb), scr_off = t.in<u64>(nb), pay_len_c = t.in<u64>(nb);
+    const Col<u8> stored_c = t.in<u8>(nb);
+    const Col<u64> res_len_c = t.out<u64>(nb);
+    const Col<int32_t> status_c = t.out<int32_t>(nb);
+    const Col<uint32_t> ck_c = t.out<uint32_t>(nb);
+    u64 *h_in_len = t.host(in_len_c), *h_dlen = t.host(dict_len_c), *pay_off = t.host(out_off), *pay_len = t.host(pay_len_c);
+    u8 *stored = t.host(stored_c);
     u64 scr_total = 0;
     for (u64 k = 0; k < nb; k++) {
         const u64 o = k * bs, l = in_len - o < bs ? in_len - o : bs;
-        h_in_off[k] = D + o; h_in_len[k] = l;
-        if (independent_blocks || k == 0) { h_doff[k] = 0; h_dlen[k] = D; }                               // :105
-        else { const u64 pl = bs < lz4c::MAX_DICT ? bs : lz4c::MAX_DICT; h_doff[k] = D + o - pl; h_dlen[k] = pl; }   // :106-110
-        h_out_off[k] = 0; h_out_cap[k] = ~0ull;
-        scr_off[k] = scr_total;
+        t.host(in_off)[k] = D + o; h_in_len[k] = l;
+        if (independent_blocks || k == 0) { t.host(dict_off)[k] = 0; h_dlen[k] = D; }                     // :105
+        else { const u64 pl = bs < lz4c::MAX_DICT ? bs : lz4c::MAX_DICT; t.host(dict_off)[k] = D + o - pl; h_dlen[k] = pl; }   // :106-110
+        pay_off[k] = 0; t.host(out_cap)[k] = ~0ull;
+        t.host(scr_off)[k] = scr_total;
         scr_total += need_of(l, h_dlen[k]);
     }
-    DevBuf d_meta, d_scr;
-    const size_t mb = nb * 8;
-    if ((st = d_meta.alloc(mb * 10 + 64))) return st;
-    u8 *m = d_meta.as<u8>();
-    u64 *d_res_len = (u64 *)(m + 6 * mb), *d_scr_off = (u64 *)(m + 7 * mb);
-    int32_t *d_status = (int32_t *)(m + 8 * mb);
-    u8 *d_stored = m + 9 * mb;
-    u32 *d_ck = (u32 *)(m + 9 * mb + ((nb + 15) & ~(u64)15));
+    DevBuf d_scr;
+    if ((st = t.alloc())) return st;
     if ((st = d_scr.alloc(scr_total + 256))) return st;
-    std::vector<uint64_t> res_len(nb);
-    std::vector<int32_t> res_st(nb);
-    std::vector<uint8_t> stored(nb);
-    std::vector<uint32_t> cks(nb);
+    std::vector<uint64_t> res_len;
+    std::vector<int32_t> res_st;
+    std::vector<uint32_t> cks;
     u64 frame_len = h;
-    std::vector<u64> pay_off(nb), pay_len(nb);
     lz4c::Args a;
     if (nb) {
-        SWC_CUDA_TRY(cudaMemcpy(m, meta.data(), 6 * mb, cudaMemcpyHostToDevice));
-        SWC_CUDA_TRY(cudaMemcpy(d_scr_off, scr_off.data(), mb, cudaMemcpyHostToDevice));
-        a.in_base = d_in.as<u8>(); a.in_off = (u64 *)m; a.in_len = (u64 *)(m + mb);
-        a.dict_off = (u64 *)(m + 2 * mb); a.dict_len = (u64 *)(m + 3 * mb);
-        a.out_base = nullptr; a.out_off = (u64 *)(m + 4 * mb); a.out_cap = (u64 *)(m + 5 * mb);
-        a.out_len = d_res_len; a.status = d_status; a.stored = nullptr; a.n = nb;
-        if ((st = lz4c::parse(a, 0, nb, d_scr.as<u8>(), d_scr_off, 0))) return st;
-        SWC_CUDA_TRY(cudaMemcpy(res_len.data(), d_res_len, mb, cudaMemcpyDeviceToHost));
-        SWC_CUDA_TRY(cudaMemcpy(res_st.data(), d_status, nb * 4, cudaMemcpyDeviceToHost));
+        if ((st = t.upload())) return st;
+        a.in_base = d_in.as<u8>(); a.in_off = t.dev(in_off); a.in_len = t.dev(in_len_c);
+        a.dict_off = t.dev(dict_off); a.dict_len = t.dev(dict_len_c);
+        a.out_base = nullptr; a.out_off = t.dev(out_off); a.out_cap = t.dev(out_cap);
+        a.out_len = t.dev(res_len_c); a.status = t.dev(status_c); a.stored = nullptr; a.n = nb;
+        if ((st = lz4c::parse(a, 0, nb, d_scr.as<u8>(), t.dev(scr_off), 0))) return st;
+        if ((st = t.fetch(res_len_c, res_len)) || (st = t.fetch(status_c, res_st))) return st;
         for (u64 k = 0; k < nb; k++) {
             if (res_st[k] != SWC_OK) return res_st[k];
             stored[k] = res_len[k] > h_in_len[k];                                                        // :112
@@ -600,25 +569,19 @@ int32_t swc_lz4_compress(const uint8_t *in, size_t in_len, int32_t independent_b
     if ((st = d_frame.alloc(frame_len + 16))) return st;
     if (nb) {
         // the payloads go straight to their frame offsets; out_cap keeps the parse's "unbounded" fence
-        memcpy(h_out_off, pay_off.data(), mb);
-        SWC_CUDA_TRY(cudaMemcpy(m + 4 * mb, h_out_off, mb, cudaMemcpyHostToDevice));
-        SWC_CUDA_TRY(cudaMemcpy(d_stored, stored.data(), nb, cudaMemcpyHostToDevice));
-        a.out_base = d_frame.as<u8>(); a.stored = d_stored;
-        if ((st = lz4c::emit(a, 0, nb, d_scr.as<u8>(), d_scr_off, 0))) return st;
+        if ((st = t.upload())) return st;
+        a.out_base = d_frame.as<u8>(); a.stored = t.dev(stored_c);
+        if ((st = lz4c::emit(a, 0, nb, d_scr.as<u8>(), t.dev(scr_off), 0))) return st;
         if (block_checksums) {                                                                           // :120-125, :133-138
-            SWC_CUDA_TRY(cudaMemcpy(d_res_len, pay_len.data(), mb, cudaMemcpyHostToDevice));
-            if ((st = checks::xxh32_batch(d_frame.as<u8>(), a.out_off, d_res_len, d_ck, nb, 0))) return st;
-            SWC_CUDA_TRY(cudaMemcpy(cks.data(), d_ck, nb * 4, cudaMemcpyDeviceToHost));
+            if ((st = checks::xxh32_batch(d_frame.as<u8>(), a.out_off, t.dev(pay_len_c), t.dev(ck_c), nb, 0))) return st;
+            if ((st = t.fetch(ck_c, cks))) return st;
         }
     }
     uint32_t content_ck = xxh32_descriptor(nullptr, 0);
     if (content_checksum && in_len) {                                                                    // :146-151
-        DevBuf d_res;
-        if ((st = d_res.alloc(16))) return st;
-        const u64 len64 = in_len;
-        SWC_CUDA_TRY(cudaMemcpy(d_res.p, &len64, 8, cudaMemcpyHostToDevice));
-        if ((st = checks::xxh32_batch(d_in.as<u8>() + D, nullptr, d_res.as<u64>(), (u32 *)(d_res.as<u8>() + 8), 1, 0))) return st;
-        SWC_CUDA_TRY(cudaMemcpy(&content_ck, d_res.as<u8>() + 8, 4, cudaMemcpyDeviceToHost));
+        u64 v = 0;
+        if ((st = checks::check_device(checks::XXH32, d_in.as<u8>() + D, in_len, &v))) return st;
+        content_ck = (uint32_t)v;
     }
     uint8_t *host = (uint8_t *)swc_alloc(frame_len);
     if (!host) return SWC_ERR_OUTPUT_OVERFLOW;

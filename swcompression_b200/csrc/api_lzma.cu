@@ -24,45 +24,25 @@ struct LzmaJob {           // one unit, resident on the device
 
 // d_in[start..in_len) holds the stream; grows the output until it fits.
 int lzma_unit_device(const u8 *d_in, size_t in_len, size_t start, const LzmaJob &job, size_t cap_hint, UnitResult &r) {
-    size_t cap = cap_hint ? cap_hint : (in_len - start) * 8 + (1u << 20);
-    DevBuf meta, lit;
-    int st = meta.alloc(512);
+    DevBuf lit;
+    int st = lit.alloc(lzma::lit_scratch_bytes(1));
     if (st) return st;
-    if ((st = lit.alloc(lzma::lit_scratch_bytes(1)))) return st;
-    for (int attempt = 0; attempt < 8; attempt++) {
-        cap = round16(cap);
-        if ((st = r.out.alloc(cap))) return st;
-        // meta: in_off, in_len, out_off, out_cap, out_len, consumed (u64) | status i32 @48 | dict_byte @64 | props u32 @72 | dict_size @80 | usize @88
-        u8 h[128] = {0};
-        u64 q[6] = {start, in_len - start, 0, cap, 0, 0};
-        memcpy(h, q, sizeof(q));
-        h[64] = job.dict_byte;
-        memcpy(h + 72, &job.props, 4); memcpy(h + 80, &job.dict_size, 8); memcpy(h + 88, &job.usize, 8);
-        SWC_CUDA_TRY(cudaMemcpy(meta.p, h, sizeof(h), cudaMemcpyHostToDevice));
-        u8 *m = meta.as<u8>();
+    UnitTable t;
+    UnitCols c(t, 1);
+    const Col<u8> dict_byte = t.in<u8>(1);
+    const Col<u32> props = t.in<u32>(1);
+    const Col<i64> dict_size = t.in<i64>(1), usize = t.in<i64>(1);
+    *t.host(dict_byte) = job.dict_byte; *t.host(props) = job.props; *t.host(dict_size) = job.dict_size; *t.host(usize) = job.usize;
+    // LZMA cannot size its output without decoding it (the dictionary IS the output): x4 per attempt
+    return decode_unit(t, c, start, in_len, cap_hint ? cap_hint : (in_len - start) * 8 + (1u << 20), 8,
+                       [](size_t cap, size_t) { return cap >= ((size_t)1 << 33) ? 0 : cap * 4; }, [&](u8 *out, size_t) {
         lzma::Args a;
-        a.mode = job.mode; a.in_base = d_in; a.in_off = (u64 *)m; a.in_len = (u64 *)m + 1;
-        a.dict_bytes = m + 64; a.props = (u32 *)(m + 72); a.dict_size = (i64 *)(m + 80); a.usize = (i64 *)(m + 88);
-        a.out_base = r.out.as<u8>(); a.out_off = (u64 *)m + 2; a.out_cap = (u64 *)m + 3; a.out_len = (u64 *)m + 4; a.consumed = (u64 *)m + 5;
-        a.status = (int32_t *)(m + 48); a.n = 1; a.lit_scratch = lit.as<u16>();
-        if ((st = lzma::launch(a, 0))) return st;
-        SWC_CUDA_TRY(cudaStreamSynchronize(0));
-        u8 res[56];
-        SWC_CUDA_TRY(cudaMemcpy(res, meta.p, 56, cudaMemcpyDeviceToHost));
-        u64 ol, cs; int32_t s32;
-        memcpy(&ol, res + 32, 8); memcpy(&cs, res + 40, 8); memcpy(&s32, res + 48, 4);
-        r.out_len = (size_t)ol; r.consumed = (size_t)cs; r.status = s32;
-        if (r.status != SWC_ERR_OUTPUT_OVERFLOW || cap >= ((size_t)1 << 33)) break;
-        cap *= 4;                 // LZMA cannot size its output without decoding it (the dictionary IS the output)
-    }
-    return SWC_OK;
-}
-
-int upload(DevBuf &d, const uint8_t *in, size_t n) {
-    int st = d.alloc(round16(n) + 256);
-    if (st) return st;
-    { int cst = copy_pageable(d.p, in, n, true); if (cst) return cst; }
-    return SWC_OK;
+        a.mode = job.mode; a.in_base = d_in; a.in_off = t.dev(c.in_off); a.in_len = t.dev(c.in_len);
+        a.dict_bytes = t.dev(dict_byte); a.props = t.dev(props); a.dict_size = t.dev(dict_size); a.usize = t.dev(usize);
+        a.out_base = out; a.out_off = t.dev(c.out_off); a.out_cap = t.dev(c.out_cap); a.out_len = t.dev(c.out_len);
+        a.consumed = t.dev(c.consumed); a.status = t.dev(c.status); a.n = 1; a.lit_scratch = lit.as<u16>();
+        return lzma::launch(a, 0);
+    }, r);
 }
 
 // ---- delta filter (DeltaFilter.swift:11-32): out[i] = in[i] + out[i - distance], one thread per residue class ----
@@ -78,12 +58,6 @@ struct Rd {
     const uint8_t *p; size_t n, off;
     bool need(size_t k) const { return n - off >= k; }
 };
-inline uint32_t le32(const uint8_t *p) { return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24; }
-uint32_t crc32_small(const uint8_t *p, size_t n) {          // header / index / footer fields only (framing)
-    uint32_t c = 0xFFFFFFFFu;
-    for (size_t i = 0; i < n; i++) { c ^= p[i]; for (int k = 0; k < 8; k++) c = (c & 1) ? 0xEDB88320u ^ (c >> 1) : c >> 1; }
-    return ~c;
-}
 int multibyte(Rd &r, int64_t *val) {                          // LittleEndianByteReader+XZ.swift:10-30
     if (!r.need(1)) return SWC_ERR_REFERENCE_TRAP;
     int i = 1;
@@ -152,7 +126,7 @@ int xz_block(Rd &r, const u8 *d_in, unsigned hsize_byte, int csize, DevBuf &blk,
     if (!r.need(4)) return SWC_ERR_REFERENCE_TRAP;
     const uint32_t hcrc = le32(r.p + r.off);
     if (r.n - hstart < real - 4) return SWC_ERR_REFERENCE_TRAP;
-    if (crc32_small(r.p + hstart, real - 4) != hcrc) return SWC_XZ_WRONG_INFO_CRC;
+    if (crc32_framing(r.p + hstart, real - 4) != hcrc) return SWC_XZ_WRONG_INFO_CRC;
     r.off = hstart + real;
 
     const size_t data_start = r.off;
@@ -209,12 +183,12 @@ int xz_block(Rd &r, const u8 *d_in, unsigned hsize_byte, int csize, DevBuf &blk,
 }
 
 // processStream XZArchive.swift:90-130 (+ processIndex, processFooter); stream data is appended to `out` (host)
-int xz_stream(Rd &r, const u8 *d_in, std::vector<uint8_t> &out, bool *check_error) {
+int xz_stream(Rd &r, const u8 *d_in, HostOut &out, bool *check_error) {
     static const uint8_t magic[6] = {0xFD, 0x37, 0x7A, 0x58, 0x5A, 0x00};
     if (!r.need(12)) return SWC_ERR_REFERENCE_TRAP;
     if (memcmp(r.p + r.off, magic, 6) != 0) return SWC_XZ_WRONG_MAGIC;
     const uint8_t *fl = r.p + r.off + 6;
-    if (crc32_small(fl, 2) != le32(r.p + r.off + 8)) return SWC_XZ_WRONG_INFO_CRC;
+    if (crc32_framing(fl, 2) != le32(r.p + r.off + 8)) return SWC_XZ_WRONG_INFO_CRC;
     if (!(fl[0] == 0 && (fl[1] & 0xF0) == 0)) return SWC_XZ_WRONG_FIELD;
     const int ctype = fl[1] & 0xF;
     if (!(ctype == 0 || ctype == 1 || ctype == 4 || ctype == 0x0A)) return SWC_XZ_WRONG_FIELD;
@@ -245,7 +219,7 @@ int xz_stream(Rd &r, const u8 *d_in, std::vector<uint8_t> &out, bool *check_erro
                 }
             }
             if (!r.need(4)) return SWC_ERR_REFERENCE_TRAP;
-            if (crc32_small(r.p + istart, (size_t)isz) != le32(r.p + r.off)) return SWC_XZ_WRONG_INFO_CRC;
+            if (crc32_framing(r.p + istart, (size_t)isz) != le32(r.p + r.off)) return SWC_XZ_WRONG_INFO_CRC;
             r.off = istart + (size_t)isz + 4;
             index_size = isz + 4;
             break;
@@ -253,9 +227,9 @@ int xz_stream(Rd &r, const u8 *d_in, std::vector<uint8_t> &out, bool *check_erro
         DevBuf blk; size_t blk_len = 0; int64_t unp = 0;
         int st = xz_block(r, d_in, hs, check_size(ctype), blk, blk_len, &unp);
         if (st) return st;
-        const size_t base = out.size();
-        out.resize(base + blk_len);
-        if (blk_len) SWC_CUDA_TRY(cudaMemcpy(out.data() + base, blk.p, blk_len, cudaMemcpyDeviceToHost));
+        uint8_t *dst = out.grow(blk_len);
+        if (!dst) return SWC_ERR_OUTPUT_OVERFLOW;
+        if (blk_len) SWC_CUDA_TRY(cudaMemcpy(dst, blk.p, blk_len, cudaMemcpyDeviceToHost));
         if (ctype == 1) {
             if (!r.need(4)) return SWC_ERR_REFERENCE_TRAP;
             const uint32_t c = le32(r.p + r.off); r.off += 4;
@@ -283,7 +257,7 @@ int xz_stream(Rd &r, const u8 *d_in, std::vector<uint8_t> &out, bool *check_erro
     const uint32_t fcrc = le32(r.p + r.off);
     const int64_t backward = ((int64_t)le32(r.p + r.off + 4) + 1) * 4;
     const unsigned fflags = r.p[r.off + 8] | r.p[r.off + 9] << 8;
-    if (crc32_small(r.p + r.off + 4, 6) != fcrc) return SWC_XZ_WRONG_INFO_CRC;
+    if (crc32_framing(r.p + r.off + 4, 6) != fcrc) return SWC_XZ_WRONG_INFO_CRC;
     if (backward != index_size) return SWC_XZ_WRONG_FIELD;
     if (!((fflags & 0xFF) == 0 && ((fflags & 0xF00) >> 8) == (unsigned)ctype && (fflags & 0xF000) == 0)) return SWC_XZ_WRONG_FIELD;
     if (!(r.p[r.off + 10] == 0x59 && r.p[r.off + 11] == 0x5A)) return SWC_XZ_WRONG_MAGIC;
@@ -305,8 +279,8 @@ int xz_padding(Rd &r) {                                               // process
 }
 
 // Walk the stream footers / indexes backwards and batch-decode every single-filter LZMA2 block. Any inconsistency simply
-// ends the discovery (the in-order parser will then report it in the reference's order).
-void xz_prefetch(const uint8_t *in, size_t n, const u8 *d_in, Prefetch &pf) {
+// ends the discovery (the in-order parser will then report it in the reference's order); only a CUDA error is returned.
+int xz_prefetch(const uint8_t *in, size_t n, const u8 *d_in, Prefetch &pf) {
     struct Blk { size_t data_off, comp_len, uncomp; u8 dict_byte; };
     std::vector<Blk> blks;
     size_t pos = n;
@@ -355,73 +329,63 @@ void xz_prefetch(const uint8_t *in, size_t n, const u8 *d_in, Prefetch &pf) {
         if (bad) break;
         pos = sstart;
     }
-    if (blks.size() < 2) return;                          // nothing to gain
+    if (blks.size() < 2) return SWC_OK;                   // nothing to gain
     uint64_t total = 0;
     for (auto &b : blks) {
-        if (b.uncomp > ((uint64_t)48 << 30)) return;
+        if (b.uncomp > ((uint64_t)48 << 30)) return SWC_OK;
         total += round16(b.uncomp + 16);
     }
-    if (total > ((uint64_t)48 << 30)) return;
+    if (total > ((uint64_t)48 << 30)) return SWC_OK;
     const size_t nb = blks.size();
-    std::vector<uint64_t> h_off(nb), h_len(nb), o_off(nb), o_cap(nb);
-    std::vector<uint8_t> h_dict(nb);
+    UnitTable t;
+    UnitCols c(t, nb);
+    const Col<u8> dict = t.in<u8>(nb);
+    u64 *h_off = t.host(c.in_off), *h_len = t.host(c.in_len), *o_off = t.host(c.out_off), *o_cap = t.host(c.out_cap);
     uint64_t run = 0;
-    for (size_t i = 0; i < nb; i++) { h_off[i] = blks[i].data_off; h_len[i] = blks[i].comp_len; o_off[i] = run; o_cap[i] = round16(blks[i].uncomp + 16); run += o_cap[i]; h_dict[i] = blks[i].dict_byte; }
-    DevBuf meta;
-    if (pf.out.alloc(run + 64) || meta.alloc(nb * 8 * 6 + nb * 4 + nb + 64)) return;
-    u64 *m = meta.as<u64>();
-    u8 *d_dict = (u8 *)(m + 6 * nb) + nb * 4;
-    if (cudaMemcpy(m + 0 * nb, h_off.data(), nb * 8, cudaMemcpyHostToDevice) != cudaSuccess) return;
-    cudaMemcpy(m + 1 * nb, h_len.data(), nb * 8, cudaMemcpyHostToDevice);
-    cudaMemcpy(m + 2 * nb, o_off.data(), nb * 8, cudaMemcpyHostToDevice);
-    cudaMemcpy(m + 3 * nb, o_cap.data(), nb * 8, cudaMemcpyHostToDevice);
-    cudaMemcpy(d_dict, h_dict.data(), nb, cudaMemcpyHostToDevice);
+    for (size_t i = 0; i < nb; i++) {
+        h_off[i] = blks[i].data_off; h_len[i] = blks[i].comp_len; o_off[i] = run; o_cap[i] = round16(blks[i].uncomp + 16); run += o_cap[i];
+        t.host(dict)[i] = blks[i].dict_byte;
+    }
+    if (pf.out.alloc(run + 64) || t.alloc()) return SWC_OK;       // no room: the in-order parser decodes block by block
+    int st = t.upload();
+    if (st) return st;
     lzma::Args a;
-    a.mode = lzma::MODE_LZMA2; a.in_base = d_in; a.in_off = m; a.in_len = m + nb; a.dict_bytes = d_dict;
+    a.mode = lzma::MODE_LZMA2; a.in_base = d_in; a.in_off = t.dev(c.in_off); a.in_len = t.dev(c.in_len); a.dict_bytes = t.dev(dict);
     a.props = nullptr; a.dict_size = nullptr; a.usize = nullptr;
-    a.out_base = pf.out.as<u8>(); a.out_off = m + 2 * nb; a.out_cap = m + 3 * nb; a.out_len = m + 4 * nb; a.consumed = m + 5 * nb;
-    a.status = (int32_t *)(m + 6 * nb); a.n = nb; a.lit_scratch = nullptr;
-    if (lzma::launch(a, 0)) return;
-    std::vector<uint64_t> r_len(nb), r_used(nb);
-    std::vector<int32_t> r_st(nb);
-    if (cudaMemcpy(r_len.data(), m + 4 * nb, nb * 8, cudaMemcpyDeviceToHost) != cudaSuccess) { cudaGetLastError(); return; }
-    cudaMemcpy(r_used.data(), m + 5 * nb, nb * 8, cudaMemcpyDeviceToHost);
-    cudaMemcpy(r_st.data(), m + 6 * nb, nb * 4, cudaMemcpyDeviceToHost);
+    a.out_base = pf.out.as<u8>(); a.out_off = t.dev(c.out_off); a.out_cap = t.dev(c.out_cap); a.out_len = t.dev(c.out_len);
+    a.consumed = t.dev(c.consumed); a.status = t.dev(c.status); a.n = nb; a.lit_scratch = nullptr;
+    if ((st = lzma::launch(a, 0))) return st;
+    std::vector<uint64_t> r_len, r_used;
+    std::vector<int32_t> r_st;
+    if ((st = t.fetch(c.out_len, r_len)) || (st = t.fetch(c.consumed, r_used)) || (st = t.fetch(c.status, r_st))) return st;
     for (size_t i = 0; i < nb; i++)
         if (r_st[i] == SWC_OK) pf.by_offset[blks[i].data_off] = PrefetchEntry{(size_t)o_off[i], (size_t)r_len[i], (size_t)r_used[i], blks[i].dict_byte};
+    return SWC_OK;
 }
 
-int xz_all(const uint8_t *in, size_t n, std::vector<uint8_t> &out, std::vector<size_t> &ends) {
+int xz_all(const uint8_t *in, size_t n, HostOut &out, std::vector<size_t> &ends) {
     DevBuf d_in;
-    int st = upload(d_in, in, n);
+    int st = upload_input(d_in, in, n);
     if (st) return st;
     Prefetch pf;
-    xz_prefetch(in, n, d_in.as<u8>(), pf);
+    if ((st = xz_prefetch(in, n, d_in.as<u8>(), pf))) return st;
     struct Guard { Guard(Prefetch *p) { g_prefetch = p; } ~Guard() { g_prefetch = nullptr; } } guard(pf.by_offset.empty() ? nullptr : &pf);
     Rd r{in, n, 0};
     while (r.off < r.n) {
         if (r.n - r.off < 32) return SWC_XZ_WRONG_MAGIC;
         bool check_error = false;
         if ((st = xz_stream(r, d_in.as<u8>(), out, &check_error))) return st;
-        ends.push_back(out.size());
+        ends.push_back(out.len);
         if (check_error) return SWC_XZ_WRONG_CHECK;
         if ((st = xz_padding(r))) return st;
     }
     return SWC_OK;
 }
 
-int give(const std::vector<uint8_t> &v, uint8_t **out, size_t *out_len) {
-    uint8_t *h = (uint8_t *)swc_alloc(v.size());
-    if (!h) return SWC_ERR_OUTPUT_OVERFLOW;
-    if (!v.empty()) memcpy(h, v.data(), v.size());
-    *out = h; *out_len = v.size();
-    return SWC_OK;
-}
-
 int single(const uint8_t *in, size_t in_len, size_t start, const LzmaJob &job, size_t hint,
            uint8_t **out, size_t *out_len, size_t *consumed, size_t header_bytes) {
     DevBuf d_in;
-    int st = upload(d_in, in, in_len);
+    int st = upload_input(d_in, in, in_len);
     if (st) return st;
     UnitResult r;
     if ((st = lzma_unit_device(d_in.as<u8>(), in_len, start, job, hint, r))) return st;
@@ -525,10 +489,10 @@ int32_t swc_xz_unarchive(const uint8_t *in, size_t in_len, uint8_t **out, size_t
     *out = nullptr; *out_len = 0;
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
-    std::vector<uint8_t> o; std::vector<size_t> ends;
+    HostOut o; std::vector<size_t> ends;
     int st = xz_all(in, in_len, o, ends);
     if (st != SWC_OK && st != SWC_XZ_WRONG_CHECK) return st;
-    int g = give(o, out, out_len);
+    int g = o.release_to(out, out_len);
     return g ? g : st;
 }
 
@@ -538,13 +502,11 @@ int32_t swc_xz_split_unarchive(const uint8_t *in, size_t in_len,
     *out = nullptr; *out_len = 0; *stream_ends = nullptr; *n_streams = 0;
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
-    std::vector<uint8_t> o; std::vector<size_t> ends;
+    HostOut o; std::vector<size_t> ends;
     int st = xz_all(in, in_len, o, ends);
     if (st != SWC_OK && st != SWC_XZ_WRONG_CHECK) return st;
-    int g = give(o, out, out_len);
-    if (g) return g;
-    *stream_ends = (size_t *)swc_alloc(sizeof(size_t) * (ends.size() + 1));
-    for (size_t i = 0; i < ends.size(); i++) (*stream_ends)[i] = ends[i];
+    int g;
+    if ((g = o.release_to(out, out_len)) || (g = give_sizes(ends, stream_ends, out, out_len))) return g;
     *n_streams = ends.size();
     return st;
 }

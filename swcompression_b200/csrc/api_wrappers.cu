@@ -14,53 +14,7 @@
 
 using namespace swc;
 
-namespace swc {
-namespace checks {
-
-int check_device(Kind k, const u8 *d, u64 n, u64 *value) {
-    DevBuf res, part;
-    int st;
-    {   // result slot + chunk partials live in a grow-only arena: per-block checks of big archives do no cudaMalloc
-        void *a = nullptr;
-        if ((st = arena_get(3, 64 + partial_bytes(n), &a, 0))) return st;
-        res.borrow(a, 32);
-        part.borrow((u8 *)a + 64, partial_bytes(n));
-    }
-    if (k == XXH32) {
-        SWC_CUDA_TRY(cudaMemcpy(res.p, &n, 8, cudaMemcpyHostToDevice));
-        if ((st = xxh32_batch(d, nullptr, res.as<u64>(), (u32 *)(res.as<u8>() + 8), 1, 0))) return st;
-        u32 v = 0;
-        SWC_CUDA_TRY(cudaMemcpy(&v, res.as<u8>() + 8, 4, cudaMemcpyDeviceToHost));
-        *value = v;
-        return SWC_OK;
-    }
-    switch (k) {
-    case CRC32: st = crc32(d, n, res.as<u64>(), part.as<u64>(), 0); break;
-    case BZIP2_CRC32: st = bzip2_crc32(d, n, res.as<u64>(), part.as<u64>(), 0); break;
-    case CRC64: st = crc64(d, n, res.as<u64>(), part.as<u64>(), 0); break;
-    default: st = adler32(d, n, res.as<u64>(), part.as<u64>(), 0); break;
-    }
-    if (st) return st;
-    SWC_CUDA_TRY(cudaMemcpy(value, res.p, 8, cudaMemcpyDeviceToHost));
-    return SWC_OK;
-}
-
-}  // namespace checks
-}  // namespace swc
-
 namespace {
-
-inline uint32_t rd32(const uint8_t *p) { return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24; }
-
-// CRC-32 of the gzip *header* bytes for FHCRC (framing; <= a few hundred bytes) — GzipHeader.swift:191-198
-uint32_t crc32_header(const uint8_t *p, size_t n) {
-    uint32_t c = 0xFFFFFFFFu;
-    for (size_t i = 0; i < n; i++) {
-        c ^= p[i];
-        for (int k = 0; k < 8; k++) c = (c & 1) ? 0xEDB88320u ^ (c >> 1) : c >> 1;
-    }
-    return ~c;
-}
 
 // GzipHeader.init(_: LsbBitReader), GzipHeader.swift:68-199 — one pass over the member's header that both validates it and
 // records where its fields are.  Written against the Swift source (guards in source order, one `Cursor` read per
@@ -127,7 +81,7 @@ int gzip_parse(const uint8_t *in, size_t n, size_t member_off, swc_gzip_header *
     if (flg & 0x02) {                                                                // FHCRC :194-200
         if (c.left() < 2) return SWC_GZIP_WRONG_MAGIC;
         const unsigned stored = (unsigned)in[c.at] | (unsigned)in[c.at + 1] << 8;
-        if ((crc32_header(in + member_off, c.at - member_off) & 0xFFFFu) != stored) return SWC_GZIP_WRONG_HEADER_CRC;
+        if ((crc32_framing(in + member_off, c.at - member_off) & 0xFFFFu) != stored) return SWC_GZIP_WRONG_HEADER_CRC;
         c.at += 2;
     }
     out.header_len = c.at - member_off;
@@ -160,34 +114,6 @@ int zlib_parse(const uint8_t *in, size_t n, swc_zlib_header *h) {
     return SWC_OK;
 }
 
-// growable malloc'ed host buffer that is handed to the C caller without another copy (swc_free == free)
-struct HostOut {
-    uint8_t *p = nullptr;
-    size_t len = 0, cap = 0;
-    HostOut() {}
-    HostOut(const HostOut &) = delete;
-    HostOut &operator=(const HostOut &) = delete;
-    ~HostOut() { free(p); }
-    uint8_t *grow(size_t add) {                                     // nullptr when out of memory
-        if (len + add > cap || !p) {
-            size_t nc = cap * 2 > len + add ? cap * 2 : len + add;
-            if (nc < 64) nc = 64;
-            uint8_t *q = (uint8_t *)realloc(p, nc);
-            if (!q) return nullptr;
-            p = q; cap = nc;
-        }
-        uint8_t *r = p + len;
-        len += add;
-        return r;
-    }
-    int release_to(uint8_t **out, size_t *out_len) {
-        if (!p && !grow(0)) return SWC_ERR_OUTPUT_OVERFLOW;
-        *out = p; *out_len = len;
-        p = nullptr; len = cap = 0;
-        return SWC_OK;
-    }
-};
-
 // processMember GzipArchive.swift:79-100; d_in holds the whole archive on the device
 int gzip_member(const uint8_t *in, size_t n, const u8 *d_in, size_t *off, HostOut &out, bool *crc_error) {
     if (n - *off < 20) return SWC_GZIP_WRONG_MAGIC;
@@ -198,7 +124,7 @@ int gzip_member(const uint8_t *in, size_t n, const u8 *d_in, size_t *off, HostOu
     if (r.status != SWC_OK) return r.status;
     size_t p = *off + (r.consumed + 7) / 8;                          // align()
     if (n - p < 8) return SWC_GZIP_WRONG_MAGIC;
-    const uint32_t crc = rd32(in + p), isize = rd32(in + p + 4);
+    const uint32_t crc = le32(in + p), isize = le32(in + p + 4);
     p += 8;
     if ((uint32_t)r.out_len != isize) return SWC_GZIP_WRONG_ISIZE;
     u64 got = 0;
@@ -243,8 +169,7 @@ int gzip_multi_batch(const uint8_t *in, size_t n, const u8 *d_in, HostOut &o, st
     while (idx < pos.size() && pos[idx] == *off && !*stop) {
         // ---- one round: candidates idx.. while the speculative outputs fit the budget
         std::vector<Cand> cs;
-        std::vector<u64> h_inoff, h_inlen, h_outoff, h_outcap;
-        size_t out_total = 0;
+        size_t nu = 0, out_total = 0;
         for (size_t k = idx; k < pos.size() && cs.size() < (1u << 22); k++) {
             Cand c;
             c.at = pos[k]; c.next = k + 1 < pos.size() ? pos[k + 1] : n; c.unit = -1; c.crc = c.isize = 0;
@@ -252,77 +177,75 @@ int gzip_multi_batch(const uint8_t *in, size_t n, const u8 *d_in, HostOut &o, st
             const bool hdr_ok = gzip_header(in, c.next, &d) == SWC_OK;   // a real header never reaches the next member
             c.dstart = d;
             if (hdr_ok && c.next >= d + 8) {
-                c.crc = rd32(in + c.next - 8); c.isize = rd32(in + c.next - 4);
-                const size_t span = c.next - 8 - d;
-                if ((u64)c.isize <= (u64)span * 1032 + 64) {            // Deflate cannot expand further than ~1032:1
+                c.crc = le32(in + c.next - 8); c.isize = le32(in + c.next - 4);
+                if ((u64)c.isize <= (u64)(c.next - 8 - d) * 1032 + 64) {    // Deflate cannot expand further than ~1032:1
                     const size_t cap16 = round16((size_t)c.isize);
                     if (out_total + cap16 > budget && !cs.empty()) break;
-                    c.unit = (long)h_inoff.size();
-                    h_inoff.push_back(d); h_inlen.push_back(span);
-                    h_outoff.push_back(out_total); h_outcap.push_back(c.isize);
+                    c.unit = (long)nu++;
                     out_total += cap16;
                 }
             }
             cs.push_back(c);
         }
-        const size_t nu = h_inoff.size();
-        std::vector<u64> h_outlen(nu), h_cons(nu);
-        std::vector<int32_t> h_status(nu);
-        std::vector<uint32_t> h_crc(nu);
-        DevBuf meta, d_out;
-        u64 *m = nullptr;
+        UnitTable t;
+        UnitCols uc(t, nu);
+        const Col<uint32_t> crc = t.out<uint32_t>(nu);
+        u64 *h_outoff = t.host(uc.out_off);
+        for (size_t k = 0, run = 0; k < cs.size(); k++) {
+            const Cand &c = cs[k];
+            if (c.unit < 0) continue;
+            t.host(uc.in_off)[c.unit] = c.dstart; t.host(uc.in_len)[c.unit] = c.next - 8 - c.dstart;
+            h_outoff[c.unit] = run; t.host(uc.out_cap)[c.unit] = c.isize;
+            run += round16((size_t)c.isize);
+        }
+        std::vector<u64> h_outlen, h_cons;
+        std::vector<int32_t> h_status;
+        std::vector<uint32_t> h_crc;
+        DevBuf d_out;
         if (nu) {
             // an allocation failure is not an error of the archive: hand the rest to the caller's sequential walk
-            int st = meta.alloc(nu * 64);                               // 7 u64 arrays + status + crc
-            if (st) return SWC_OK;
-            if ((st = d_out.alloc(out_total + 64))) return SWC_OK;
+            if (t.alloc()) return SWC_OK;
+            if (d_out.alloc(out_total + 64)) return SWC_OK;
             { void *scr = nullptr; if (scratch_get(inflate_scratch_bytes(nu, out_total), &scr, stream)) return SWC_OK; }
-            m = meta.as<u64>();
-            SWC_CUDA_TRY(cudaMemcpyAsync(m, h_inoff.data(), nu * 8, cudaMemcpyHostToDevice, stream));
-            SWC_CUDA_TRY(cudaMemcpyAsync(m + nu, h_inlen.data(), nu * 8, cudaMemcpyHostToDevice, stream));
-            SWC_CUDA_TRY(cudaMemcpyAsync(m + 2 * nu, h_outoff.data(), nu * 8, cudaMemcpyHostToDevice, stream));
-            SWC_CUDA_TRY(cudaMemcpyAsync(m + 3 * nu, h_outcap.data(), nu * 8, cudaMemcpyHostToDevice, stream));
-            int32_t *d_status = (int32_t *)(m + 7 * nu);
-            uint32_t *d_crc = (uint32_t *)(d_status + nu);
-            if ((st = deflate_batch_impl(d_in, m, m + nu, nullptr, d_out.as<u8>(), m + 2 * nu, m + 3 * nu, out_total,
-                                         m + 4 * nu, m + 5 * nu, d_status, nu, nullptr, 0, stream))) return st;
-            if ((st = checks::crc32_units(d_out.as<u8>(), m + 2 * nu, m + 4 * nu, d_status, d_crc, nu, stream))) return st;
-            SWC_CUDA_TRY(cudaMemcpyAsync(h_outlen.data(), m + 4 * nu, nu * 8, cudaMemcpyDeviceToHost, stream));
-            SWC_CUDA_TRY(cudaMemcpyAsync(h_cons.data(), m + 5 * nu, nu * 8, cudaMemcpyDeviceToHost, stream));
-            SWC_CUDA_TRY(cudaMemcpyAsync(h_status.data(), d_status, nu * 4, cudaMemcpyDeviceToHost, stream));
-            SWC_CUDA_TRY(cudaMemcpyAsync(h_crc.data(), d_crc, nu * 4, cudaMemcpyDeviceToHost, stream));
-            SWC_CUDA_TRY(cudaStreamSynchronize(stream));
+            int st = t.upload(stream);
+            if (st) return st;
+            if ((st = deflate_batch_impl(d_in, t.dev(uc.in_off), t.dev(uc.in_len), nullptr, d_out.as<u8>(), t.dev(uc.out_off), t.dev(uc.out_cap),
+                                         out_total, t.dev(uc.out_len), t.dev(uc.consumed), t.dev(uc.status), nu, nullptr, 0, stream))) return st;
+            if ((st = checks::crc32_units(d_out.as<u8>(), t.dev(uc.out_off), t.dev(uc.out_len), t.dev(uc.status), t.dev(crc), nu, stream))) return st;
+            if ((st = t.fetch(uc.out_len, h_outlen, stream)) || (st = t.fetch(uc.consumed, h_cons, stream)) ||
+                (st = t.fetch(uc.status, h_status, stream)) || (st = t.fetch(crc, h_crc, stream))) return st;
         }
         if (trace) fprintf(stderr, "[swc] gzip round: %zu units, %.1f MB out, decode+crc done at %.1f ms\n", nu, out_total / 1e6, now() - t0);
         // ---- the in-order walk: accept the longest validated prefix
-        std::vector<u64> g_src, g_len, g_dst;
-        size_t acc_bytes = 0, k = 0;
-        for (; k < cs.size(); k++) {
-            const Cand &c = cs[k];
+        size_t accepted = 0;
+        for (; accepted < cs.size(); accepted++) {
+            const Cand &c = cs[accepted];
             if (c.unit < 0) break;
             const size_t u = (size_t)c.unit;
             if (h_status[u] != SWC_OK || c.dstart + (h_cons[u] + 7) / 8 + 8 != c.next || h_outlen[u] != c.isize) break;
-            g_src.push_back(h_outoff[u]); g_len.push_back(h_outlen[u]); g_dst.push_back(acc_bytes);
-            acc_bytes += h_outlen[u];
-            if (h_crc[u] != c.crc) { *result = SWC_GZIP_WRONG_CRC; *stop = true; k++; break; }   // the member is still returned
+            if (h_crc[u] != c.crc) { *result = SWC_GZIP_WRONG_CRC; *stop = true; accepted++; break; }   // the member is still returned
         }
-        const size_t accepted = g_src.size();
         if (accepted) {
-            DevBuf gm, d_g;
-            int st = gm.alloc(accepted * 24);
-            if (st) return SWC_OK;
-            if ((st = d_g.alloc(acc_bytes + 16))) return SWC_OK;
-            u64 *g = gm.as<u64>();
-            SWC_CUDA_TRY(cudaMemcpyAsync(g, g_src.data(), accepted * 8, cudaMemcpyHostToDevice, stream));
-            SWC_CUDA_TRY(cudaMemcpyAsync(g + accepted, g_len.data(), accepted * 8, cudaMemcpyHostToDevice, stream));
-            SWC_CUDA_TRY(cudaMemcpyAsync(g + 2 * accepted, g_dst.data(), accepted * 8, cudaMemcpyHostToDevice, stream));
-            if ((st = checks::gather_units(d_out.as<u8>(), g, g + accepted, d_g.as<u8>(), g + 2 * accepted, accepted, stream))) return st;
+            UnitTable g;
+            const Col<u64> src = g.in<u64>(accepted), len = g.in<u64>(accepted), dst = g.in<u64>(accepted);
+            size_t acc_bytes = 0;
+            for (size_t i = 0; i < accepted; i++) {
+                const size_t u = (size_t)cs[i].unit;
+                g.host(src)[i] = h_outoff[u]; g.host(len)[i] = h_outlen[u]; g.host(dst)[i] = acc_bytes;
+                acc_bytes += h_outlen[u];
+            }
+            DevBuf d_g;
+            if (g.alloc()) return SWC_OK;
+            if (d_g.alloc(acc_bytes + 16)) return SWC_OK;
+            int st = g.upload(stream);
+            if (st) return st;
+            if ((st = checks::gather_units(d_out.as<u8>(), g.dev(src), g.dev(len), d_g.as<u8>(), g.dev(dst), accepted, stream))) return st;
             const size_t base = o.len;
-            uint8_t *dst = o.grow(acc_bytes);
-            if (!dst) return SWC_ERR_OUTPUT_OVERFLOW;
+            uint8_t *out = o.grow(acc_bytes);
+            if (!out) return SWC_ERR_OUTPUT_OVERFLOW;
             SWC_CUDA_TRY(cudaStreamSynchronize(stream));
-            if ((st = copy_pageable(dst, d_g.p, acc_bytes, false))) return st;
-            for (size_t i = 0; i < accepted; i++) { ends.push_back(base + g_dst[i] + g_len[i]); starts.push_back(cs[i].at); }
+            if ((st = copy_pageable(out, d_g.p, acc_bytes, false))) return st;
+            for (size_t i = 0; i < accepted; i++) { ends.push_back(base + g.host(dst)[i] + g.host(len)[i]); starts.push_back(cs[i].at); }
             *off = cs[accepted - 1].next;
             if (trace) fprintf(stderr, "[swc] gzip round: %zu accepted, gathered + copied back at %.1f ms\n", accepted, now() - t0);
         }
@@ -341,18 +264,12 @@ int gzip_multi_batch(const uint8_t *in, size_t n, const u8 *d_in, HostOut &o, st
     return SWC_OK;
 }
 
-int upload(DevBuf &d, const uint8_t *in, size_t n) {
-    int st = d.alloc(round16(n) + 32);
-    if (st) return st;
-    return copy_pageable(d.p, in, n, true);
-}
-
 template <typename F>
 int host_check(const uint8_t *in, size_t n, F fn) {
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
     DevBuf d;
-    int st = upload(d, in, n);
+    int st = upload_input(d, in, n);
     if (st) return st;
     return fn(d.as<u8>());
 }
@@ -368,7 +285,7 @@ int32_t swc_gzip_unarchive(const uint8_t *in, size_t in_len, uint8_t **out, size
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
     DevBuf d_in;
-    int st = upload(d_in, in, in_len);
+    int st = upload_input(d_in, in, in_len);
     if (st) return st;
     HostOut o;
     size_t off = 0; bool crc_error = false;
@@ -387,7 +304,7 @@ static int gzip_multi(const uint8_t *in, size_t in_len, uint8_t **out, size_t *o
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
     DevBuf d_in;
-    int st = upload(d_in, in, in_len);
+    int st = upload_input(d_in, in, in_len);
     if (st) return st;
     HostOut o;
     std::vector<size_t> ends, starts;
@@ -402,13 +319,10 @@ static int gzip_multi(const uint8_t *in, size_t in_len, uint8_t **out, size_t *o
         ends.push_back(o.len); starts.push_back(member_at);
         if (crc_error) { result = SWC_GZIP_WRONG_CRC; break; }
     }
-    if ((st = o.release_to(out, out_len))) return st;
-    *member_ends = (size_t *)swc_alloc(sizeof(size_t) * (ends.size() + 1));
-    for (size_t i = 0; i < ends.size(); i++) (*member_ends)[i] = ends[i];
+    if ((st = o.release_to(out, out_len)) || (st = give_sizes(ends, member_ends, out, out_len))) return st;
     if (member_in_off) {
-        *member_in_off = (size_t *)swc_alloc(sizeof(size_t) * (starts.size() + 1));
-        for (size_t i = 0; i < starts.size(); i++) (*member_in_off)[i] = starts[i];
-        (*member_in_off)[starts.size()] = off;
+        starts.push_back(off);                                           // one past the last member
+        if ((st = give_sizes(starts, member_in_off, out, out_len))) { swc_free(*member_ends); *member_ends = nullptr; return st; }
     }
     *n_members = ends.size();
     return result;
@@ -445,7 +359,7 @@ int32_t swc_zlib_unarchive(const uint8_t *in, size_t n, uint8_t **out, size_t *o
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
     DevBuf d_in;
-    int st = upload(d_in, in, n);
+    int st = upload_input(d_in, in, n);
     if (st) return st;
     UnitResult r;
     if ((st = deflate_unit_device(d_in.as<u8>(), n, off * 8, r))) return st;

@@ -303,17 +303,21 @@ int32_t swc_zip_open(const uint8_t *in, size_t in_len, uint8_t **out, size_t *ou
         out_total += round16((size_t)cap) + 16;
         grp[g].push_back(u);
     }
-    DevBuf d_in, d_out, d_meta;
-    if ((st = d_in.alloc(round16(in_len) + 256))) return st;
-    if ((st = copy_pageable(d_in.p, in, in_len, true))) return st;
+    DevBuf d_in, d_out;
+    if ((st = upload_input(d_in, in, in_len))) return st;
     if ((st = d_out.alloc((size_t)out_total + 64))) return st;
     const size_t nu = grp[0].size() + grp[1].size() + grp[2].size() + grp[3].size();
-    // per unit: in_off, in_len, out_off, cap, out_len, consumed (u64) | status, crc (u32) | props (u32) | dict, usize (i64)
-    const size_t row = 8 * 6 + 4 * 3 + 8 * 2 + 4;
-    if ((st = d_meta.alloc(nu * row + 256))) return st;
-    std::vector<uint64_t> h_tab(nu * 6, 0);
-    std::vector<uint32_t> h_props(nu, 0);
-    std::vector<int64_t> h_dict(nu, 0), h_usize(nu, 0);
+    // stored units are copies: their length, consumed bytes and (zero) status are filled in here
+    UnitTable t;
+    const Col<u64> in_off = t.in<u64>(nu), in_len_c = t.in<u64>(nu), out_off = t.in<u64>(nu), cap = t.in<u64>(nu);
+    const Col<u64> got_len = t.in<u64>(nu), consumed = t.in<u64>(nu);
+    const Col<int32_t> status = t.in<int32_t>(nu);
+    const Col<uint32_t> props = t.in<uint32_t>(nu);
+    const Col<int64_t> dict = t.in<int64_t>(nu), usize = t.in<int64_t>(nu);
+    const Col<uint32_t> crc = t.out<uint32_t>(nu);
+    if ((st = t.alloc())) return st;
+    int64_t *h_dict = t.host(dict);
+    const u64 *h_out_off = t.host(out_off);
     std::vector<size_t> unit_of_item(n, (size_t)-1);
     size_t base[5] = {0, grp[0].size(), 0, 0, 0};
     base[2] = base[1] + grp[1].size(); base[3] = base[2] + grp[2].size(); base[4] = base[3] + grp[3].size();
@@ -322,51 +326,36 @@ int32_t swc_zip_open(const uint8_t *in, size_t in_len, uint8_t **out, size_t *ou
             const Unit &u = grp[g][k];
             const size_t j = base[g] + k;
             unit_of_item[u.item] = j;
-            h_tab[j] = u.in_off; h_tab[nu + j] = u.in_len; h_tab[2 * nu + j] = u.out_off; h_tab[3 * nu + j] = u.cap;
-            if (g == 0) { h_tab[4 * nu + j] = u.cap; h_tab[5 * nu + j] = u.cap; }        // stored: length and consumed are the size
+            t.host(in_off)[j] = u.in_off; t.host(in_len_c)[j] = u.in_len; t.host(out_off)[j] = u.out_off; t.host(cap)[j] = u.cap;
+            if (g == 0) { t.host(got_len)[j] = u.cap; t.host(consumed)[j] = u.cap; }      // stored: length and consumed are the size
             if (g == 3) {
                 const uint8_t *p = in + items[u.item].data_off;
                 const unsigned b = p[4];
-                h_props[j] = (b % 9) | (((b / 9) % 5) << 8) | (((b / 9) / 5) << 16);    // LZMAProperties.swift:49-58
+                t.host(props)[j] = (b % 9) | (((b / 9) % 5) << 8) | (((b / 9) / 5) << 16);    // LZMAProperties.swift:49-58
                 h_dict[j] = (int64_t)p[5] | (int64_t)p[6] << 8 | (int64_t)p[7] << 16 | (int64_t)p[8] << 24;
-                h_usize[j] = (int64_t)items[u.item].uncomp;
+                t.host(usize)[j] = (int64_t)items[u.item].uncomp;
             }
         }
-    u64 *m = d_meta.as<u64>();
-    int32_t *d_status = (int32_t *)(m + 6 * nu);
-    uint32_t *d_crc = (uint32_t *)(d_status + nu), *d_props = d_crc + nu;
-    int64_t *d_dict = (int64_t *)(((uintptr_t)(d_props + nu) + 7) & ~(uintptr_t)7), *d_usize = d_dict + nu;
     cudaStream_t s = 0;
-    if (nu) {
-        SWC_CUDA_TRY(cudaMemcpyAsync(m, h_tab.data(), nu * 48, cudaMemcpyHostToDevice, s));
-        SWC_CUDA_TRY(cudaMemsetAsync(d_status, 0, nu * 4, s));
-        SWC_CUDA_TRY(cudaMemcpyAsync(d_props, h_props.data(), nu * 4, cudaMemcpyHostToDevice, s));
-        SWC_CUDA_TRY(cudaMemcpyAsync(d_dict, h_dict.data(), nu * 8, cudaMemcpyHostToDevice, s));
-        SWC_CUDA_TRY(cudaMemcpyAsync(d_usize, h_usize.data(), nu * 8, cudaMemcpyHostToDevice, s));
-    }
+    if (nu && (st = t.upload(s))) return st;
     for (const Unit &u : grp[0])
         if (u.cap) SWC_CUDA_TRY(cudaMemcpyAsync(d_out.as<u8>() + u.out_off, d_in.as<u8>() + u.in_off, (size_t)u.cap, cudaMemcpyDeviceToDevice, s));
-    auto col = [&](int c, int g) { return m + (size_t)c * nu + base[g]; };
+    auto at = [&](auto c, int g) { return t.dev(c) + base[g]; };     // the columns of method group g
     if (!grp[1].empty() &&
-        (st = swc_deflate_decompress_batch(d_in.as<u8>(), col(0, 1), col(1, 1), nullptr, d_out.as<u8>(), col(2, 1), col(3, 1), out_total,
-                                           col(4, 1), col(5, 1), d_status + base[1], grp[1].size(), nullptr, 0, s))) return st;
+        (st = swc_deflate_decompress_batch(d_in.as<u8>(), at(in_off, 1), at(in_len_c, 1), nullptr, d_out.as<u8>(), at(out_off, 1), at(cap, 1),
+                                           out_total, at(got_len, 1), at(consumed, 1), at(status, 1), grp[1].size(), nullptr, 0, s))) return st;
     if (!grp[2].empty() &&
-        (st = swc_bzip2_decompress_batch(d_in.as<u8>(), col(0, 2), col(1, 2), d_out.as<u8>(), col(2, 2), col(3, 2), col(4, 2), col(5, 2),
-                                         d_status + base[2], grp[2].size(), s))) return st;
+        (st = swc_bzip2_decompress_batch(d_in.as<u8>(), at(in_off, 2), at(in_len_c, 2), d_out.as<u8>(), at(out_off, 2), at(cap, 2),
+                                         at(got_len, 2), at(consumed, 2), at(status, 2), grp[2].size(), s))) return st;
     if (!grp[3].empty() &&
-        (st = swc_lzma_decompress_batch(d_in.as<u8>(), col(0, 3), col(1, 3), d_props + base[3], d_dict + base[3], d_usize + base[3], d_out.as<u8>(),
-                                        col(2, 3), col(3, 3), col(4, 3), col(5, 3), d_status + base[3], grp[3].size(), s))) return st;
-    if (nu && (st = swc_crc32_batch(d_out.as<u8>(), m + 2 * nu, m + 4 * nu, d_status, d_crc, nu, s))) return st;
-    std::vector<uint64_t> r_len(nu), r_used(nu);
-    std::vector<int32_t> r_st(nu);
-    std::vector<uint32_t> r_crc(nu);
-    if (nu) {
-        SWC_CUDA_TRY(cudaMemcpyAsync(r_len.data(), m + 4 * nu, nu * 8, cudaMemcpyDeviceToHost, s));
-        SWC_CUDA_TRY(cudaMemcpyAsync(r_used.data(), m + 5 * nu, nu * 8, cudaMemcpyDeviceToHost, s));
-        SWC_CUDA_TRY(cudaMemcpyAsync(r_st.data(), d_status, nu * 4, cudaMemcpyDeviceToHost, s));
-        SWC_CUDA_TRY(cudaMemcpyAsync(r_crc.data(), d_crc, nu * 4, cudaMemcpyDeviceToHost, s));
-    }
-    SWC_CUDA_TRY(cudaStreamSynchronize(s));
+        (st = swc_lzma_decompress_batch(d_in.as<u8>(), at(in_off, 3), at(in_len_c, 3), at(props, 3), at(dict, 3), at(usize, 3), d_out.as<u8>(),
+                                        at(out_off, 3), at(cap, 3), at(got_len, 3), at(consumed, 3), at(status, 3), grp[3].size(), s))) return st;
+    if (nu && (st = swc_crc32_batch(d_out.as<u8>(), t.dev(out_off), t.dev(got_len), t.dev(status), t.dev(crc), nu, s))) return st;
+    std::vector<uint64_t> r_len, r_used;
+    std::vector<int32_t> r_st;
+    std::vector<uint32_t> r_crc;
+    if ((st = t.fetch(got_len, r_len, s)) || (st = t.fetch(consumed, r_used, s)) || (st = t.fetch(status, r_st, s)) ||
+        (st = t.fetch(crc, r_crc, s))) return st;
     // ---- the reference's loop over the entries (ZipContainer.swift:46-57), now only checking ----
     View v{in, in_len};
     int result = SWC_OK;
@@ -436,7 +425,7 @@ int32_t swc_zip_open(const uint8_t *in, size_t in_len, uint8_t **out, size_t *ou
             es[i].data_off = tail; es[i].data_len = redone[i].second;
             tail += round16(redone[i].second);
         } else {
-            es[i].data_off = h_tab[2 * nu + unit_of_item[i]];
+            es[i].data_off = h_out_off[unit_of_item[i]];
         }
     }
     free_redone();

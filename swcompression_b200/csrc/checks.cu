@@ -9,6 +9,7 @@
 #include <algorithm>
 #include <vector>
 #include "checks.cuh"
+#include "host_util.h"
 
 namespace swc {
 namespace checks {
@@ -417,6 +418,35 @@ int sha256(const u8 *d, u64 n, u8 *d_digest, cudaStream_t s) {
     sha256_kernel<<<1, 1, 0, s>>>(d, n, d_digest);
     count_launch();
     SWC_CUDA_TRY(cudaGetLastError());
+    return SWC_OK;
+}
+
+// ---- host convenience ----
+int check_device(Kind k, const u8 *d, u64 n, u64 *value) {
+    DevBuf res, part;
+    int st;
+    {   // result slot + chunk partials live in a grow-only arena: per-block checks of big archives do no cudaMalloc
+        void *a = nullptr;
+        if ((st = arena_get(3, 64 + partial_bytes(n), &a, 0))) return st;
+        res.borrow(a, 32);
+        part.borrow((u8 *)a + 64, partial_bytes(n));
+    }
+    if (k == XXH32) {
+        SWC_CUDA_TRY(cudaMemcpy(res.p, &n, 8, cudaMemcpyHostToDevice));
+        if ((st = xxh32_batch(d, nullptr, res.as<u64>(), (u32 *)(res.as<u8>() + 8), 1, 0))) return st;
+        u32 v = 0;
+        SWC_CUDA_TRY(cudaMemcpy(&v, res.as<u8>() + 8, 4, cudaMemcpyDeviceToHost));
+        *value = v;
+        return SWC_OK;
+    }
+    switch (k) {
+    case CRC32: st = crc32(d, n, res.as<u64>(), part.as<u64>(), 0); break;
+    case BZIP2_CRC32: st = bzip2_crc32(d, n, res.as<u64>(), part.as<u64>(), 0); break;
+    case CRC64: st = crc64(d, n, res.as<u64>(), part.as<u64>(), 0); break;
+    default: st = adler32(d, n, res.as<u64>(), part.as<u64>(), 0); break;
+    }
+    if (st) return st;
+    SWC_CUDA_TRY(cudaMemcpy(value, res.p, 8, cudaMemcpyDeviceToHost));
     return SWC_OK;
 }
 

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stddef.h>
 #include <stdint.h>
+#include <stdlib.h>
 #include <vector>
 #include "common.cuh"
 
@@ -70,6 +71,50 @@ struct DevBuf {
     template <typename T> T *as() const { return (T *)p; }
 };
 
+inline size_t round16(size_t v) { return (v + 15) & ~(size_t)15; }
+
+// ---- unit tables: the per-unit metadata of one batch, as typed columns in one device allocation ----
+// Declare every column first, then seat the table with alloc() (its own cudaMalloc) or place() (memory the caller owns);
+// host() pointers stay valid from the last declaration on.  in<T>() columns have a zero-filled host side that upload()
+// sends in one copy; out<T>() columns exist on the device only (kernel results, or filled by the caller's own copies).
+// Every column starts on a 256-byte boundary, so a column never overlaps its neighbour whatever its type and length.
+template <typename T> struct Col { size_t off = 0, n = 0; bool dev_only = false; };
+class UnitTable {
+  public:
+    template <typename T> Col<T> in(size_t n) { Col<T> c{host_.size(), n, false}; host_.resize(host_.size() + span(n * sizeof(T))); return c; }
+    template <typename T> Col<T> out(size_t n) { Col<T> c{out_bytes_, n, true}; out_bytes_ += span(n * sizeof(T)); return c; }
+    template <typename T> T *host(Col<T> c) { return (T *)(host_.data() + c.off); }
+    template <typename T> T *dev(Col<T> c) const { return (T *)(dev_.as<u8>() + (c.dev_only ? host_.size() : 0) + c.off); }
+    size_t bytes() const { return host_.size() + out_bytes_; }
+    int alloc() { return dev_.alloc(bytes()); }
+    void place(void *p) { dev_.borrow(p, bytes()); }
+    int upload(cudaStream_t s = 0) {
+        if (!host_.empty()) SWC_CUDA_TRY(cudaMemcpyAsync(dev_.p, host_.data(), host_.size(), cudaMemcpyHostToDevice, s));
+        return SWC_OK;
+    }
+    // one column back into `v` (blocking: waits for `s`)
+    template <typename T> int fetch(Col<T> c, std::vector<T> &v, cudaStream_t s = 0) const {
+        v.resize(c.n);
+        if (c.n) SWC_CUDA_TRY(cudaMemcpyAsync(v.data(), dev(c), c.n * sizeof(T), cudaMemcpyDeviceToHost, s));
+        SWC_CUDA_TRY(cudaStreamSynchronize(s));
+        return SWC_OK;
+    }
+  private:
+    static size_t span(size_t b) { return (b + 255) & ~(size_t)255; }
+    std::vector<u8> host_;
+    size_t out_bytes_ = 0;
+    DevBuf dev_;
+};
+
+// the columns every batched decoder takes: the unit's input and output regions in, its results out
+struct UnitCols {
+    Col<u64> in_off, in_len, out_off, out_cap, out_len, consumed;
+    Col<int32_t> status;
+    UnitCols(UnitTable &t, size_t n)
+        : in_off(t.in<u64>(n)), in_len(t.in<u64>(n)), out_off(t.in<u64>(n)), out_cap(t.in<u64>(n)),
+          out_len(t.out<u64>(n)), consumed(t.out<u64>(n)), status(t.out<int32_t>(n)) {}
+};
+
 // result of decoding ONE unit that is already resident on the device
 struct UnitResult {
     DevBuf out;            // decoded bytes (device)
@@ -77,6 +122,33 @@ struct UnitResult {
     size_t consumed = 0;   // bits (Deflate/BZip2) or bytes (LZ4/LZMA)
     int status = 0;
 };
+
+// Decodes the unit d_in[start, in_len) described by the 1-unit table `t` / `c` (the codec's own columns already declared
+// and filled) into r.out, growing the output until it fits: `cap` bytes first, then, while the unit overflows and
+// `attempts` last, grow(cap, reported out_len) bytes — 0 stops.  launch(out, cap) runs the codec on the table.
+template <typename Grow, typename Launch>
+int decode_unit(UnitTable &t, const UnitCols &c, size_t start, size_t in_len, size_t cap, int attempts, Grow grow,
+                Launch launch, UnitResult &r) {
+    int st = t.alloc();
+    if (st) return st;
+    *t.host(c.in_off) = start;
+    *t.host(c.in_len) = in_len - start;
+    for (int attempt = 0; attempt < attempts; attempt++) {
+        cap = round16(cap);
+        if ((st = r.out.alloc(cap))) return st;
+        *t.host(c.out_cap) = cap;
+        if ((st = t.upload())) return st;
+        if ((st = launch(r.out.as<u8>(), cap))) return st;
+        std::vector<u64> len, used;
+        std::vector<int32_t> status;
+        if ((st = t.fetch(c.out_len, len)) || (st = t.fetch(c.consumed, used)) || (st = t.fetch(c.status, status))) return st;
+        r.out_len = (size_t)len[0];
+        r.consumed = (size_t)used[0];
+        r.status = status[0];
+        if (r.status != SWC_ERR_OUTPUT_OVERFLOW || !(cap = grow(cap, r.out_len))) break;
+    }
+    return SWC_OK;
+}
 
 // Deflate stream starting at byte `start` + `start_bit` bits inside d_in[0..in_len)
 int deflate_unit_device(const u8 *d_in, size_t in_len, size_t start_bit_abs, UnitResult &r, size_t hint = 0);
@@ -87,12 +159,66 @@ int deflate_batch_impl(const uint8_t *in_base, const uint64_t *in_off, const uin
                        uint64_t *out_len, uint64_t *consumed_bits, int32_t *status, uint64_t n,
                        void *scratch, size_t scratch_bytes, cudaStream_t stream);
 
-inline size_t round16(size_t v) { return (v + 15) & ~(size_t)15; }
-
 // large transfers between pageable host memory and the device: T threads x (stream + two pinned bounce buffers) (runtime.cu)
 int copy_pageable(void *dst, const void *src, size_t bytes, bool to_device);
 
+// the caller's input on the device, with 256 bytes of slack behind it for the decoders' wide loads
+int upload_input(DevBuf &d, const uint8_t *in, size_t n);
+
 // hand a device buffer back to a C caller as swc_alloc'ed host memory
 int to_host_alloc(const void *d, size_t n, uint8_t **out, size_t *out_len);
+
+// growable malloc'ed host buffer that is handed to the C caller without another copy (swc_free == free)
+struct HostOut {
+    uint8_t *p = nullptr;
+    size_t len = 0, cap = 0;
+    HostOut() {}
+    HostOut(const HostOut &) = delete;
+    HostOut &operator=(const HostOut &) = delete;
+    ~HostOut() { free(p); }
+    uint8_t *grow(size_t add) {                                     // nullptr when out of memory
+        if (len + add > cap || !p) {
+            size_t nc = cap * 2 > len + add ? cap * 2 : len + add;
+            if (nc < 64) nc = 64;
+            uint8_t *q = (uint8_t *)realloc(p, nc);
+            if (!q) return nullptr;
+            p = q; cap = nc;
+        }
+        uint8_t *r = p + len;
+        len += add;
+        return r;
+    }
+    int release_to(uint8_t **out, size_t *out_len) {
+        if (!p && !grow(0)) return SWC_ERR_OUTPUT_OVERFLOW;
+        *out = p; *out_len = len;
+        p = nullptr; len = cap = 0;
+        return SWC_OK;
+    }
+};
+
+// Hands `v` to a C caller as an swc_alloc'ed array.  When that allocation fails, the bytes this call already handed out
+// (*out) are freed again and the call returns SWC_ERR_OUTPUT_OVERFLOW.
+int give_sizes(const std::vector<size_t> &v, size_t **dst, uint8_t **out, size_t *out_len);
+
+// checks shared by the *_batch_host calls: every unit lies inside the two host arenas (overflow-safe) and every output
+// region is 16-byte aligned; *monotone tells whether the units follow each other on both sides
+int check_host_units(const uint64_t *in_off, const uint64_t *in_len, uint64_t in_total, const uint64_t *out_off,
+                     const uint64_t *out_cap, uint64_t out_total, uint64_t n, bool *monotone);
+// copies the output regions of units [b, e) from d_out back to out_base — only those: the caller's bytes between and
+// around them are not ours to overwrite (regions that touch are merged, so densely packed units are one copy)
+int copy_back_regions(uint8_t *out_base, const u8 *d_out, const uint64_t *out_off, const uint64_t *out_cap, uint64_t b,
+                      uint64_t e, cudaStream_t s);
+
+// ---- container framing (a few bytes per header / block mark) read on the host ----
+inline uint32_t le32(const uint8_t *p) { return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24; }
+// bitwise CRC-32 of header / index / footer fields; payload CRCs run on the device
+inline uint32_t crc32_framing(const uint8_t *p, size_t n) {
+    uint32_t c = 0xFFFFFFFFu;
+    for (size_t i = 0; i < n; i++) {
+        c ^= p[i];
+        for (int k = 0; k < 8; k++) c = (c & 1) ? 0xEDB88320u ^ (c >> 1) : c >> 1;
+    }
+    return ~c;
+}
 
 }  // namespace swc

@@ -250,6 +250,13 @@ lz_resolve_kernel(BatchArgs a) {
 }
 
 // ------------------------------------------------------------------------------------------------ host
+void seat_scratch(BatchArgs &a, void *scratch, u64 n, u64 first, int tickets, int ticket) {
+    u8 *s = (u8 *)scratch;
+    a.ticket = (unsigned long long *)(s + (size_t)256 * ticket);
+    a.rec_count = (u32 *)(s + (size_t)256 * tickets) + first;
+    a.rec_base = (u32 *)(s + scratch_header(n, tickets));
+}
+
 int launch(const BatchArgs &a, cudaStream_t stream) {
     if (a.n == 0) return SWC_OK;
     // Huffman stage.

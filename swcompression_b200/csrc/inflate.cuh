@@ -43,9 +43,13 @@ struct BatchArgs {
 // word lies below the records; only the last, partial word of a unit with fewer than 8 literals (and records for almost
 // all of its bytes) may find no room: such a unit goes to inflate_slow_kernel (SWC_INTERNAL_NEEDS_SLOW).
 __host__ __device__ __forceinline__ u64 rec_start(u64 out_off) { return out_off / 3; }
-inline size_t scratch_bytes(u64 n, u64 out_capacity_total) {
+// Scratch layout: `tickets` ticket blocks of 256 bytes, rec_count[n] rounded up to 256 bytes, then the record words.
+inline size_t scratch_header(u64 n, int tickets) { return (size_t)256 * tickets + ((n * 4 + 255) & ~(size_t)255); }
+inline size_t scratch_bytes(u64 n, u64 out_capacity_total) {           // one ticket block
     return (size_t)((out_capacity_total / 3 + 2) * 4 + n * 4 + 1024);
 }
+// seats a.ticket (block `ticket` of `tickets`), a.rec_count (entries first .. first + a.n of the n-unit table) and a.rec_base
+void seat_scratch(BatchArgs &a, void *scratch, u64 n, u64 first, int tickets, int ticket);
 // bytes of the scratch region of a unit
 __device__ __forceinline__ u64 region_bytes(u64 out_off, u64 cap) { return (rec_start(out_off + cap) - rec_start(out_off)) * 4; }
 

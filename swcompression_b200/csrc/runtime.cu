@@ -1,4 +1,5 @@
-// runtime.cu — library plumbing: error text, launch counter, host/pinned allocators, scratch pool, status names.
+// runtime.cu — library plumbing: error text, launch counter, host/pinned allocators, scratch pool, host <-> device hand-off
+// helpers of the C-ABI files, status names.
 #include <algorithm>
 #include <cstring>
 #include <mutex>
@@ -131,6 +132,58 @@ int copy_pageable(void *dst, const void *src, size_t bytes, bool to_device) {
     }
     for (auto &x : th) x.join();
     if (err) return cuda_fail(cudaGetLastError(), "copy_pageable");
+    return SWC_OK;
+}
+
+int upload_input(DevBuf &d, const uint8_t *in, size_t n) {
+    int st = d.alloc(round16(n) + 256);
+    if (st) return st;
+    return copy_pageable(d.p, in, n, true);
+}
+
+int to_host_alloc(const void *d, size_t n, uint8_t **out, size_t *out_len) {
+    uint8_t *h = (uint8_t *)swc_alloc(n);
+    if (!h) return SWC_ERR_OUTPUT_OVERFLOW;
+    if (n) {
+        int st = copy_pageable(h, d, n, false);
+        if (st) { swc_free(h); return st; }
+    }
+    *out = h;
+    *out_len = n;
+    return SWC_OK;
+}
+
+int give_sizes(const std::vector<size_t> &v, size_t **dst, uint8_t **out, size_t *out_len) {
+    *dst = (size_t *)swc_alloc(sizeof(size_t) * (v.size() + 1));
+    if (!*dst) {
+        swc_free(*out);
+        *out = nullptr; *out_len = 0;
+        return SWC_ERR_OUTPUT_OVERFLOW;
+    }
+    if (!v.empty()) memcpy(*dst, v.data(), sizeof(size_t) * v.size());
+    return SWC_OK;
+}
+
+int check_host_units(const uint64_t *in_off, const uint64_t *in_len, uint64_t in_total, const uint64_t *out_off,
+                     const uint64_t *out_cap, uint64_t out_total, uint64_t n, bool *monotone) {
+    *monotone = true;
+    for (uint64_t i = 0; i < n; i++) {
+        if (in_off[i] > in_total || in_len[i] > in_total - in_off[i] || out_off[i] > out_total || out_cap[i] > out_total - out_off[i])
+            return SWC_ERR_INVALID_ARG;
+        if (out_off[i] & 15) return SWC_ERR_INVALID_ARG;
+        if (i && (in_off[i] < in_off[i - 1] + in_len[i - 1] || out_off[i] < out_off[i - 1] + out_cap[i - 1])) *monotone = false;
+    }
+    return SWC_OK;
+}
+
+int copy_back_regions(uint8_t *out_base, const u8 *d_out, const uint64_t *out_off, const uint64_t *out_cap, uint64_t b,
+                      uint64_t e, cudaStream_t s) {
+    for (uint64_t i = b; i < e;) {
+        const uint64_t r0 = out_off[i];
+        uint64_t r1 = r0 + out_cap[i++];
+        while (i < e && out_off[i] == r1) r1 += out_cap[i++];
+        if (r1 > r0) SWC_CUDA_TRY(cudaMemcpyAsync(out_base + r0, d_out + r0, r1 - r0, cudaMemcpyDeviceToHost, s));
+    }
     return SWC_OK;
 }
 
