@@ -1,5 +1,5 @@
 // deflate_tables.cuh — Deflate constants and the canonical limit-compare decoder shared by the Huffman-stage kernels
-// (inflate_lut.cu, inflate_warp.cu) and the generic decoder (inflate_slow.cu).
+// (inflate_lut.cu, inflate_warp.cu) and the generic decoder (inflate_slow.cu); their block-header grammar is deflate_header.cuh.
 // The library is built without relocatable device code, so every translation unit gets its own module: the tables are
 // `static` to give each one a private copy (a plain __constant__ here would define the host shadow symbols twice).
 #pragma once
@@ -21,11 +21,6 @@ static __constant__ u32 c_dist_tab[32] = {
 // order of the code-length code lengths in a dynamic block header (RFC 1951 3.2.7)
 static __constant__ u8 c_cl_order[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
 
-// code length of symbol i of a fixed-Huffman block: i < 288 lit/len, else distance (32 symbols of 5 bits)
-__device__ __forceinline__ int static_len(int i) {
-    return i < 144 ? 8 : i < 256 ? 9 : i < 280 ? 7 : i < 288 ? 8 : 5;
-}
-
 struct Limits {
     u32 p[8];   // p[k] = limit[2k+1] | limit[2k+2] << 16 ; limit[L] = left-justified end of the length-L code range
 };
@@ -42,6 +37,12 @@ __device__ __forceinline__ int code_length(u32 r15, const Limits &lim) {
     u32 c = __byte_perm(t[4], t[5], 0x7531), d = __byte_perm(t[6], t[7], 0x7531);
     u32 v = (a & 0x80808080u) | ((b & 0x80808080u) >> 1) | ((c & 0x80808080u) >> 2) | ((d & 0x80808080u) >> 3);
     return 1 + __popc(v);                                    // 16 => no code matches (incomplete set)
+}
+
+// Index in the canonically sorted symbol list of the length-L code at the head of r15, given
+// w = {first left-justified code of length L | index of its first symbol << 16}.
+__device__ __forceinline__ u32 canonical_index(u32 r15, int L, u32 w) {
+    return (w >> 16) + ((r15 - (w & 0xFFFFu)) >> (15 - L));
 }
 
 }  // namespace inflate

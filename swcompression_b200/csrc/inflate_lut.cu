@@ -24,7 +24,7 @@
 // Code sets with Kraft sum > 1 go to inflate_slow_kernel via SWC_INTERNAL_NEEDS_SLOW.
 // Variants that fused the LZ77 copy into this kernel were slower than this kernel followed by lz_resolve_kernel.
 #include "common.cuh"
-#include "deflate_tables.cuh"
+#include "deflate_header.cuh"
 #include "inflate.cuh"
 #include "host_util.h"
 
@@ -172,7 +172,7 @@ struct HeaderBits {
         return v;
     }
     __device__ __forceinline__ u32 peek32() const { return __funnelshift_r(word(pos >> 5), word((pos >> 5) + 1), pos); }
-    __device__ __forceinline__ u32 take(int n) { const u32 v = peek32() & ((1u << n) - 1); pos += n; return v; }
+    __device__ __forceinline__ void skip(int n) { pos += n; }
     __device__ __forceinline__ i64 avail() const { return (i64)sp.end - (i64)pos; }
 };
 
@@ -279,86 +279,55 @@ struct LaneMem {
     u32 *bol, *bod; // header phase: per-length counters, then code / long-index cursors, [1..15] (local memory)
 };
 
-// code-length alphabet: canonical decode (<= 7-bit codes, 19 symbols)
-__device__ __forceinline__ int decode_cl(u32 peek, const Limits &lim, const LaneMem &M, int &L) {
+// code-length alphabet: canonical decode (<= 7-bit codes, 19 symbols) of the next symbol, its bits consumed; -1 if none
+__device__ __forceinline__ int decode_cl(HeaderBits &hb, u32 peek, const Limits &lim, const LaneMem &M) {
     const u32 r15 = __brev(peek & 0x7FFFu) >> 17;
-    L = code_length(r15, lim);
-    if (L > 15) return -1;
-    const u32 w = M.W[(W_CL_BO + L) * 32];
-    const u32 idx = (w >> 16) + ((r15 - (w & 0xFFFFu)) >> (15 - L));
+    const int L = code_length(r15, lim);
+    if (L > 15 || hb.avail() < L) return -1;
+    hb.skip(L);
+    const u32 idx = canonical_index(r15, L, M.W[(W_CL_BO + L) * 32]);
     return ((const u8 *)(M.W + (W_CL_SYM + (idx >> 2)) * 32))[idx & 3];
 }
 
-// One pass over the HLIT+HDIST code lengths of a dynamic block (Deflate.swift:119-161) or the fixed lengths of a static
-// block (Deflate+Constants.swift:11-173). PASS 0 counts lengths into the BO areas; PASS 1 assigns codes: short codes fill
-// the LUTs, long ones are appended to the sorted symbol lists.
+// One pass over the code lengths of a block (hdr::code_lengths, or hdr::fixed_lengths for a fixed block).  PASS 0 counts
+// lengths into the BO areas; PASS 1 assigns codes: short codes fill the LUTs, long ones are appended to the sorted symbol lists.
 template <int PASS>
 __device__ int run_lengths(HeaderBits &hb, const LaneMem &M, const Limits &cl_lim, bool dynamic, int hlit, int hdist) {
-    const int count = hlit + hdist;
-    int n = 0, prev = 0;
-    while (n < count) {
-        int len, reps = 1;
-        if (!dynamic) {
-            len = static_len(n < hlit ? n : 288 + (n - hlit));
-        } else {
-            int cl;
-            const int sym = decode_cl(hb.peek32(), cl_lim, M, cl);
-            if (sym < 0 || hb.avail() < cl) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-            hb.pos += cl;
-            if (sym <= 15) {
-                len = sym;
-            } else if (sym == 16) {
-                if (n == 0) return SWC_DEFLATE_WRONG_SYMBOL;
-                if (hb.avail() < 2) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-                reps = (int)hb.take(2) + 3;
-                if (n + reps > count) return SWC_DEFLATE_WRONG_SYMBOL;
-                len = prev;
-            } else if (sym == 17) {
-                if (hb.avail() < 3) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-                reps = (int)hb.take(3) + 3;
-                len = 0;
-            } else {   // 18 (the alphabet has 19 symbols)
-                if (hb.avail() < 7) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-                reps = (int)hb.take(7) + 11;
-                len = 0;
-            }
-        }
-        if (len == 0) {
-            n += reps;      // zeros: nothing to count or place (may overshoot `count`: checked below)
-        } else {
-            for (int r = 0; r < reps; r++, n++) {
-                const bool is_lit = n < hlit;
-                u32 *bo = (is_lit ? M.bol : M.bod) + len;
-                if (PASS == 0) {
-                    *bo += 1;
-                } else {
-                    const u32 w = *bo;
-                    const int lutbits = is_lit ? LB : DB;
-                    const u32 sym = is_lit ? (u32)n : (u32)(n - hlit);
-                    if (len <= lutbits) {
-                        *bo = w + (1u << (15 - len));
-                        const u32 step = 1u << len, lim = 1u << lutbits;
-                        if (!is_lit) {
-                            for (u32 k = __brev(w & 0xFFFFu) >> 17; k < lim; k += step) M.D[k * 32] = (u8)(((u32)len << 5) | sym);
-                        } else {
-                            u32 e;
-                            if (sym < 256) e = ((u32)len << 8) | sym;
-                            else e = E_NONLIT | ((u32)len << 8) | (sym == 256 ? CODE_EOB : sym - 257);
-                            for (u32 k = __brev(w & 0xFFFFu) >> 17; k < lim; k += step) M.H[(H_LIT + k) * 32] = (u16)e;
-                        }
+    auto sink = [&](int n, int len, int reps) {
+        for (int r = 0; r < reps; r++, n++) {
+            const bool is_lit = n < hlit;
+            u32 *bo = (is_lit ? M.bol : M.bod) + len;
+            if (PASS == 0) {
+                *bo += 1;
+            } else {
+                const u32 w = *bo;
+                const int lutbits = is_lit ? LB : DB;
+                const u32 sym = is_lit ? (u32)n : (u32)(n - hlit);
+                if (len <= lutbits) {
+                    *bo = w + (1u << (15 - len));
+                    const u32 step = 1u << len, lim = 1u << lutbits;
+                    if (!is_lit) {
+                        for (u32 k = __brev(w & 0xFFFFu) >> 17; k < lim; k += step) M.D[k * 32] = (u8)(((u32)len << 5) | sym);
                     } else {
-                        *bo = w + (1u << (15 - len)) + 0x10000u;
-                        const u32 pos = w >> 16;
-                        if (is_lit) M.longsym[pos] = (u16)sym;
-                        else M.longdst[pos] = (u8)sym;
+                        u32 e;
+                        if (sym < 256) e = ((u32)len << 8) | sym;
+                        else e = E_NONLIT | ((u32)len << 8) | (sym == 256 ? CODE_EOB : sym - 257);
+                        for (u32 k = __brev(w & 0xFFFFu) >> 17; k < lim; k += step) M.H[(H_LIT + k) * 32] = (u16)e;
                     }
+                } else {
+                    *bo = w + (1u << (15 - len)) + 0x10000u;
+                    const u32 pos = w >> 16;
+                    if (is_lit) M.longsym[pos] = (u16)sym;
+                    else M.longdst[pos] = (u8)sym;
                 }
             }
         }
-        prev = len;
+    };
+    if (!dynamic) {
+        hdr::fixed_lengths(sink);
+        return SWC_OK;
     }
-    if (n != count) return SWC_DEFLATE_WRONG_SYMBOL;          // Deflate.swift:161
-    return SWC_OK;
+    return hdr::code_lengths(hb, hlit + hdist, [&](HeaderBits &r, u32 pk) { return decode_cl(r, pk, cl_lim, M); }, sink);
 }
 
 enum { ST_HEADER = 0, ST_SYMBOLS = 1, ST_PARKED = 2, ST_DONE = 3 };
@@ -371,21 +340,13 @@ struct BlockCtx {
 // Block header (Deflate.swift:41-168): stored blocks are copied here; for Huffman blocks the per-lane tables are built.
 // On entry hb.pos is the header's first bit; on SWC_OK exit it is the first bit after the header (or after the stored bytes).
 __device__ __forceinline__ int begin_block(HeaderBits &hb, Emit &em, const LaneMem &M, BlockCtx &bc, int &next) {
-    if (hb.avail() < 3) return SWC_ERR_REFERENCE_TRAP;                                  // :41-43 unguarded reads
-    const u32 hdr = hb.take(3);
-    bc.is_last = (hdr & 1) != 0;
-    const u32 btype = hdr >> 1;
-    if (btype == 3) return SWC_DEFLATE_WRONG_BLOCK_TYPE;                                 // :239
-    if (btype == 0) {                                                                   // :45-65
-        hb.pos += (u32)(hb.avail() & 7);
-        if (hb.avail() < 32) return SWC_DEFLATE_WRONG_UNCOMPRESSED_BLOCK_LENGTHS;
-        const u32 length = hb.take(16);
-        const u32 nlength = hb.take(16);
-        if ((length & nlength) != 0) return SWC_DEFLATE_WRONG_UNCOMPRESSED_BLOCK_LENGTHS;
-        if ((hb.avail() >> 3) < (i64)length) return SWC_DEFLATE_WRONG_UNCOMPRESSED_BLOCK_LENGTHS;
+    u32 btype, length;
+    if (const int st = hdr::block_start(hb, bc.is_last, btype)) return st;
+    if (btype == 0) {
+        if (const int st = hdr::stored_length(hb, length)) return st;
         const u8 *src = hb.sp.origin + (hb.pos >> 3);                                   // byte aligned here
         for (u32 i = 0; i < length; i++) em.stored_byte(__ldg(src + i));
-        hb.pos += length * 8;
+        hb.skip(length * 8);
         next = bc.is_last ? ST_DONE : ST_HEADER;
         return SWC_OK;
     }
@@ -396,14 +357,8 @@ __device__ __forceinline__ int begin_block(HeaderBits &hb, Emit &em, const LaneM
 #pragma unroll
     for (int L = 1; L <= 15; L++) { M.bol[L] = 0; M.bod[L] = 0; }
     if (dynamic) {
-        if (hb.avail() < 14) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-        hlit = (int)hb.take(5) + 257;
-        if (hlit > 286) return SWC_DEFLATE_WRONG_SYMBOL;                                 // :94
-        hdist = (int)hb.take(5) + 1;
-        const int hclen = (int)hb.take(4) + 4;
-        if (hb.avail() < 3 * hclen) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-        u64 cl = 0;                                 // 19 x 3-bit code lengths, indexed by symbol
-        for (int i = 0; i < hclen; i++) cl |= (u64)hb.take(3) << (3 * c_cl_order[i]);
+        u64 cl;                                     // 19 x 3-bit code lengths, indexed by symbol
+        if (const int st = hdr::dynamic_counts(hb, hlit, hdist, cl)) return st;
         u64 cnt = 0;                                // 8 x 8-bit counters
         for (int s = 0; s < 19; s++) cnt += 1ull << (8 * ((cl >> (3 * s)) & 7));
 #pragma unroll
@@ -422,7 +377,7 @@ __device__ __forceinline__ int begin_block(HeaderBits &hb, Emit &em, const LaneM
         rewind_tables<32>(M.W + W_CL_BO * 32, 7);
         lens_pos = hb.pos;
     }
-    int st = run_lengths<0>(hb, M, cl_lim, dynamic, hlit, hdist);
+    const int st = run_lengths<0>(hb, M, cl_lim, dynamic, hlit, hdist);
     if (st) return st;
     const u32 k1 = finalize_tables<1>(M.bol, bc.lit_lim, 15, LB);
     const u32 k2 = finalize_tables<1>(M.bod, bc.dst_lim, 15, DB);
@@ -452,8 +407,7 @@ __device__ __forceinline__ int parked_step(Reader &br, Emit &em, const LaneMem &
         const u32 r15 = __brev(w0 & 0x7FFFu) >> 17;
         const int CL = code_length(r15, bc.lit_lim);
         if (CL > 15) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-        const u32 w = M.W[(W_LONG_LIT + CL - LB - 1) * 32];          // CL > LB: the LUT holds every shorter code
-        const u32 sym = M.longsym[(w >> 16) + ((r15 - (w & 0xFFFFu)) >> (15 - CL))];
+        const u32 sym = M.longsym[canonical_index(r15, CL, M.W[(W_LONG_LIT + CL - LB - 1) * 32])];   // CL > LB: the LUT holds every shorter code
         br.pos += CL;
         L = (u32)CL;
         if (sym < 256) {
@@ -481,8 +435,7 @@ __device__ __forceinline__ int parked_step(Reader &br, Emit &em, const LaneMem &
         const u32 r15 = __brev(w32 & 0x7FFFu) >> 17;
         DL = (u32)code_length(r15, bc.dst_lim);
         if (DL > 15) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
-        const u32 w = M.W[(W_LONG_DST + DL - DB - 1) * 32];
-        dsym = M.longdst[(w >> 16) + ((r15 - (w & 0xFFFFu)) >> (15 - DL))];
+        dsym = M.longdst[canonical_index(r15, DL, M.W[(W_LONG_DST + DL - DB - 1) * 32])];
     }
     br.pos += DL;
     if (br.pos > sp.end) return SWC_DEFLATE_SYMBOL_NOT_FOUND;

@@ -5,7 +5,7 @@
 // wins, and among equal paths the code assigned last wins".  That rule is emulated here directly on the sorted code
 // list (no 2^16-slot heap per tree).  Only units the Huffman stage (K1L / K1w) flagged SWC_INTERNAL_NEEDS_SLOW are touched.
 #include "common.cuh"
-#include "deflate_tables.cuh"
+#include "deflate_header.cuh"
 #include "inflate.cuh"
 
 namespace swc {
@@ -14,9 +14,16 @@ namespace inflate {
 struct SlowBits {
     const u8 *p;
     u64 nbits, pos;
-    __device__ u64 left() const { return nbits - pos; }
+    __device__ i64 avail() const { return (i64)(nbits - pos); }
     __device__ u32 bit() { u32 b = (p[pos >> 3] >> (pos & 7)) & 1; pos++; return b; }
     __device__ u32 bits(int n) { u32 v = 0; for (int i = 0; i < n; i++) v |= bit() << i; return v; }
+    __device__ u32 peek32() const {      // zero past the end
+        SlowBits c = *this;
+        u32 v = 0;
+        for (int i = 0; i < 32 && c.avail() > 0; i++) v |= c.bit() << i;
+        return v;
+    }
+    __device__ void skip(int n) { pos += n; }
 };
 
 template <int N>
@@ -45,7 +52,7 @@ struct SlowTree {
     }
     // DecodingTree.findNextSymbol
     __device__ int next(SlowBits &r) const {
-        u64 left = r.left();
+        i64 left = r.avail();
         u32 v = 0;
         for (int d = 1; left > 0; d++) {
             v = (v << 1) | r.bit();
@@ -79,57 +86,29 @@ __global__ void __launch_bounds__(64) inflate_slow_kernel(BatchArgs a) {
     SlowTree<19> cl;
     u8 lens[320];
 #define FAIL(c) do { status = (c); goto done; } while (0)
-    if (r.left() < 10) FAIL(SWC_DEFLATE_WRONG_BLOCK_TYPE);
+#define TRY(e) do { status = (e); if (status != SWC_OK) goto done; } while (0)
+    if (r.avail() < 10) FAIL(SWC_DEFLATE_WRONG_BLOCK_TYPE);
     for (;;) {
-        if (r.left() < 3) FAIL(SWC_ERR_REFERENCE_TRAP);
-        const u32 is_last = r.bit();
-        const u32 btype = r.bits(2);
+        bool is_last;
+        u32 btype;
+        TRY(hdr::block_start(r, is_last, btype));
         if (btype == 0) {
-            r.pos = (r.pos + 7) & ~7ull;
-            if (r.left() < 32) FAIL(SWC_DEFLATE_WRONG_UNCOMPRESSED_BLOCK_LENGTHS);
-            const u32 length = r.bits(16), nlength = r.bits(16);
-            if (length & nlength) FAIL(SWC_DEFLATE_WRONG_UNCOMPRESSED_BLOCK_LENGTHS);
-            if ((r.left() >> 3) < length) FAIL(SWC_DEFLATE_WRONG_UNCOMPRESSED_BLOCK_LENGTHS);
+            u32 length;
+            TRY(hdr::stored_length(r, length));
             for (u32 i = 0; i < length; i++) { u8 b = (u8)r.bits(8); if (op < cap) out[op] = b; op++; }
-        } else if (btype == 3) {
-            FAIL(SWC_DEFLATE_WRONG_BLOCK_TYPE);
         } else {
             int hlit = 288, hdist = 32;
+            auto sink = [&](int n, int len, int reps) { for (int i = 0; i < reps; i++) lens[n + i] = (u8)len; };
             if (btype == 1) {
-                for (int i = 0; i < 320; i++) lens[i] = (u8)static_len(i);
+                hdr::fixed_lengths(sink);
             } else {
-                if (r.left() < 14) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
-                hlit = (int)r.bits(5) + 257;
-                if (hlit > 286) FAIL(SWC_DEFLATE_WRONG_SYMBOL);
-                hdist = (int)r.bits(5) + 1;
-                const int hclen = (int)r.bits(4) + 4;
-                if (r.left() < (u64)(3 * hclen)) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
+                u64 cl_lens;
+                TRY(hdr::dynamic_counts(r, hlit, hdist, cl_lens));
                 u8 cll[19];
-                for (int i = 0; i < 19; i++) cll[i] = 0;
-                for (int i = 0; i < hclen; i++) cll[c_cl_order[i]] = (u8)r.bits(3);
+                for (int s = 0; s < 19; s++) cll[s] = (u8)((cl_lens >> (3 * s)) & 7);
                 cl.build(cll, 19);
-                const int count = hlit + hdist;
-                for (int i = 0; i < count; i++) lens[i] = 0;
-                int n = 0;
-                while (n < count) {
-                    const int s = cl.next(r);
-                    if (s < 0) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
-                    if (s <= 15) { lens[n++] = (u8)s; }
-                    else if (s == 16 && n > 0) {
-                        if (r.left() < 2) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
-                        const int c = (int)r.bits(2) + 3;
-                        if (n + c > count) FAIL(SWC_DEFLATE_WRONG_SYMBOL);
-                        for (int i = 0; i < c; i++) lens[n + i] = lens[n - 1];
-                        n += c;
-                    } else if (s == 17) {
-                        if (r.left() < 3) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
-                        n += (int)r.bits(3) + 3;
-                    } else if (s == 18) {
-                        if (r.left() < 7) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
-                        n += (int)r.bits(7) + 11;
-                    } else FAIL(SWC_DEFLATE_WRONG_SYMBOL);
-                }
-                if (n != count) FAIL(SWC_DEFLATE_WRONG_SYMBOL);
+                for (int i = 0; i < hlit + hdist; i++) lens[i] = 0;
+                TRY(hdr::code_lengths(r, hlit + hdist, [&](SlowBits &b, u32) { return cl.next(b); }, sink));
             }
             lit.build(lens, hlit);
             dist.build(lens + hlit, hdist);
@@ -141,14 +120,14 @@ __global__ void __launch_bounds__(64) inflate_slow_kernel(BatchArgs a) {
                 if (s > 285) FAIL(SWC_DEFLATE_WRONG_SYMBOL);
                 const u32 le = c_len_tab[s - 257];
                 const int eb = (int)(le >> 16);
-                if (r.left() < (u64)eb) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
+                if (r.avail() < eb) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
                 const u32 length = (le & 0xFFFFu) + r.bits(eb);
                 const int dc = dist.next(r);
                 if (dc < 0) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
                 if (dc > 29) FAIL(SWC_DEFLATE_WRONG_SYMBOL);
                 const u32 de = c_dist_tab[dc];
                 const int db = (int)(de >> 16);
-                if (r.left() < (u64)db) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
+                if (r.avail() < db) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
                 const u64 d = (u64)(de & 0xFFFFu) + r.bits(db);
                 if (d > op) FAIL(SWC_ERR_REFERENCE_TRAP);
                 for (u32 i = 0; i < length; i++) { if (op < cap) out[op] = out[op - d]; op++; }
@@ -158,6 +137,7 @@ __global__ void __launch_bounds__(64) inflate_slow_kernel(BatchArgs a) {
     }
 done:
 #undef FAIL
+#undef TRY
     if (status == SWC_OK && op > cap) status = SWC_ERR_OUTPUT_OVERFLOW;
     a.out_len[unit] = op;
     a.consumed_bits[unit] = r.pos - skip;

@@ -14,7 +14,7 @@
 // Block headers (code lengths, table build) and stored blocks are handled warp-uniformly / cooperatively.
 // Code sets with Kraft sum > 1 are routed to inflate_slow_kernel exactly like in K1L.
 #include "common.cuh"
-#include "deflate_tables.cuh"
+#include "deflate_header.cuh"
 #include "inflate.cuh"
 #include "host_util.h"
 
@@ -46,19 +46,21 @@ struct Smem {
     u8 cl_lut[128];              // code-length alphabet: sym << 3 | len (0 = no code)
 };
 
-// ---- warp-uniform view of the unit's bitstream (header parsing): positions are bits from `wbase` ----
+// ---- warp-uniform view of the unit's bitstream and the position of the true chain (header parsing reads it directly) ----
 struct Stream {
     const u32 *wbase;     // 4-byte aligned word containing the unit's first byte
     u64 bit0;             // bit offset of the unit's first bit inside wbase (0..31+7)
     u64 total;            // unit length in bits counted from bit0 (the reference's initial bitsLeft)
     u64 nwords;           // words that may be read
+    u64 pos;              // bits consumed from the unit start
     __device__ __forceinline__ u32 word(u64 i) const { return i < nwords ? __ldg(wbase + i) : 0u; }
-    // 32 bits starting at absolute bit position p (p counts from bit0)
-    __device__ __forceinline__ u32 peek32(u64 p) const {
-        const u64 q = p + bit0;
+    __device__ __forceinline__ u32 peek32() const {
+        const u64 q = pos + bit0;
         const u64 wi = q >> 5;
         return __funnelshift_r(word(wi), word(wi + 1), (u32)(q & 31));
     }
+    __device__ __forceinline__ void skip(int n) { pos += n; }
+    __device__ __forceinline__ i64 avail() const { return (i64)(total - pos); }
 };
 
 // ---- per-lane bit cursor over the shared staging buffer ----
@@ -87,8 +89,7 @@ __device__ __forceinline__ int canon_decode(const Smem &S, const Limits &lim, u3
     const u32 r15 = __brev(peek15) >> 17;
     L = code_length(r15, lim);
     if (L > 15) return -1;
-    const u32 wv = KIND == 0 ? S.lit_bo[L] : S.dst_bo[L];
-    const u32 idx = (wv >> 16) + ((r15 - (wv & 0xFFFFu)) >> (15 - L));
+    const u32 idx = canonical_index(r15, L, KIND == 0 ? S.lit_bo[L] : S.dst_bo[L]);
     return KIND == 0 ? (int)S.lit_sym[idx] : (int)S.dst_sym[idx];
 }
 
@@ -265,7 +266,6 @@ inflate_warp_kernel(BatchArgs a) {
         u32 *rec = a.rec_base + rec_start(a.out_off[unit] + cap64);
         const u32 bitskip = a.start_bits ? a.start_bits[unit] : 0;
         int status = SWC_OK;
-        u64 pos = 0;                 // bits consumed from the unit start (true chain)
         u64 op = 0;                  // bytes produced
         u32 nlit = 0;                // literals produced
         u32 nrec = 0;
@@ -277,30 +277,26 @@ inflate_warp_kernel(BatchArgs a) {
             st.bit0 = (addr & 3) * 8 + bitskip;
             st.total = in_len * 8 - bitskip;
             st.nwords = ((addr & 3) + in_len + 3) >> 2;
+            st.pos = 0;
         }
         Tables T;
 #define FAIL(c) do { status = (c); goto unit_done; } while (0)
+#define TRY(e) do { status = (e); if (status != SWC_OK) goto unit_done; } while (0)
         if (in_len >= (1ull << 32)) FAIL(SWC_ERR_UNSUPPORTED);
         if (st.total < 10) FAIL(SWC_DEFLATE_WRONG_BLOCK_TYPE);                                   // Deflate.swift:36
         for (;;) {
             // ------------------------------------------------------------ block header (warp-uniform)
-            if (st.total - pos < 3) FAIL(SWC_ERR_REFERENCE_TRAP);                               // :41-43
-            const u32 hdr = st.peek32(pos) & 7; pos += 3;
-            const bool is_last = hdr & 1;
-            const u32 btype = hdr >> 1;
-            if (btype == 3) FAIL(SWC_DEFLATE_WRONG_BLOCK_TYPE);
-            if (btype == 0) {                                                                   // stored :45-65
-                pos += (st.total - pos) & 7;
-                if (st.total - pos < 32) FAIL(SWC_DEFLATE_WRONG_UNCOMPRESSED_BLOCK_LENGTHS);
-                const u32 v = st.peek32(pos); pos += 32;
-                const u32 length = v & 0xFFFF, nlength = v >> 16;
-                if (length & nlength) FAIL(SWC_DEFLATE_WRONG_UNCOMPRESSED_BLOCK_LENGTHS);
-                if (((st.total - pos) >> 3) < length) FAIL(SWC_DEFLATE_WRONG_UNCOMPRESSED_BLOCK_LENGTHS);
-                const u8 *src = (const u8 *)st.wbase + ((pos + st.bit0) >> 3);
+            bool is_last;
+            u32 btype;
+            TRY(hdr::block_start(st, is_last, btype));
+            if (btype == 0) {
+                u32 length;
+                TRY(hdr::stored_length(st, length));
+                const u8 *src = (const u8 *)st.wbase + ((st.pos + st.bit0) >> 3);
                 if (op + length > 0xFFFFFFF0ull) FAIL(SWC_ERR_UNSUPPORTED);
                 if (op + length <= cap) for (u32 i = lane; i < length; i += 32) lits[nlit + i] = src[i];
                 op += length; nlit += length; run_carry += length;
-                pos += (u64)length * 8;
+                st.pos += (u64)length * 8;
                 __syncwarp();
                 if (is_last) break;
                 continue;
@@ -308,17 +304,10 @@ inflate_warp_kernel(BatchArgs a) {
             // ---- code lengths -> S.lens[0..hlit+hdist)
             int hlit = 288, hdist = 32;
             if (btype == 1) {
-                for (int i = lane; i < 320; i += 32) S.lens[i] = static_len(i);
+                hdr::fixed_lengths([&](int n, int len, int reps) { for (int i = lane; i < reps; i += 32) S.lens[n + i] = (u8)len; });
             } else {
-                if (st.total - pos < 14) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
-                const u32 h = st.peek32(pos); pos += 14;
-                hlit = (int)(h & 31) + 257;
-                if (hlit > 286) FAIL(SWC_DEFLATE_WRONG_SYMBOL);
-                hdist = (int)((h >> 5) & 31) + 1;
-                const int hclen = (int)((h >> 10) & 15) + 4;
-                if (st.total - pos < (u64)(3 * hclen)) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
-                u64 cl = 0;
-                for (int i = 0; i < hclen; i++) { cl |= (u64)(st.peek32(pos) & 7) << (3 * c_cl_order[i]); pos += 3; }
+                u64 cl;
+                TRY(hdr::dynamic_counts(st, hlit, hdist, cl));
                 // canonical code of the 19-symbol alphabet -> 7-bit LUT (lane s handles symbol s)
                 u32 cnt8[8];
 #pragma unroll
@@ -346,34 +335,16 @@ inflate_warp_kernel(BatchArgs a) {
                     }
                 }
                 __syncwarp();
-                const int count = hlit + hdist;
-                int n = 0; u32 prev = 0;
                 for (int i = lane; i < 320; i += 32) S.lens[i] = 0;
                 __syncwarp();
-                while (n < count) {                                                             // :119-158 (uniform)
-                    const u32 pk = st.peek32(pos);
-                    const u32 ce = S.cl_lut[pk & 127];
-                    const u32 cll = ce & 7, sym = ce >> 3;
-                    if (cll == 0 || st.total - pos < cll) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
-                    pos += cll;
-                    const u32 x = pk >> cll;
-                    if (sym <= 15) { if (lane == 0) S.lens[n] = (u8)sym; prev = sym; n++; }
-                    else if (sym == 16) {
-                        if (n == 0) FAIL(SWC_DEFLATE_WRONG_SYMBOL);
-                        if (st.total - pos < 2) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
-                        const int reps = (int)(x & 3) + 3; pos += 2;
-                        if (n + reps > count) FAIL(SWC_DEFLATE_WRONG_SYMBOL);
-                        if ((int)lane < reps) S.lens[n + lane] = (u8)prev;
-                        n += reps;
-                    } else if (sym == 17) {
-                        if (st.total - pos < 3) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
-                        n += (int)(x & 7) + 3; pos += 3; prev = 0;
-                    } else {
-                        if (st.total - pos < 7) FAIL(SWC_DEFLATE_SYMBOL_NOT_FOUND);
-                        n += (int)(x & 127) + 11; pos += 7; prev = 0;
-                    }
-                }
-                if (n != count) FAIL(SWC_DEFLATE_WRONG_SYMBOL);                                 // :161
+                auto decode = [&](Stream &r, u32 pk) {                                          // uniform
+                    const u32 ce = S.cl_lut[pk & 127], cll = ce & 7;
+                    const bool ok = cll != 0 && r.avail() >= cll;
+                    r.skip(ok ? cll : 0);
+                    return ok ? (int)(ce >> 3) : -1;
+                };
+                // runs of at most 6: lane i writes length n + i
+                TRY(hdr::code_lengths(st, hlit + hdist, decode, [&](int n, int len, int reps) { if ((int)lane < reps) S.lens[n + lane] = (u8)len; }));
             }
             __syncwarp();
             // ---- canonical tables for both alphabets
@@ -438,12 +409,12 @@ inflate_warp_kernel(BatchArgs a) {
             bool block_done = false;
             while (!block_done) {
                 // stage the chunk: words covering bits [pos, pos + 32*WIN_BITS + margin)
-                const u64 q = pos + st.bit0;
+                const u64 q = st.pos + st.bit0;
                 const u64 w0 = q >> 5;
                 const u32 stage_bit0 = (u32)(q & 31);
                 for (int i = lane; i < STAGE_WORDS; i += 32) S.stage[i] = st.word(w0 + i);
                 __syncwarp();
-                const u64 left = st.total - pos;
+                const u64 left = st.total - st.pos;
                 const u32 hi = (lane + 1) * WIN_BITS;
                 u32 start = lane * WIN_BITS;
                 bool dirty = true, valid = true;
@@ -509,7 +480,7 @@ inflate_warp_kernel(BatchArgs a) {
                 const u32 endbits = __shfl_sync(SWC_FULL, r.end, last);
                 const u32 lflags = __shfl_sync(SWC_FULL, r.flags, last);
                 op += tot_b; nlit += tot_l; nrec += tot_r; run_carry = carry;
-                pos += endbits;
+                st.pos += endbits;
                 __syncwarp();
                 if (lflags & 2) block_done = true;
             }
@@ -517,12 +488,13 @@ inflate_warp_kernel(BatchArgs a) {
         }
     unit_done:
 #undef FAIL
+#undef TRY
         __syncwarp();
         if (lane == 0) {
             if (status == SWC_OK && op > cap64) status = SWC_ERR_OUTPUT_OVERFLOW;
             // a unit of fewer than 8 literals may not fit its literals below its records (inflate.cuh)
             if (status == SWC_OK && (u64)nlit + 4ull * nrec > region_bytes(a.out_off[unit], cap64)) status = SWC_INTERNAL_NEEDS_SLOW;
-            a.consumed_bits[unit] = pos;
+            a.consumed_bits[unit] = st.pos;
             a.out_len[unit] = op;
             a.status[unit] = status;
             a.rec_count[unit] = nrec;

@@ -40,8 +40,8 @@ def _caps(lay, short):
     lay.out_off, lay.out_cap, lay.total = offs, caps, pos + H.GUARD
 
 
-def catalogue_batches(oracle):
-    cases = D.catalogue()
+def case_batches(oracle, cases):
+    """cases (deflate_cases.Case or anything with its fields) as one batch, at exact and one-short capacities"""
     units = [H.LayoutUnit(c.data, aux=c.start_bit, raw=c.expect) for c in cases]
     lay = Layout("deflate", oracle, units, 301)
     wrong = [(c.name, e[0]) for c, e in zip(cases, lay.expect) if e[0] != c.status or (e[0] == 0 and e[2] != c.nbits)]
@@ -49,6 +49,10 @@ def catalogue_batches(oracle):
     for short in (0, 1):
         _caps(lay, short)
         lay.check(*run_both(lay, run_deflate, start_bits=[u.aux for u in units]))
+
+
+def catalogue_batches(oracle):
+    case_batches(oracle, D.catalogue())
 
 
 def truncation_batch(oracle):
@@ -59,12 +63,12 @@ def truncation_batch(oracle):
     lay.check(*run_both(lay, run_deflate, start_bits=[u.aux for u in units]))
 
 
-def _child(kernel, fn):
+def _child(kernel, fn, module="test_gpu_deflate_handmade"):
     env = dict(os.environ, SWC_DEFLATE_K1=kernel)
     env["PYTHONPATH"] = os.pathsep.join([ROOT, os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tests")] +
                                         ([env["PYTHONPATH"]] if env.get("PYTHONPATH") else []))
     flags = ["-s"] if sys.flags.no_user_site else []
-    code = f"import swco, test_gpu_deflate_handmade as T; T.{fn}(swco)"
+    code = f"import swco, {module} as T; T.{fn}(swco)"
     p = subprocess.run([sys.executable] + flags + ["-c", code], cwd=ROOT, env=env, stdout=subprocess.PIPE,
                        stderr=subprocess.PIPE, text=True, timeout=900)
     assert p.returncode == 0, p.stderr[-4000:]
