@@ -68,7 +68,7 @@ enum swc_status {
     SWC_GZIP_WRONG_HEADER_CRC         = 604,
     SWC_GZIP_WRONG_CRC                = 605,  /* payload-carrying */
     SWC_GZIP_WRONG_ISIZE              = 606,
-    SWC_GZIP_CANNOT_ENCODE_ISO_LATIN1 = 607,  /* compress-side only; never produced here */
+    SWC_GZIP_CANNOT_ENCODE_ISO_LATIN1 = 607,  /* swc_gzip_archive: extra fields longer than 65 535 bytes */
 
     SWC_ZLIB_WRONG_COMPRESSION_METHOD = 701,
     SWC_ZLIB_WRONG_COMPRESSION_INFO   = 702,

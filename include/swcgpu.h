@@ -131,6 +131,46 @@ int32_t swc_lz4_block_compress_batch(const uint8_t *in_base, const uint64_t *in_
                                      uint64_t *out_len, int32_t *status, uint64_t n,
                                      void *scratch, size_t scratch_bytes, void *cuda_stream);
 
+/* ---- Deflate compression ------------------------------------------------------------------------------------
+ * Deflate.compress(data:)                                                 Sources/Deflate/Deflate+Compress.swift:22-42
+ * ZlibArchive.archive(data:)                                              Sources/Zlib/ZlibArchive.swift:54-70
+ * GzipArchive.archive(data:comment:fileName:writeHeaderCRC:isTextFile:osType:modificationTime:extraFields:)
+ *                                                                          Sources/GZip/GzipArchive.swift:126-241
+ * The output bytes equal the reference's: one block, stored or static Huffman, from its greedy parse (not zlib's).  The
+ * single calls read host memory and return an swc_alloc'ed buffer; the CRC-32 / Adler-32 of the input run on the device.
+ * Inputs of 4 GiB or more return SWC_ERR_UNSUPPORTED. */
+int32_t swc_deflate_compress(const uint8_t *in, size_t in_len, uint8_t **out, size_t *out_len);
+int32_t swc_zlib_archive(const uint8_t *in, size_t in_len, uint8_t **out, size_t *out_len);
+/* GzipArchive.archive's options.  file_name / comment: NULL = nil, else ISO-Latin-1 bytes (the caller encodes; a NUL is
+ * appended unless the last byte is one, so an empty string becomes a single NUL).  os_type: the OS byte (255 = nil or
+ * .other).  mtime: Int(timeIntervalSince1970) when has_mtime, of which the low 32 bits are written.  Extra field i has
+ * the ids extra_ids[2i], extra_ids[2i+1] and extra_lens[i] bytes; the fields' bytes follow each other in extra_bytes.
+ * An XLEN (sum of 4 + length) over 65 535 returns SWC_GZIP_CANNOT_ENCODE_ISO_LATIN1, as the reference throws. */
+typedef struct swc_gzip_options {
+    const uint8_t *file_name; size_t file_name_len;
+    const uint8_t *comment; size_t comment_len;
+    int32_t write_header_crc, is_text_file;
+    int32_t has_mtime; int64_t mtime;
+    uint8_t os_type;
+    size_t n_extra;
+    const uint8_t *extra_ids;
+    const uint64_t *extra_lens;
+    const uint8_t *extra_bytes;
+} swc_gzip_options;
+int32_t swc_gzip_archive(const uint8_t *in, size_t in_len, const swc_gzip_options *options, uint8_t **out, size_t *out_len);
+/* Raw Deflate streams, device memory, asynchronous on `cuda_stream` (the unit sizes are read back first, which
+ * synchronises).  Unit i compresses in_base[in_off[i] ..+ in_len[i]) (any alignment) into out_base + out_off[i] (a
+ * multiple of 16).  out_len[i] is the exact stream size, at most (9 in_len[i] + 17) / 8; if it exceeds out_cap[i] the
+ * unit reports SWC_ERR_OUTPUT_OVERFLOW and writes nothing.  Nothing outside [out_off[i], out_off[i] + out_cap[i]) is
+ * written, nor past out_len[i].  scratch may be NULL (library pool); a caller's scratch of
+ * swc_deflate_compress_batch_scratch_bytes(n, sum of in_len[i]) bytes runs the batch in one slice, a smaller one in
+ * several (it must hold the largest unit). */
+size_t  swc_deflate_compress_batch_scratch_bytes(uint64_t n, uint64_t in_bytes_total);
+int32_t swc_deflate_compress_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                                   uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                   uint64_t *out_len, int32_t *status, uint64_t n,
+                                   void *scratch, size_t scratch_bytes, void *cuda_stream);
+
 /* ---- BZip2--------------------------------------------------------------------------------------------------
  * BZip2.decompress(data:)            Sources/BZip2/BZip2.swift:22-26
  * BZip2.multiDecompress(data:)       Sources/BZip2/BZip2.swift:40-48

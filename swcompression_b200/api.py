@@ -9,6 +9,9 @@ meaning, same error cases), routed through the C ABI of libswcgpu.so.
     LZ4.decompress(data:[dictionary:dictionaryID:])     LZ4.decompress(data[, dictionary, dictionaryID])
     LZ4.multiDecompress(data:dictionary:dictionaryID:)  LZ4.multiDecompress(...)
     LZ4.compress(data:[independentBlocks:...])          LZ4.compress(data[, independentBlocks, ...])
+    Deflate.compress(data:)                             Deflate.compress(data)
+    GzipArchive.archive(data:comment:...)               GzipArchive.archive(data, comment=None, fileName=None, ...)
+    ZlibArchive.archive(data:)                          ZlibArchive.archive(data)
     GzipArchive.unarchive / multiUnarchive -> [Member]  GzipArchive.unarchive / multiUnarchive -> [GzipArchive.Member]
     GzipHeader(archive:) / ZlibHeader(archive:)         GzipHeader(archive) / ZlibHeader(archive)
     ZlibArchive.unarchive                               ZlibArchive.unarchive
@@ -52,8 +55,24 @@ def _multi(fn, data, *extra):
     return parts
 
 
+def _compressed(fn, data, *extra):
+    L = _lib.lib()
+    buf, n = _lib.inbuf(data)
+    out, out_len = C.c_void_p(), C.c_size_t(0)
+    st = getattr(L, fn)(buf, n, *extra, C.byref(out), C.byref(out_len))
+    payload = _lib.take(out, out_len)
+    if st != 0:
+        raise error_for(st, None)
+    return payload
+
+
 class Deflate:
-    """Sources/Deflate/Deflate.swift:10-28"""
+    """Sources/Deflate/Deflate.swift:10-28, Sources/Deflate/Deflate+Compress.swift:22-42"""
+
+    @staticmethod
+    def compress(data):
+        """Deflate.compress(data:): one stored or static-Huffman block, equal to the reference's byte for byte."""
+        return _compressed("swc_deflate_compress", data)
 
     @staticmethod
     def decompress(data):
@@ -174,6 +193,24 @@ class ExtraField:
 
 # FileSystemType(rawOsType), Sources/Common/FileSystemType.swift (gzip OS byte)
 _OS_TYPES = {0: "fat", 3: "unix", 7: "macintosh", 11: "ntfs"}
+_OS_BYTES = {v: k for k, v in _OS_TYPES.items()}      # osTypeByte (FileSystemType+Gzip.swift:23-36); others are 255
+
+
+class _CGzipOptions(C.Structure):
+    _fields_ = [("file_name", C.c_void_p), ("file_name_len", C.c_size_t), ("comment", C.c_void_p), ("comment_len", C.c_size_t),
+                ("write_header_crc", C.c_int32), ("is_text_file", C.c_int32), ("has_mtime", C.c_int32), ("mtime", C.c_int64),
+                ("os_type", C.c_uint8), ("n_extra", C.c_size_t), ("extra_ids", C.c_void_p), ("extra_lens", C.c_void_p),
+                ("extra_bytes", C.c_void_p)]
+
+
+def _latin1(text):
+    """String.data(using: .isoLatin1) of the text with a NUL appended unless it ends with one (GzipArchive.swift:132-161)"""
+    if not text or text[-1] != "\0":
+        text = text + "\0"
+    try:
+        return text.encode("latin-1")
+    except UnicodeEncodeError:
+        raise error_for(607, None) from None
 
 
 class GzipHeader:
@@ -214,7 +251,41 @@ class ZlibHeader:
 
 
 class GzipArchive:
-    """Sources/GZip/GzipArchive.swift:10-77"""
+    """Sources/GZip/GzipArchive.swift:10-241"""
+
+    @staticmethod
+    def archive(data, comment=None, fileName=None, writeHeaderCRC=False, isTextFile=False, osType=None,
+                modificationTime=None, extraFields=()):
+        """GzipArchive.archive(data:comment:fileName:writeHeaderCRC:isTextFile:osType:modificationTime:extraFields:).
+        osType is a FileSystemType name ("fat", "unix", "macintosh", "ntfs", "other") or None; modificationTime a
+        datetime or seconds since 1970.  Text that is not ISO-Latin-1, and extra fields whose XLEN exceeds 65 535, raise
+        GzipError.cannotEncodeISOLatin1 as the reference throws."""
+        # the reference encodes the comment first, then the file name (:130-157); both fail the same way
+        c = None if comment is None else _latin1(comment)
+        f = None if fileName is None else _latin1(fileName)
+        o = _CGzipOptions()
+        keep = []
+        for text, ptr, ln in ((f, "file_name", "file_name_len"), (c, "comment", "comment_len")):
+            if text is not None:
+                b = C.create_string_buffer(text, len(text))
+                keep.append(b)
+                setattr(o, ptr, C.cast(b, C.c_void_p))
+                setattr(o, ln, len(text))
+        o.write_header_crc, o.is_text_file = int(bool(writeHeaderCRC)), int(bool(isTextFile))
+        if modificationTime is not None:
+            t = modificationTime.timestamp() if isinstance(modificationTime, datetime.datetime) else modificationTime
+            o.has_mtime, o.mtime = 1, int(t)                 # Int(timeIntervalSince1970) truncates toward zero
+        o.os_type = 255 if osType is None else _OS_BYTES.get(osType, 255)
+        fields = list(extraFields)
+        if fields:
+            ids = (C.c_uint8 * (2 * len(fields)))(*[v for e in fields for v in (e.si1, e.si2)])
+            lens = (C.c_uint64 * len(fields))(*[len(e.bytes) for e in fields])
+            blob = b"".join(bytes(e.bytes) for e in fields)
+            bb = C.create_string_buffer(blob, max(len(blob), 1))
+            keep += [ids, lens, bb]
+            o.n_extra, o.extra_ids, o.extra_lens = len(fields), C.cast(ids, C.c_void_p), C.cast(lens, C.c_void_p)
+            o.extra_bytes = C.cast(bb, C.c_void_p)
+        return _compressed("swc_gzip_archive", data, C.byref(o))
 
     @dataclass
     class Member:
@@ -247,7 +318,12 @@ class GzipArchive:
 
 
 class ZlibArchive:
-    """Sources/Zlib/ZlibArchive.swift:10-42"""
+    """Sources/Zlib/ZlibArchive.swift:10-70"""
+
+    @staticmethod
+    def archive(data):
+        """ZlibArchive.archive(data:): 78 DA, the Deflate.compress stream, the big-endian Adler-32."""
+        return _compressed("swc_zlib_archive", data)
 
     @staticmethod
     def unarchive(archive):

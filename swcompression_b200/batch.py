@@ -30,12 +30,16 @@ def pack_units(units, align=16):
 
 
 class Batch:
-    """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'lzma2', 'lz4_block_compress').
+    """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'lzma2', 'lz4_block_compress',
+    'deflate_compress').
 
     'lz4_block_compress' compresses each unit into a raw LZ4 block (LZ4+Compress.swift:156-277); `aux` is then an optional
-    (dict_off, dict_len) pair of u64 arrays placing each unit's dictionary window inside `in_buf`."""
+    (dict_off, dict_len) pair of u64 arrays placing each unit's dictionary window inside `in_buf`.
+    'deflate_compress' compresses each unit into a raw Deflate stream (Deflate.compress, Deflate+Compress.swift:22-42); a
+    unit of n bytes needs at most (9 n + 17) // 8 bytes of output.  `scratch_bytes` caps the caller scratch it passes
+    (the library then runs the batch in slices)."""
 
-    def __init__(self, codec, in_buf, in_off, in_len, out_cap, device="cuda:0", aux=None):
+    def __init__(self, codec, in_buf, in_off, in_len, out_cap, device="cuda:0", aux=None, scratch_bytes=None):
         self.codec = codec
         self.device = torch.device(device)
         self.n = len(in_off)
@@ -70,14 +74,20 @@ class Batch:
             self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         else:
             self.d_aux = None if aux is None else torch.from_numpy(np.frombuffer(bytes(aux), dtype=np.uint8).copy()).to(self.device)
+        if codec == "deflate_compress":
+            total = int(np.asarray(in_len, dtype=np.uint64).sum())
+            nbytes = min(_lib.lib().swc_deflate_compress_batch_scratch_bytes(self.n, total), 16 << 30)
+            if scratch_bytes is not None:
+                nbytes = min(nbytes, int(scratch_bytes))
+            self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         if codec == "deflate":
             nbytes = _lib.lib().swc_deflate_batch_scratch_bytes(self.n, self.out_total)
             self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
 
     @classmethod
-    def from_units(cls, codec, units, out_cap, device="cuda:0", aux=None):
+    def from_units(cls, codec, units, out_cap, device="cuda:0", aux=None, scratch_bytes=None):
         buf, offs, lens = pack_units(units)
-        return cls(codec, buf, offs, lens, out_cap, device, aux)
+        return cls(codec, buf, offs, lens, out_cap, device, aux, scratch_bytes)
 
     def run(self):
         L = _lib.lib()
@@ -98,6 +108,10 @@ class Batch:
                                                 opt(self.d_dict_len), p(self.d_out), p(self.d_out_off), p(self.d_out_cap),
                                                 p(self.d_out_len), p(self.d_status), self.n, p(self.d_scratch),
                                                 self.d_scratch.numel(), stream)
+        elif self.codec == "deflate_compress":
+            st = L.swc_deflate_compress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out), p(self.d_out_off),
+                                              p(self.d_out_cap), p(self.d_out_len), p(self.d_status), self.n, p(self.d_scratch),
+                                              self.d_scratch.numel(), stream)
         elif self.codec == "bzip2":
             st = L.swc_bzip2_decompress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out), p(self.d_out_off),
                                               p(self.d_out_cap), p(self.d_out_len), p(self.d_consumed), p(self.d_status), self.n, stream)

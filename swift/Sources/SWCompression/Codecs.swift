@@ -1,7 +1,7 @@
 // Public decode API of the reference, bodies routed through libswcgpu (include/swcgpu.h).
 //   DecompressionAlgorithm  Sources/Common/DecompressionAlgorithm.swift:9-14
 //   Archive                 Sources/Common/Archive.swift:9-14
-//   CompressionAlgorithm    Sources/Common/CompressionAlgorithm.swift (LZ4 is its only GPU-backed conformer here)
+//   CompressionAlgorithm    Sources/Common/CompressionAlgorithm.swift (LZ4 and Deflate are its GPU-backed conformers here)
 import CSWCGPU
 import Foundation
 
@@ -119,6 +119,68 @@ extension LZ4: CompressionAlgorithm {                                // Sources/
         }
         defer { swc_free(out) }
         guard status == 0 else { fatalError("LZ4.compress: \(String(cString: swc_status_name(status)))") }
+        return out.map { Data(bytes: $0, count: outLen) } ?? Data()
+    }
+}
+
+/// Runs a compress entry point `(in, len, &out, &outLen) -> status`.  Non-throwing as in the reference: an engine status (no
+/// device, CUDA failure, an input of 4 GiB or more) stops the program.  Compile-unverified, like the rest of this shim.
+private func compressed(_ name: String, _ data: Data, _ body: (UnsafePointer<UInt8>?, Int, UnsafeMutablePointer<UnsafeMutablePointer<UInt8>?>,
+                                                                 UnsafeMutablePointer<Int>) -> Int32) -> Data {
+    var out: UnsafeMutablePointer<UInt8>? = nil
+    var outLen = 0
+    let status: Int32 = data.withUnsafeBytes { raw in body(raw.bindMemory(to: UInt8.self).baseAddress, raw.count, &out, &outLen) }
+    defer { swc_free(out) }
+    guard status == 0 else { fatalError("\(name): \(String(cString: swc_status_name(status)))") }
+    return out.map { Data(bytes: $0, count: outLen) } ?? Data()
+}
+
+extension Deflate: CompressionAlgorithm {                            // Sources/Deflate/Deflate+Compress.swift:10-42
+    public static func compress(data: Data) -> Data {
+        compressed("Deflate.compress", data) { p, n, o, ol in swc_deflate_compress(p, n, o, ol) }
+    }
+}
+
+extension ZlibArchive {                                              // Sources/Zlib/ZlibArchive.swift:54-70
+    public static func archive(data: Data) -> Data {
+        compressed("ZlibArchive.archive", data) { p, n, o, ol in swc_zlib_archive(p, n, o, ol) }
+    }
+}
+
+extension GzipArchive {                                              // Sources/GZip/GzipArchive.swift:126-241
+    public static func archive(data: Data, comment: String? = nil, fileName: String? = nil, writeHeaderCRC: Bool = false,
+                               isTextFile: Bool = false, osType: FileSystemType? = nil, modificationTime: Date? = nil,
+                               extraFields: [GzipHeader.ExtraField] = []) throws -> Data {
+        // :130-157: the comment first, then the file name, each NUL-terminated and ISO-Latin-1
+        func latin1(_ s: String?) throws -> Data? {
+            guard var s = s else { return nil }
+            if s.last != "\u{00}" { s.append("\u{00}") }
+            guard let d = s.data(using: .isoLatin1) else { throw GzipError.cannotEncodeISOLatin1 }
+            return d
+        }
+        let c = try latin1(comment), f = try latin1(fileName)
+        let ids = extraFields.flatMap { [$0.si1, $0.si2] }
+        let lens = extraFields.map { UInt64($0.bytes.count) }
+        let blob = extraFields.flatMap { $0.bytes } + [0]
+        var out: UnsafeMutablePointer<UInt8>? = nil
+        var outLen = 0
+        let status: Int32 = (f ?? Data([0])).withUnsafeBytes { fr in (c ?? Data([0])).withUnsafeBytes { cr in
+            ids.withUnsafeBufferPointer { ir in lens.withUnsafeBufferPointer { lr in blob.withUnsafeBufferPointer { br in
+                var o = swc_gzip_options()
+                if let f = f { o.file_name = fr.bindMemory(to: UInt8.self).baseAddress; o.file_name_len = f.count }
+                if let c = c { o.comment = cr.bindMemory(to: UInt8.self).baseAddress; o.comment_len = c.count }
+                o.write_header_crc = writeHeaderCRC ? 1 : 0
+                o.is_text_file = isTextFile ? 1 : 0
+                if let t = modificationTime { o.has_mtime = 1; o.mtime = Int64(Int(t.timeIntervalSince1970)) }
+                o.os_type = osType?.osTypeByte ?? 255
+                o.n_extra = extraFields.count
+                o.extra_ids = ir.baseAddress; o.extra_lens = lr.baseAddress; o.extra_bytes = br.baseAddress
+                return data.withUnsafeBytes { raw in swc_gzip_archive(raw.bindMemory(to: UInt8.self).baseAddress, raw.count, &o, &out, &outLen) }
+            } } }
+        } }
+        defer { swc_free(out) }
+        if status == 607 { throw GzipError.cannotEncodeISOLatin1 }                   // XLEN > 65 535 (:205-207)
+        guard status == 0 else { fatalError("GzipArchive.archive: \(String(cString: swc_status_name(status)))") }
         return out.map { Data(bytes: $0, count: outLen) } ?? Data()
     }
 }

@@ -5,7 +5,8 @@ bench.py stays the headline (config 2, Deflate).  Each workload prints one JSON 
 with the batch resident in HBM, the HBM roofline fraction of the (single) kernel, and the CPU restatement's throughput.
 Unit counts are scaled to one GPU / a few minutes (stated in `config`); distinct units are tiled on the device.
 `--workload lz4c` is the compress direction (LZ4.compress, LZ4+Compress.swift): it reports INPUT GB/s and prints a second
-line for single LZ4.compress(data:) calls of 256 MiB.
+line for single LZ4.compress(data:) calls of 256 MiB.  `--workload deflatec` does the same for Deflate.compress
+(Deflate+Compress.swift), with single calls of 256 MiB of text-like data and of zeros.
 """
 import argparse
 import ctypes as C
@@ -175,9 +176,94 @@ def run_lz4c(args):
                       "host_buffers": True, "calls": single}))
 
 
+def run_deflatec(args):
+    """Deflate compression: independent 64 KiB units of the lz4 mix through swc_deflate_compress_batch, then single
+    Deflate.compress calls of 256 MiB (one parse thread each)"""
+    import torch
+    import swco_deflatec
+    from swcompression_b200 import Deflate, _lib
+    from swcompression_b200.batch import Batch
+    n_units = args.units or 262144
+    distinct = min(2048, n_units)
+    tile = max(n_units // distinct, 1)
+    n_units = tile * distinct
+    with Pool(min(os.cpu_count() or 1, 32)) as pool:
+        raws = pool.map(_raw64k, range(3, 3 + distinct), chunksize=1)
+    dev = torch.device("cuda:0")
+    L = _lib.lib()
+    one = torch.from_numpy(np.frombuffer(b"".join(raws), dtype=np.uint8).copy()).to(dev)
+    d_in = torch.cat([one.repeat(tile), torch.zeros(64, dtype=torch.uint8, device=dev)])
+    del one
+    offs = np.arange(n_units, dtype=np.uint64) * np.uint64(65536)
+    cap = (9 * 65536 + 17) // 8
+    b = Batch("deflate_compress", np.zeros(1, dtype=np.uint8), offs, np.full(n_units, 65536, dtype=np.uint64), cap, device=str(dev))
+    b.d_in = d_in
+    for _ in range(args.warmup):
+        b.run()
+    st, ln, _ = b.results()
+    assert (st == 0).all()
+    pc = (cap + 15) // 16 * 16
+    sample = list(range(min(distinct, 16)))
+    host = b.d_out[: len(sample) * pc].cpu().numpy()
+    for i in sample:
+        assert bytes(host[i * pc:i * pc + int(ln[i])]) == swco_deflatec.deflate_compress(raws[i])[1], "parity vs oracle failed"
+    total_in, total_out = n_units * 65536, int(ln.sum())
+    L.swc_timing_collect.argtypes = [C.c_void_p, C.c_int32]
+    L.swc_timing_enable(1)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    e0.record()
+    for _ in range(args.steps):
+        b.run()
+    e1.record()
+    torch.cuda.synchronize()
+    ms = e0.elapsed_time(e1) / args.steps
+    tbuf = (C.c_float * 4096)()
+    nint = L.swc_timing_collect(tbuf, 4096)
+    L.swc_timing_enable(0)
+    # every slice drops marks before link_kernel and after each of the four kernels: the intervals run link, parse, emit,
+    # seam, then the host's planning of the next slice
+    per = [sum(float(tbuf[i]) for i in range(k, nint, 5)) / args.steps for k in range(5)]
+    cpu = None
+    if not args.no_cpu:
+        threads = os.cpu_count() or 1
+        sec, _, fails = swco_deflatec.batch_mt(raws, max(threads * 4, 64), threads)
+        total = max(int(8.0 / (sec / max(threads * 4, 64))), threads)
+        sec, _, fails = swco_deflatec.batch_mt(raws, total, threads)
+        assert fails == 0
+        cpu = {"value": total * 65536 / sec / 1e9, "unit": "GB/s (input)", "cores": threads, "kind": "port",
+               "sample": f"{total} units in {sec:.1f} s on {threads} pthreads (oracle/deflate_compress.c)"}
+    del b, d_in
+    torch.cuda.empty_cache()
+    print(json.dumps({
+        "metric": "compressed_input_GB_per_s", "value": total_in / (ms * 1e-3) / 1e9, "unit": "GB/s", "n_gpus": 1,
+        "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms, "higher_is_better": True, "data": "synthetic",
+        "config": {"workload": "Deflate compression, Deflate+Compress.swift parse: independent 64 KiB units (80 % text-like, "
+                               "10 % zeros, 10 % incompressible)", "units": n_units, "distinct_units": distinct,
+                   "input_bytes": total_in, "compressed_bytes": total_out},
+        "kernel_ms_link_parse_emit_seam": [round(x, 3) for x in per[:4]], "between_slices_ms": round(per[4], 3),
+        "cpu_baseline": cpu}))
+    # one Deflate.compress(data:) call of 256 MiB is one unit: one parse thread
+    calls = {}
+    import helpers as H
+    text = b"".join(H.textlike(65536, 9000 + i) for i in range(256))
+    for label, data in (("textlike", text * 16), ("zeros", bytes(256 << 20))):
+        t0 = time.perf_counter()
+        out = Deflate.compress(data)
+        dt = time.perf_counter() - t0
+        t0 = time.perf_counter()
+        ref = swco_deflatec.deflate_compress(data)[1]
+        dc = time.perf_counter() - t0
+        assert out == ref, "parity vs oracle failed"
+        calls[label] = {"gpu_seconds": round(dt, 3), "cpu_restatement_seconds_1_thread": round(dc, 3),
+                        "input_GB_per_s": len(data) / dt / 1e9, "compressed_bytes": len(out)}
+    print(json.dumps({"metric": "single_call_input_GB_per_s", "unit": "GB/s", "input_bytes": 256 << 20,
+                      "host_buffers": True, "calls": calls}))
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", choices=list(WORKLOADS) + ["lz4c"], required=True)
+    ap.add_argument("--workload", choices=list(WORKLOADS) + ["lz4c", "deflatec"], required=True)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--units", type=int, default=0)
@@ -185,6 +271,8 @@ def main():
     args = ap.parse_args()
     if args.workload == "lz4c":
         return run_lz4c(args)
+    if args.workload == "deflatec":
+        return run_deflatec(args)
     W = WORKLOADS[args.workload]
     n_units = args.units or W["units"]
     distinct = min(W["distinct"], n_units)
