@@ -197,13 +197,16 @@ int32_t swc_lzma_decompress_raw(const uint8_t *in, size_t in_len, int32_t lc, in
 int32_t swc_lzma2_decompress(const uint8_t *in, size_t in_len, uint8_t **out, size_t *out_len, size_t *consumed_bytes);
 /* one raw LZMA stream per unit (the ZIP / 7-Zip form, LZMA.decompress(data:properties:uncompressedSize:), LZMA.swift:56-61):
  * props[i] = lc | lp << 8 | pb << 16, dict_size[i] as in LZMAProperties, uncompressed_size[i] < 0 = nil (end marker).
- * lc + lp must be <= 4 in the batched form (the literal coders live in shared memory); other units report SWC_ERR_UNSUPPORTED. */
+ * lc + lp must be <= 4 in the batched form (the literal coders live in shared memory); other units report SWC_ERR_UNSUPPORTED,
+ * as do lc > 8, lp > 4 or pb > 4 here and in swc_lzma_decompress_raw: no properties byte expresses them. */
 int32_t swc_lzma_decompress_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
                                   const uint32_t *props, const int64_t *dict_size, const int64_t *uncompressed_size,
                                   uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
                                   uint64_t *out_len, uint64_t *consumed_bytes, int32_t *status,
                                   uint64_t n, void *cuda_stream);
-/* one raw LZMA2 stream per unit; dict_bytes[i] is the XZ filter property byte */
+/* one raw LZMA2 stream per unit; dict_bytes[i] is the XZ filter property byte.  The reference accepts any properties byte
+ * below 225 in a chunk (lc <= 8, lp <= 4), but here too the literal coders live in shared memory: a unit reaching an LZMA
+ * chunk with lc + lp > 4 reports SWC_ERR_UNSUPPORTED.  swc_lzma2_decompress and swc_xz_unarchive take such streams. */
 int32_t swc_lzma2_decompress_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
                                    const uint8_t *dict_bytes,
                                    uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,

@@ -259,7 +259,9 @@ int swco_lzma_decompress_raw(const uint8_t *in, size_t in_len, int lc, int lp, i
     d->lc = lc; d->lp = lp; d->pb = pb; d->dict_size = dict_size;
     d->uncompressed_size = uncompressed_size < 0 ? -1 : uncompressed_size;   /* LZMA.swift:69 nil -> -1 */
     int st;
-    if (lc < 0 || lp < 0 || pb < 0 || lc > 8 || lp > 4 || pb > 4) st = SWC_ERR_REFERENCE_TRAP; /* "no validation": OOB shifts/indices */
+    /* properties no properties byte can express: the reference ("no validation") decodes some such streams -- Swift's >> by
+       a negative count shifts left -- and traps on others; refused as valid input the engine does not take (DESIGN §6) */
+    if (lc < 0 || lp < 0 || pb < 0 || lc > 8 || lp > 4 || pb > 4) st = SWC_ERR_UNSUPPORTED;
     else if (reset_state(d)) st = SWC_ERR_OUTPUT_OVERFLOW;
     else st = lzma_decode(d);
     if (consumed) *consumed = d->rc.ip;

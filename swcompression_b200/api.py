@@ -104,9 +104,12 @@ class LZMAProperties:
     pb: int = 2
     dictionarySize: int = 1 << 24
 
-    def __post_init__(self):
-        if self.dictionarySize < (1 << 12):     # the reference's didSet clamp (it does not fire in Swift's init, but the
-            pass                                # memberwise init assigns through the property: LZMAProperties.swift:39-44)
+    def __setattr__(self, name, value):
+        # the reference's didSet (LZMAProperties.swift:26-32) raises a dictionarySize below 4096 to 4096 when the property is
+        # assigned; Swift does not call didSet from the type's own initializers, so the constructor keeps any value
+        if name == "dictionarySize" and "dictionarySize" in self.__dict__ and value < (1 << 12):
+            value = 1 << 12
+        object.__setattr__(self, name, value)
 
 
 class LZMA:

@@ -425,7 +425,8 @@ int32_t swc_lzma_decompress_raw(const uint8_t *in, size_t in_len, int32_t lc, in
     if (!out || !out_len) return SWC_ERR_INVALID_ARG;
     *out = nullptr; *out_len = 0;
     if (consumed_bytes) *consumed_bytes = 0;
-    if (lc < 0 || lp < 0 || pb < 0 || lc > 8 || lp > 4 || pb > 4) return SWC_ERR_REFERENCE_TRAP;   // "no validation": OOB in the reference
+    // properties no properties byte can express: the reference decodes some such streams and traps on others (DESIGN §6)
+    if (lc < 0 || lp < 0 || pb < 0 || lc > 8 || lp > 4 || pb > 4) return SWC_ERR_UNSUPPORTED;
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
     LzmaJob job; job.mode = lzma::MODE_RAW; job.dict_byte = 0;
@@ -480,7 +481,7 @@ int32_t swc_lzma2_decompress_batch(const uint8_t *in_base, const uint64_t *in_of
     a.mode = lzma::MODE_LZMA2; a.in_base = in_base; a.in_off = in_off; a.in_len = in_len; a.dict_bytes = dict_bytes;
     a.props = nullptr; a.dict_size = nullptr; a.usize = nullptr;
     a.out_base = out_base; a.out_off = out_off; a.out_cap = out_cap; a.out_len = out_len; a.consumed = consumed_bytes;
-    a.status = status; a.n = n; a.lit_scratch = nullptr;      // LZMA2 requires lc + lp <= 4: the literal coders fit in shared memory
+    a.status = status; a.n = n; a.lit_scratch = nullptr;      // a chunk with lc + lp > 4 would need 6 MB of literal coders: refused here
     return lzma::launch(a, (cudaStream_t)cuda_stream);
 }
 

@@ -145,7 +145,6 @@ struct Dec {
             if (bit(&probs[(state << 4) + pos_state]) == 0) {                        // literal :119-172
                 if (trap) return SWC_ERR_REFERENCE_TRAP;
                 if (usize == 0) return SWC_LZMA_EXCEEDED_UNCOMPRESSED_SIZE;
-                if ((u64)dict_end >= cap) return SWC_ERR_OUTPUT_OVERFLOW;
                 const u32 prev = dict_end == dict_start ? 0 : prev_byte;
                 int symbol = 1;
                 u16 *lpz = lit + ((((u32)dict_end & lp_mask) << lc) + (prev >> (8 - lc))) * 0x300;
@@ -165,6 +164,8 @@ struct Dec {
                     while (symbol < 0x100) symbol = (symbol << 1) | bit(&lpz[symbol]);
                 }
                 if (trap) return SWC_ERR_REFERENCE_TRAP;
+                // capacity is checked once the literal is known to decode: a stream cut inside it traps in the reference
+                if ((u64)dict_end >= cap) return SWC_ERR_OUTPUT_OVERFLOW;
                 usize -= 1;
                 put((u32)symbol - 0x100);
                 state = state < 4 ? 0 : (state < 10 ? state - 3 : state - 6);
@@ -284,7 +285,9 @@ __global__ void __launch_bounds__(WARPS * 32) lzma_kernel(Args a) {
         d.lc = pr & 0xFF; d.lp = (pr >> 8) & 0xFF; d.pb = (pr >> 16) & 0xFF;
         d.dict_size = a.dict_size[unit];
         d.usize = a.usize[unit] < 0 ? -1 : a.usize[unit];
-        if (d.lc > 8 || d.lp > 4 || d.pb > 4) st = SWC_ERR_REFERENCE_TRAP;
+        // no properties byte holds these; the reference decodes some such streams (Swift's >> by a negative count shifts
+        // left) and traps on others, the engine takes none of them (DESIGN §6)
+        if (d.lc > 8 || d.lp > 4 || d.pb > 4) st = SWC_ERR_UNSUPPORTED;
         else { d.reset_state(lit_global); st = d.decode(); }
     } else {
         // LZMA2Decoder.init + decode()  LZMA2Decoder.swift:17-53
