@@ -171,6 +171,35 @@ int32_t swc_deflate_compress_batch(const uint8_t *in_base, const uint64_t *in_of
                                    uint64_t *out_len, int32_t *status, uint64_t n,
                                    void *scratch, size_t scratch_bytes, void *cuda_stream);
 
+/* ---- BZip2 compression ---------------------------------------------------------------------------------------
+ * BZip2.compress(data:) / compress(data:blockSize:)   Sources/BZip2/BZip2+Compress.swift:19-74
+ * block_size is BlockSize.rawValue (1 = .one ... 9 = .nine); any other value returns SWC_ERR_INVALID_ARG.  The output
+ * bytes equal the reference's: raw blocks of 80 000 x block_size bytes, its table choice and its code lengths (libbz2
+ * and the engine's own decoder read them).  The reference cannot fail, so there are no other statuses; inputs of
+ * 2^40 bytes or more return SWC_ERR_UNSUPPORTED.
+ * swc_bzip2_compress_max_bytes is the proved largest stream for in_len bytes (DESIGN.md §4.11, lemma 4):
+ *   14 + ceil(sum over raw blocks of r bytes, R = r + floor(r / 4), of
+ *             (395 + 6 ceil((R + 1) / 50) + 6 x 283 + 11 (R + 1)) / 8)   (with the 4 header and 10 EOS bytes summed
+ *   as bits: 112 + that sum, rounded up to bytes).
+ * Device memory: a unit is never split across slices, so one unit of n bytes needs about 40 n bytes of device scratch
+ * (swc_bzip2_compress_batch_scratch_bytes(1, n, k)) besides its input and output.  The single call takes it from the
+ * library's grow-only pool, which keeps it for later calls (swc_release_scratch frees it).  On an 80 GB card that caps
+ * one call at about 1.8 GB of input; a larger input returns SWC_ERR_CUDA (the allocation fails) rather than a stream. */
+int32_t swc_bzip2_compress(const uint8_t *in, size_t in_len, int32_t block_size, uint8_t **out, size_t *out_len);
+size_t  swc_bzip2_compress_max_bytes(uint64_t in_len, int32_t block_size);
+/* .bz2 streams, device memory, asynchronous on `cuda_stream` (the unit sizes are read back first, which synchronises).
+ * Unit i compresses in_base[in_off[i] ..+ in_len[i]) (any alignment) into one complete stream at out_base + out_off[i]
+ * (any alignment).  out_len[i] is the exact stream size; if it exceeds out_cap[i] the unit reports
+ * SWC_ERR_OUTPUT_OVERFLOW and writes nothing.  Nothing outside [out_off[i], out_off[i] + out_len[i]) is written.  The
+ * result depends only on the unit's bytes and block_size.  scratch may be NULL (library pool); a caller's scratch of
+ * swc_bzip2_compress_batch_scratch_bytes(n, sum of in_len[i], block_size) bytes runs the batch in one slice, a
+ * smaller one in several (it must hold the largest unit, else SWC_ERR_INVALID_ARG). */
+size_t  swc_bzip2_compress_batch_scratch_bytes(uint64_t n, uint64_t in_bytes_total, int32_t block_size);
+int32_t swc_bzip2_compress_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, int32_t block_size,
+                                 uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                 uint64_t *out_len, int32_t *status, uint64_t n,
+                                 void *scratch, size_t scratch_bytes, void *cuda_stream);
+
 /* ---- BZip2--------------------------------------------------------------------------------------------------
  * BZip2.decompress(data:)            Sources/BZip2/BZip2.swift:22-26
  * BZip2.multiDecompress(data:)       Sources/BZip2/BZip2.swift:40-48

@@ -71,6 +71,12 @@ def lib():
         L.swc_deflate_compress_batch_scratch_bytes.restype = C.c_size_t
         L.swc_deflate_compress_batch_scratch_bytes.argtypes = [C.c_uint64, C.c_uint64]
         L.swc_deflate_compress_batch.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, u64, vp, sz, vp]
+        L.swc_bzip2_compress.argtypes = [vp, sz, i32, C.POINTER(vp), szp]
+        L.swc_bzip2_compress_max_bytes.restype = C.c_size_t
+        L.swc_bzip2_compress_max_bytes.argtypes = [C.c_uint64, i32]
+        L.swc_bzip2_compress_batch_scratch_bytes.restype = C.c_size_t
+        L.swc_bzip2_compress_batch_scratch_bytes.argtypes = [C.c_uint64, C.c_uint64, i32]
+        L.swc_bzip2_compress_batch.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp, u64, vp, sz, vp]
         L.swc_bzip2_decompress.argtypes = [vp, sz, sz, C.POINTER(vp), szp, szp]
         L.swc_bzip2_multi_decompress.argtypes = [vp, sz, C.POINTER(vp), szp, C.POINTER(vp), szp]
         L.swc_bzip2_decompress_batch.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, u64, vp]

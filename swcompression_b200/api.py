@@ -19,6 +19,7 @@ meaning, same error cases), routed through the C ABI of libswcgpu.so.
 """
 import ctypes as C
 import datetime
+import enum
 from dataclasses import dataclass, field
 
 from . import _lib
@@ -85,7 +86,30 @@ class Deflate:
 
 
 class BZip2:
-    """Sources/BZip2/BZip2.swift:10-48"""
+    """Sources/BZip2/BZip2.swift:10-48, Sources/BZip2/BZip2+Compress.swift:19-74"""
+
+    class BlockSize(enum.IntEnum):
+        """BZip2+BlockSize.swift: raw blocks of 80 000 x rawValue bytes, header byte '0' + rawValue"""
+        one = 1
+        two = 2
+        three = 3
+        four = 4
+        five = 5
+        six = 6
+        seven = 7
+        eight = 8
+        nine = 9
+
+    @staticmethod
+    def compress(data, blockSize=None):
+        """BZip2.compress(data:) (blockSize .one) and compress(data:blockSize:): equal to the reference byte for byte."""
+        k = 1 if blockSize is None else int(blockSize)
+        return _compressed("swc_bzip2_compress", data, C.c_int32(k))
+
+    @staticmethod
+    def max_compressed_size(n, blockSize=None):
+        """the largest stream compress(data:blockSize:) writes for n bytes (DESIGN.md §4.11)"""
+        return int(_lib.lib().swc_bzip2_compress_max_bytes(n, 1 if blockSize is None else int(blockSize)))
 
     @staticmethod
     def decompress(data):

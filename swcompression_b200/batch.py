@@ -37,9 +37,12 @@ class Batch:
     (dict_off, dict_len) pair of u64 arrays placing each unit's dictionary window inside `in_buf`.
     'deflate_compress' compresses each unit into a raw Deflate stream (Deflate.compress, Deflate+Compress.swift:22-42); a
     unit of n bytes needs at most (9 n + 17) // 8 bytes of output.  `scratch_bytes` caps the caller scratch it passes
-    (the library then runs the batch in slices)."""
+    (the library then runs the batch in slices).
+    'bzip2_compress' compresses each unit into a complete .bz2 stream (BZip2.compress(data:blockSize:),
+    BZip2+Compress.swift:44-74) with raw blocks of 80 000 x `block_size` bytes; api.BZip2.max_compressed_size gives the
+    output a unit may need.  `scratch_bytes` caps the caller scratch as for 'deflate_compress'."""
 
-    def __init__(self, codec, in_buf, in_off, in_len, out_cap, device="cuda:0", aux=None, scratch_bytes=None):
+    def __init__(self, codec, in_buf, in_off, in_len, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=1):
         self.codec = codec
         self.device = torch.device(device)
         self.n = len(in_off)
@@ -80,14 +83,21 @@ class Batch:
             if scratch_bytes is not None:
                 nbytes = min(nbytes, int(scratch_bytes))
             self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        self.block_size = int(block_size)
+        if codec == "bzip2_compress":
+            total = int(np.asarray(in_len, dtype=np.uint64).sum())
+            nbytes = min(_lib.lib().swc_bzip2_compress_batch_scratch_bytes(self.n, total, max(1, min(9, self.block_size))), 16 << 30)
+            if scratch_bytes is not None:
+                nbytes = min(nbytes, int(scratch_bytes))
+            self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         if codec == "deflate":
             nbytes = _lib.lib().swc_deflate_batch_scratch_bytes(self.n, self.out_total)
             self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
 
     @classmethod
-    def from_units(cls, codec, units, out_cap, device="cuda:0", aux=None, scratch_bytes=None):
+    def from_units(cls, codec, units, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=1):
         buf, offs, lens = pack_units(units)
-        return cls(codec, buf, offs, lens, out_cap, device, aux, scratch_bytes)
+        return cls(codec, buf, offs, lens, out_cap, device, aux, scratch_bytes, block_size)
 
     def run(self):
         L = _lib.lib()
@@ -112,6 +122,10 @@ class Batch:
             st = L.swc_deflate_compress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out), p(self.d_out_off),
                                               p(self.d_out_cap), p(self.d_out_len), p(self.d_status), self.n, p(self.d_scratch),
                                               self.d_scratch.numel(), stream)
+        elif self.codec == "bzip2_compress":
+            st = L.swc_bzip2_compress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), self.block_size, p(self.d_out),
+                                            p(self.d_out_off), p(self.d_out_cap), p(self.d_out_len), p(self.d_status), self.n,
+                                            p(self.d_scratch), self.d_scratch.numel(), stream)
         elif self.codec == "bzip2":
             st = L.swc_bzip2_decompress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out), p(self.d_out_off),
                                               p(self.d_out_cap), p(self.d_out_len), p(self.d_consumed), p(self.d_status), self.n, stream)

@@ -1,7 +1,7 @@
 // Public decode API of the reference, bodies routed through libswcgpu (include/swcgpu.h).
 //   DecompressionAlgorithm  Sources/Common/DecompressionAlgorithm.swift:9-14
 //   Archive                 Sources/Common/Archive.swift:9-14
-//   CompressionAlgorithm    Sources/Common/CompressionAlgorithm.swift (LZ4 and Deflate are its GPU-backed conformers here)
+//   CompressionAlgorithm    Sources/Common/CompressionAlgorithm.swift (LZ4, Deflate and BZip2 are its GPU-backed conformers here)
 import CSWCGPU
 import Foundation
 
@@ -138,6 +138,17 @@ private func compressed(_ name: String, _ data: Data, _ body: (UnsafePointer<UIn
 extension Deflate: CompressionAlgorithm {                            // Sources/Deflate/Deflate+Compress.swift:10-42
     public static func compress(data: Data) -> Data {
         compressed("Deflate.compress", data) { p, n, o, ol in swc_deflate_compress(p, n, o, ol) }
+    }
+}
+
+extension BZip2: CompressionAlgorithm {                              // Sources/BZip2/BZip2+Compress.swift:19-74
+    /// BZip2+BlockSize.swift: raw blocks of 80 000 x rawValue bytes.
+    public enum BlockSize: Int {
+        case one = 1, two, three, four, five, six, seven, eight, nine
+    }
+    public static func compress(data: Data) -> Data { compress(data: data, blockSize: .one) }
+    public static func compress(data: Data, blockSize: BlockSize) -> Data {
+        compressed("BZip2.compress", data) { p, n, o, ol in swc_bzip2_compress(p, n, Int32(blockSize.rawValue), o, ol) }
     }
 }
 

@@ -6,7 +6,9 @@ with the batch resident in HBM, the HBM roofline fraction of the (single) kernel
 Unit counts are scaled to one GPU / a few minutes (stated in `config`); distinct units are tiled on the device.
 `--workload lz4c` is the compress direction (LZ4.compress, LZ4+Compress.swift): it reports INPUT GB/s and prints a second
 line for single LZ4.compress(data:) calls of 256 MiB.  `--workload deflatec` does the same for Deflate.compress
-(Deflate+Compress.swift), with single calls of 256 MiB of text-like data and of zeros.
+(Deflate+Compress.swift), with single calls of 256 MiB of text-like data and of zeros.  `--workload bzip2c` does the
+same for BZip2.compress (BZip2+Compress.swift) in two batched shapes, 720 000-byte units at .nine and 80 000-byte units
+at .one, with the per-kernel split, and single calls of 256 MiB at .one.
 """
 import argparse
 import ctypes as C
@@ -261,9 +263,108 @@ def run_deflatec(args):
                       "host_buffers": True, "calls": calls}))
 
 
+def _bzip2c_unit(arg):
+    import helpers as H
+    seed, size = arg
+    rng = np.random.Generator(np.random.PCG64(seed))
+    k = rng.random()
+    return bytes(size) if k < 0.1 else rng.integers(0, 256, size, dtype=np.uint8).tobytes() if k < 0.2 else H.textlike(size, seed)
+
+
+BZIP2C_STAGES = ["rle", "sort", "mtf", "group", "select", "layout", "header_emit", "copy", "between_slices"]
+
+
+def run_bzip2c(args):
+    """BZip2 compression: independent units of the lz4 mix (80 % text-like, 10 % zeros, 10 % random) through
+    swc_bzip2_compress_batch at .nine (720 000 B: one full block each) and .one (80 000 B), then single
+    BZip2.compress(data:) calls of 256 MiB"""
+    import torch
+    import swco_bzip2c
+    from swcompression_b200 import BZip2, _lib
+    from swcompression_b200.batch import Batch
+    dev = torch.device("cuda:0")
+    L = _lib.lib()
+    L.swc_timing_collect.argtypes = [C.c_void_p, C.c_int32]
+    for label, size, k, distinct in (("nine", 720000, 9, 128), ("one", 80000, 1, 128)):
+        n_units = args.units or (1 << 30) // size
+        tile = max(n_units // distinct, 1)
+        n_units = tile * distinct
+        with Pool(min(os.cpu_count() or 1, 32)) as pool:
+            raws = pool.map(_bzip2c_unit, [(seed, size) for seed in range(11, 11 + distinct)], chunksize=1)
+        one = torch.from_numpy(np.frombuffer(b"".join(raws), dtype=np.uint8).copy()).to(dev)
+        d_in = torch.cat([one.repeat(tile), torch.zeros(64, dtype=torch.uint8, device=dev)])
+        del one
+        offs = np.arange(n_units, dtype=np.uint64) * np.uint64(size)
+        cap = BZip2.max_compressed_size(size, k)
+        b = Batch("bzip2_compress", np.zeros(1, dtype=np.uint8), offs, np.full(n_units, size, dtype=np.uint64), cap,
+                  device=str(dev), block_size=k)
+        b.d_in = d_in
+        for _ in range(args.warmup):
+            b.run()
+        st, ln, _ = b.results()
+        assert (st == 0).all()
+        pc = (cap + 15) // 16 * 16
+        sample = list(range(min(distinct, 16)))
+        host = b.d_out[: len(sample) * pc].cpu().numpy()
+        for i in sample:
+            assert bytes(host[i * pc:i * pc + int(ln[i])]) == swco_bzip2c.bzip2_compress(raws[i], k)[1], "parity vs oracle failed"
+        total_in, total_out = n_units * size, int(ln.sum())
+        L.swc_timing_enable(1)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize()
+        e0.record()
+        for _ in range(args.steps):
+            b.run()
+        e1.record()
+        torch.cuda.synchronize()
+        ms = e0.elapsed_time(e1) / args.steps
+        tbuf = (C.c_float * 4096)()
+        nint = L.swc_timing_collect(tbuf, 4096)
+        L.swc_timing_enable(0)
+        # every slice drops a mark in front and one after each of its 8 stages; the 9th interval is the host's planning
+        # of the next slice
+        per = {name: round(sum(float(tbuf[i]) for i in range(j, nint, 9)) / args.steps, 3)
+               for j, name in enumerate(BZIP2C_STAGES)}
+        cpu = None
+        if not args.no_cpu:
+            threads = os.cpu_count() or 1
+            sec, _, fails = swco_bzip2c.batch_mt(raws, threads * 2, threads, k)
+            total = max(int(8.0 / (sec / (threads * 2))), threads)
+            sec, _, fails = swco_bzip2c.batch_mt(raws, total, threads, k)
+            assert fails == 0
+            cpu = {"value": total * size / sec / 1e9, "unit": "GB/s (input)", "cores": threads, "kind": "port",
+                   "sample": f"{total} units in {sec:.1f} s on {threads} pthreads (oracle/bzip2_compress.c)"}
+        del b, d_in
+        torch.cuda.empty_cache()
+        print(json.dumps({
+            "metric": "compressed_input_GB_per_s", "value": total_in / (ms * 1e-3) / 1e9, "unit": "GB/s", "n_gpus": 1,
+            "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms, "higher_is_better": True, "data": "synthetic",
+            "config": {"workload": f"BZip2 compression at .{label}, BZip2+Compress.swift: independent {size}-byte units "
+                                   "(80 % text-like, 10 % zeros, 10 % incompressible)", "units": n_units,
+                       "distinct_units": distinct, "input_bytes": total_in, "compressed_bytes": total_out},
+            "kernel_ms": per, "cpu_baseline": cpu, "gpu_name": torch.cuda.get_device_name(dev)}), flush=True)
+    # one BZip2.compress(data:) call of 256 MiB: 3 356 blocks at .one
+    calls = {}
+    import helpers as H
+    text = b"".join(H.textlike(65536, 9000 + i) for i in range(64))
+    for label, data in (("textlike", text * 64), ("zeros", bytes(256 << 20))):
+        BZip2.compress(data[: 1 << 20])
+        t0 = time.perf_counter()
+        out = BZip2.compress(data)
+        dt = time.perf_counter() - t0
+        t0 = time.perf_counter()
+        ref = swco_bzip2c.bzip2_compress(data, 1)[1]
+        dc = time.perf_counter() - t0
+        assert out == ref, "parity vs oracle failed"
+        calls[label] = {"gpu_seconds": round(dt, 3), "cpu_restatement_seconds_1_thread": round(dc, 3),
+                        "input_GB_per_s": len(data) / dt / 1e9, "compressed_bytes": len(out)}
+    print(json.dumps({"metric": "single_call_input_GB_per_s", "unit": "GB/s", "input_bytes": 256 << 20,
+                      "host_buffers": True, "block_size": 1, "calls": calls}))
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", choices=list(WORKLOADS) + ["lz4c", "deflatec"], required=True)
+    ap.add_argument("--workload", choices=list(WORKLOADS) + ["lz4c", "deflatec", "bzip2c"], required=True)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--units", type=int, default=0)
@@ -273,6 +374,8 @@ def main():
         return run_lz4c(args)
     if args.workload == "deflatec":
         return run_deflatec(args)
+    if args.workload == "bzip2c":
+        return run_bzip2c(args)
     W = WORKLOADS[args.workload]
     n_units = args.units or W["units"]
     distinct = min(W["distinct"], n_units)
