@@ -159,7 +159,8 @@ __device__ __forceinline__ void lz4_block_body(const Args &a) {
 //      positions; literals (sources in the compressed block: no hazards) are copied first, then matches run 8 at a time on
 //      4-lane sub-groups under the same "oldest pending record" readiness rule as the Deflate resolve kernel; long copies
 //      (>= 64 bytes: incompressible or zero-filled blocks) are done by the whole warp.
-// Units whose lengths do not fit 24 bits are flagged for the one-kernel decoder above.
+// Units whose lengths do not fit 24 bits, and units that read or write 4 GiB or more, are flagged for the one-kernel
+// decoder above.
 constexpr int LZ4_INTERNAL_FALLBACK = 9002;
 
 __device__ __forceinline__ u32 ext_bytes(u32 len_field_value /* length minus its base */) {
@@ -215,6 +216,9 @@ __global__ void __launch_bounds__(128) lz4_parse_kernel(Args a, const u64 *rec_b
         op += mlen;
     }
     if (status == SWC_OK && op > cap) status = SWC_ERR_OUTPUT_OVERFLOW;
+    // the exec kernel keeps input and output positions in 32 bits: a block that reads or writes 4 GiB or more goes to the
+    // fallback (after the capacity check, so that an overflowing unit still reports its exact size)
+    if (status == SWC_OK && ((op >> 32) != 0 || (n >> 32) != 0)) status = LZ4_INTERNAL_FALLBACK;
     a.out_len[unit] = op;
     a.status[unit] = status;
     rec_count[unit] = nrec;
