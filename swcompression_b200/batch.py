@@ -15,6 +15,29 @@ def _align(v, a=16):
     return (v + a - 1) // a * a
 
 
+# the most scratch a compress Batch allocates: past it the library runs the batch in slices that fit
+COMPRESS_SCRATCH_LIMIT = 16 << 30
+
+
+def compress_scratch_bytes(codec, in_len, dict_len=None, block_size=1):
+    """The scratch that runs a compress batch of units of `in_len` bytes in one slice, capped at COMPRESS_SCRATCH_LIMIT.
+    `dict_len` are the LZ4 units' dictionary window lengths (None: no dictionaries)."""
+    L = _lib.lib()
+    lens = np.asarray(in_len, dtype=np.uint64)
+    n, total = len(lens), int(lens.sum())
+    if codec == "lz4_block_compress":
+        if dict_len is not None:
+            total += int(np.minimum(np.asarray(dict_len, dtype=np.uint64), np.uint64(65536)).sum())
+        nbytes = L.swc_lz4_compress_batch_scratch_bytes(n, total)
+    elif codec == "deflate_compress":
+        nbytes = L.swc_deflate_compress_batch_scratch_bytes(n, total)
+    elif codec == "bzip2_compress":
+        nbytes = L.swc_bzip2_compress_batch_scratch_bytes(n, total, max(1, min(9, int(block_size))))
+    else:
+        raise ValueError(codec)
+    return min(nbytes, COMPRESS_SCRATCH_LIMIT)
+
+
 def pack_units(units, align=16):
     """list of bytes -> (uint8 numpy buffer, offsets u64, lengths u64)"""
     lens = np.fromiter((len(u) for u in units), dtype=np.uint64, count=len(units))
@@ -36,11 +59,13 @@ class Batch:
     'lz4_block_compress' compresses each unit into a raw LZ4 block (LZ4+Compress.swift:156-277); `aux` is then an optional
     (dict_off, dict_len) pair of u64 arrays placing each unit's dictionary window inside `in_buf`.
     'deflate_compress' compresses each unit into a raw Deflate stream (Deflate.compress, Deflate+Compress.swift:22-42); a
-    unit of n bytes needs at most (9 n + 17) // 8 bytes of output.  `scratch_bytes` caps the caller scratch it passes
-    (the library then runs the batch in slices).
+    unit of n bytes needs at most (9 n + 17) // 8 bytes of output.
     'bzip2_compress' compresses each unit into a complete .bz2 stream (BZip2.compress(data:blockSize:),
     BZip2+Compress.swift:44-74) with raw blocks of 80 000 x `block_size` bytes; api.BZip2.max_compressed_size gives the
-    output a unit may need.  `scratch_bytes` caps the caller scratch as for 'deflate_compress'."""
+    output a unit may need.
+    The three compress codecs pass a caller scratch of compress_scratch_bytes(...), which runs the batch in one slice up
+    to COMPRESS_SCRATCH_LIMIT; `scratch_bytes` caps it lower (the library then runs the batch in slices; a scratch that
+    cannot hold the largest unit fails the run with SWC_ERR_INVALID_ARG)."""
 
     def __init__(self, codec, in_buf, in_off, in_len, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=1):
         self.codec = codec
@@ -65,28 +90,15 @@ class Batch:
         self.d_status = torch.full((self.n,), -1, dtype=torch.int32, device=self.device)
         self.d_scratch = None
         self.d_dict_off = self.d_dict_len = None
+        self.block_size = int(block_size)
         if codec == "lz4_block_compress":
             self.d_aux = None
-            dl = np.zeros(self.n, dtype=np.uint64)
             if aux is not None:
                 self.d_dict_off, self.d_dict_len = t(np.asarray(aux[0], dtype=np.uint64)), t(np.asarray(aux[1], dtype=np.uint64))
-                dl = np.asarray(aux[1], dtype=np.uint64)
-            window = int(np.asarray(in_len, dtype=np.uint64).sum()) + int(np.minimum(dl, np.uint64(65536)).sum())
-            # past 16 GiB of scratch the library runs the batch in slices that fit
-            nbytes = min(_lib.lib().swc_lz4_compress_batch_scratch_bytes(self.n, window), 16 << 30)
-            self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         else:
             self.d_aux = None if aux is None else torch.from_numpy(np.frombuffer(bytes(aux), dtype=np.uint8).copy()).to(self.device)
-        if codec == "deflate_compress":
-            total = int(np.asarray(in_len, dtype=np.uint64).sum())
-            nbytes = min(_lib.lib().swc_deflate_compress_batch_scratch_bytes(self.n, total), 16 << 30)
-            if scratch_bytes is not None:
-                nbytes = min(nbytes, int(scratch_bytes))
-            self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        self.block_size = int(block_size)
-        if codec == "bzip2_compress":
-            total = int(np.asarray(in_len, dtype=np.uint64).sum())
-            nbytes = min(_lib.lib().swc_bzip2_compress_batch_scratch_bytes(self.n, total, max(1, min(9, self.block_size))), 16 << 30)
+        if codec in ("lz4_block_compress", "deflate_compress", "bzip2_compress"):
+            nbytes = compress_scratch_bytes(codec, in_len, None if aux is None else aux[1], self.block_size)
             if scratch_bytes is not None:
                 nbytes = min(nbytes, int(scratch_bytes))
             self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)

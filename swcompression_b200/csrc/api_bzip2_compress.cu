@@ -1,44 +1,20 @@
 // api_bzip2_compress.cu — C ABI for BZip2 compression: .bz2 stream batches in device memory, and the single call
 // BZip2.compress(data:blockSize:) (BZip2+Compress.swift:44-74).
-#include <cstring>
 #include <vector>
 #include "../../include/swcgpu.h"
-#include "host_util.h"
+#include "compress_host.h"
 #include "bzip2_compress.cuh"
 
 using namespace swc;
 
 namespace {
 
-constexpr u64 kCompressPoolLimit = 16ull << 30;      // library-pool scratch per slice of a compress batch
-
-int batch_impl(const bzip2c::Args &a, const std::vector<uint64_t> &lens, void *scratch, size_t scratch_bytes, cudaStream_t s) {
+int batch_impl(const bzip2c::Args &a, const std::vector<u64> &lens, void *scratch, size_t scratch_bytes, cudaStream_t s) {
     using namespace bzip2c;
-    const u64 n = a.n, raw = (u64)RAW_PER_LEVEL * a.level;
-    u64 total = 4096, biggest = 0;
-    for (u64 i = 0; i < n; i++) {
-        const u64 need = unit_scratch(lens[i], a.level);
-        total += need;
-        if (need > biggest) biggest = need;
-    }
-    size_t cap = scratch_bytes;
-    if (!scratch) {
-        cap = (size_t)(total < kCompressPoolLimit ? total : kCompressPoolLimit);
-        if (cap < 4096 + biggest) cap = (size_t)(4096 + biggest);
-        int st = scratch_get(cap, &scratch, s);
-        if (st) return st;
-    }
-    u8 *scr = (u8 *)scratch;
+    const u64 raw = (u64)RAW_PER_LEVEL * a.level;
     std::vector<u8> plan;
-    for (u64 first = 0; first < n;) {
-        u64 count = 0, used = 4096;
-        while (first + count < n) {
-            const u64 need = unit_scratch(lens[first + count], a.level);
-            if (used + need > cap) break;
-            used += need;
-            count++;
-        }
-        if (count == 0) return SWC_ERR_INVALID_ARG;                       // caller scratch smaller than one unit needs
+    return run_in_slices(a.n, [&](u64 i) { return unit_scratch(lens[i], a.level); }, [](u64) { return (u64)4096; }, scratch,
+                         scratch_bytes, s, [&](u64 first, u64 count, u8 *scr, size_t cap) -> int {
         // plans first, then per-block results, per-group results, block scratch and the units' staging words
         std::vector<BlockPlan> bl;
         std::vector<UnitPlan> un(count);
@@ -81,11 +57,8 @@ int batch_impl(const bzip2c::Args &a, const std::vector<uint64_t> &lens, void *s
         for (const UnitPlan &u : un) sl.max_stage = u.stage_bytes > sl.max_stage ? u.stage_bytes : sl.max_stage;
         sl.copy_chunk = 64 << 10;                                         // at most 65 535 chunks per unit
         while ((sl.max_stage + sl.copy_chunk - 1) / sl.copy_chunk > 65535) sl.copy_chunk *= 2;
-        int st = run(a, first, count, sl, s);
-        if (st) return st;
-        first += count;
-    }
-    return SWC_OK;
+        return run(a, first, count, sl, s);
+    });
 }
 
 }  // namespace
@@ -117,15 +90,12 @@ int32_t swc_bzip2_compress_batch(const uint8_t *in_base, const uint64_t *in_off,
     if (n == 0) return SWC_OK;
     if (!in_base || !in_off || !in_len || !out_base || !out_off || !out_cap || !out_len || !status) return SWC_ERR_INVALID_ARG;
     const cudaStream_t s = (cudaStream_t)cuda_stream;
-    std::vector<uint64_t> lens(n);
-    SWC_CUDA_TRY(cudaMemcpyAsync(lens.data(), in_len, n * 8, cudaMemcpyDeviceToHost, s));
-    SWC_CUDA_TRY(cudaStreamSynchronize(s));
+    std::vector<u64> lens;
+    int st = read_lens(in_len, n, s, lens);
+    if (st) return st;
     for (u64 l : lens)
         if (l >= (1ull << 40)) return SWC_ERR_UNSUPPORTED;
-    bzip2c::Args a;
-    a.in_base = in_base; a.in_off = in_off; a.in_len = in_len;
-    a.out_base = out_base; a.out_off = out_off; a.out_cap = out_cap; a.out_len = out_len; a.status = status; a.n = n;
-    a.level = (u32)block_size;
+    const bzip2c::Args a{{in_base, in_off, in_len, out_base, out_off, out_cap, out_len, status, n}, (u32)block_size};
     return batch_impl(a, lens, scratch, scratch_bytes, s);
 }
 
@@ -135,34 +105,8 @@ int32_t swc_bzip2_compress(const uint8_t *in, size_t in_len, int32_t block_size,
     *out = nullptr; *out_len = 0;
     if (block_size < 1 || block_size > 9) return SWC_ERR_INVALID_ARG;
     if ((u64)in_len >= (1ull << 40)) return SWC_ERR_UNSUPPORTED;
-    if (ensure_device()) return SWC_ERR_NO_DEVICE;
-    ApiLock api_lock;
-    DevBuf d_in, d_out;
-    int st;
-    if ((st = upload_input(d_in, in, in_len))) return st;
-    const u64 cap = round16(bzip2c::max_stream_bytes(in_len, (u32)block_size));
-    UnitTable t;
-    const Col<u64> in_off = t.in<u64>(1), c_len = t.in<u64>(1), out_off = t.in<u64>(1), out_cap = t.in<u64>(1);
-    const Col<u64> r_len = t.out<u64>(1);
-    const Col<int32_t> r_st = t.out<int32_t>(1);
-    if ((st = t.alloc()) || (st = d_out.alloc(cap))) return st;
-    *t.host(c_len) = in_len; *t.host(out_cap) = cap;
-    if ((st = t.upload())) return st;
-    bzip2c::Args a;
-    a.in_base = d_in.as<u8>(); a.in_off = t.dev(in_off); a.in_len = t.dev(c_len);
-    a.out_base = d_out.as<u8>(); a.out_off = t.dev(out_off); a.out_cap = t.dev(out_cap);
-    a.out_len = t.dev(r_len); a.status = t.dev(r_st); a.n = 1; a.level = (u32)block_size;
-    const std::vector<uint64_t> lens(1, in_len);
-    if ((st = batch_impl(a, lens, nullptr, 0, 0))) return st;
-    std::vector<u64> len;
-    std::vector<int32_t> status;
-    if ((st = t.fetch(r_len, len)) || (st = t.fetch(r_st, status))) return st;
-    if (status[0] != SWC_OK) return status[0];
-    uint8_t *host = (uint8_t *)swc_alloc((size_t)len[0]);
-    if (!host) return SWC_ERR_OUTPUT_OVERFLOW;
-    if ((st = copy_pageable(host, d_out.p, (size_t)len[0], false))) { swc_free(host); return st; }
-    *out = host; *out_len = (size_t)len[0];
-    return SWC_OK;
+    return compress_one(bzip2c::Args{{}, (u32)block_size}, batch_impl, bzip2c::max_stream_bytes(in_len, (u32)block_size), in,
+                        in_len, out, out_len);
 }
 
 }  // extern "C"

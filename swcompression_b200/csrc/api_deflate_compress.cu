@@ -2,53 +2,26 @@
 // Deflate.compress (Deflate+Compress.swift:22-42), ZlibArchive.archive (ZlibArchive.swift:54-70) and GzipArchive.archive
 // (GzipArchive.swift:126-241).  The stream and the CRC-32 / Adler-32 of the input are computed on the device; the host
 // writes the few framing bytes around them.
-#include <cstring>
 #include <vector>
 #include "../../include/swcgpu.h"
-#include "host_util.h"
+#include "compress_host.h"
 #include "deflate_compress.cuh"
-#include "checks.cuh"
 
 using namespace swc;
 
 namespace {
 
-constexpr u64 kCompressPoolLimit = 16ull << 30;      // library-pool scratch per slice of a compress batch
-
 inline u64 meta_bytes(u64 count) { return (3 * count + 2) * 8 + 3 * 256; }
 
 // the batch on device-resident tables; `lens` is the host copy of in_len
-int batch_impl(const deflatec::Args &a, const std::vector<uint64_t> &lens, void *scratch, size_t scratch_bytes, cudaStream_t s) {
-    const u64 n = a.n;
-    u64 total = meta_bytes(n), biggest = 0;
-    for (u64 i = 0; i < n; i++) {
-        const u64 need = deflatec::unit_scratch(lens[i]);
-        total += need;
-        if (need > biggest) biggest = need;
-    }
-    size_t cap = scratch_bytes;
-    if (!scratch) {
-        cap = (size_t)(total < kCompressPoolLimit ? total : kCompressPoolLimit);
-        if (cap < meta_bytes(1) + biggest) cap = (size_t)(meta_bytes(1) + biggest);
-        int st = scratch_get(cap, &scratch, s);
-        if (st) return st;
-    }
-    u8 *scr = (u8 *)scratch;
-    // a slice's plan first (scratch offsets, tile and chunk prefix sums), then each unit's region
-    std::vector<uint64_t> plan;
-    for (u64 first = 0; first < n;) {
-        u64 count = 0, used = 0;
-        while (first + count < n) {
-            const u64 need = deflatec::unit_scratch(lens[first + count]);
-            if (meta_bytes(count + 1) + used + need > cap) break;
-            used += need;
-            count++;
-        }
-        if (count == 0) return SWC_ERR_INVALID_ARG;                       // caller scratch smaller than one unit needs
-        const u64 mb = meta_bytes(count);
+int batch_impl(const deflatec::Args &a, const std::vector<u64> &lens, void *scratch, size_t scratch_bytes, cudaStream_t s) {
+    std::vector<u64> plan;
+    return run_in_slices(a.n, [&](u64 i) { return deflatec::unit_scratch(lens[i]); }, meta_bytes, scratch, scratch_bytes, s,
+                         [&](u64 first, u64 count, u8 *scr, size_t) -> int {
+        // the slice's plan first (scratch offsets, tile and chunk prefix sums), then each unit's region
         plan.assign(3 * count + 2, 0);
         u64 *off = plan.data(), *tiles = off + count, *chunks = tiles + count + 1;
-        u64 at = mb;
+        u64 at = meta_bytes(count);
         for (u64 j = 0; j < count; j++) {
             const u64 l = lens[first + j];
             off[j] = at; at += deflatec::unit_scratch(l);
@@ -60,37 +33,8 @@ int batch_impl(const deflatec::Args &a, const std::vector<uint64_t> &lens, void 
         deflatec::Plan p;
         p.scr_off = (const u64 *)scr; p.tile_start = p.scr_off + count; p.chunk_start = p.tile_start + count + 1;
         p.tiles = tiles[count]; p.chunks = chunks[count];
-        int st = deflatec::run(a, first, count, scr, p, s);
-        if (st) return st;
-        first += count;
-    }
-    return SWC_OK;
-}
-
-// Deflate.compress of d_in[0, n) into a new device buffer; *len = the stream's size
-int compress_device(const u8 *d_in, u64 n, DevBuf &d_out, u64 *len) {
-    if (n >= deflatec::MAX_UNIT) return SWC_ERR_UNSUPPORTED;
-    UnitTable t;
-    const Col<u64> in_off = t.in<u64>(1), in_len = t.in<u64>(1), out_off = t.in<u64>(1), out_cap = t.in<u64>(1);
-    const Col<u64> out_len = t.out<u64>(1);
-    const Col<int32_t> status = t.out<int32_t>(1);
-    const u64 cap = round16((9 * n + 17) / 8);               // the largest stream Deflate.compress writes for n bytes
-    int st;
-    if ((st = t.alloc()) || (st = d_out.alloc(cap))) return st;
-    *t.host(in_len) = n; *t.host(out_cap) = cap;
-    if ((st = t.upload())) return st;
-    deflatec::Args a;
-    a.in_base = d_in; a.in_off = t.dev(in_off); a.in_len = t.dev(in_len);
-    a.out_base = d_out.as<u8>(); a.out_off = t.dev(out_off); a.out_cap = t.dev(out_cap);
-    a.out_len = t.dev(out_len); a.status = t.dev(status); a.n = 1;
-    const std::vector<uint64_t> lens(1, n);
-    if ((st = batch_impl(a, lens, nullptr, 0, 0))) return st;
-    std::vector<u64> r_len;
-    std::vector<int32_t> r_st;
-    if ((st = t.fetch(out_len, r_len)) || (st = t.fetch(status, r_st))) return st;
-    if (r_st[0] != SWC_OK) return r_st[0];
-    *len = r_len[0];
-    return SWC_OK;
+        return deflatec::run(a, first, count, scr, p, s);
+    });
 }
 
 // one framed result: `head`, the Deflate stream of `in`, then `tail_len` bytes of trailer written by `tail`
@@ -98,26 +42,10 @@ template <typename Tail>
 int framed(const uint8_t *in, size_t in_len, const std::vector<uint8_t> &head, checks::Kind kind, size_t tail_len, Tail tail,
            uint8_t **out, size_t *out_len) {
     if (in_len >= deflatec::MAX_UNIT) return SWC_ERR_UNSUPPORTED;
-    if (ensure_device()) return SWC_ERR_NO_DEVICE;
-    ApiLock api_lock;
-    DevBuf d_in, d_out;
-    int st;
-    if ((st = upload_input(d_in, in, in_len))) return st;
-    u64 len = 0;
-    if ((st = compress_device(d_in.as<u8>(), in_len, d_out, &len))) return st;
-    u64 check = kind == checks::ADLER32 ? 1 : 0;
-    if (tail_len && in_len && (st = checks::check_device(kind, d_in.as<u8>(), in_len, &check))) return st;
-    const size_t total = head.size() + (size_t)len + tail_len;
-    uint8_t *host = (uint8_t *)swc_alloc(total);
-    if (!host) return SWC_ERR_OUTPUT_OVERFLOW;
-    if (!head.empty()) memcpy(host, head.data(), head.size());
-    if (len && (st = copy_pageable(host + head.size(), d_out.p, (size_t)len, false))) { swc_free(host); return st; }
-    tail(host + head.size() + len, (uint32_t)check);
-    *out = host; *out_len = total;
-    return SWC_OK;
+    // (9 n + 17) / 8: the largest stream Deflate.compress writes for n bytes
+    return compress_one(deflatec::Args{}, batch_impl, (9 * (u64)in_len + 17) / 8, in, in_len, out, out_len, head, kind, tail_len,
+                        tail);
 }
-
-inline void put_le32(uint8_t *p, uint32_t v) { for (int k = 0; k < 4; k++) p[k] = (uint8_t)(v >> (8 * k)); }
 
 }  // namespace
 
@@ -138,12 +66,10 @@ int32_t swc_deflate_compress_batch(const uint8_t *in_base, const uint64_t *in_of
     if (!in_base || !in_off || !in_len || !out_base || !out_off || !out_cap || !out_len || !status) return SWC_ERR_INVALID_ARG;
     const cudaStream_t s = (cudaStream_t)cuda_stream;
     // the scratch layout is planned on the host from the unit sizes (n x 8 bytes)
-    std::vector<uint64_t> lens(n);
-    SWC_CUDA_TRY(cudaMemcpyAsync(lens.data(), in_len, n * 8, cudaMemcpyDeviceToHost, s));
-    SWC_CUDA_TRY(cudaStreamSynchronize(s));
-    deflatec::Args a;
-    a.in_base = in_base; a.in_off = in_off; a.in_len = in_len;
-    a.out_base = out_base; a.out_off = out_off; a.out_cap = out_cap; a.out_len = out_len; a.status = status; a.n = n;
+    std::vector<u64> lens;
+    int st = read_lens(in_len, n, s, lens);
+    if (st) return st;
+    const deflatec::Args a{{in_base, in_off, in_len, out_base, out_off, out_cap, out_len, status, n}};
     return batch_impl(a, lens, scratch, scratch_bytes, s);
 }
 

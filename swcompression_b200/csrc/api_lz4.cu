@@ -8,10 +8,9 @@
 #include <cstring>
 #include <vector>
 #include "../../include/swcgpu.h"
-#include "host_util.h"
+#include "compress_host.h"
 #include "lz4.cuh"
 #include "lz4_compress.cuh"
-#include "checks.cuh"
 
 using namespace swc;
 
@@ -270,13 +269,13 @@ int32_t swc_lz4_block_decompress_batch(const uint8_t *in_base, const uint64_t *i
     a.out_base = out_base; a.out_off = out_off; a.out_cap = out_cap; a.out_len = out_len; a.status = status; a.n = n;
     // two-phase path needs a record scratch sized from the compressed lengths: fetch them once (n x 8 bytes)
     {
-        std::vector<uint64_t> lens(n);
-        SWC_CUDA_TRY(cudaMemcpyAsync(lens.data(), in_len, n * 8, cudaMemcpyDeviceToHost, (cudaStream_t)cuda_stream));
-        SWC_CUDA_TRY(cudaStreamSynchronize((cudaStream_t)cuda_stream));
+        std::vector<u64> lens;
+        int st = read_lens(in_len, n, (cudaStream_t)cuda_stream, lens);
+        if (st) return st;
         uint64_t total = 0;
         for (uint64_t i = 0; i < n; i++) total += lens[i] & ~(1ull << 63);
         void *scratch = nullptr;
-        int st = scratch_get(lz4::two_phase_scratch_bytes(n, total), &scratch, (cudaStream_t)cuda_stream);
+        st = scratch_get(lz4::two_phase_scratch_bytes(n, total), &scratch, (cudaStream_t)cuda_stream);
         if (st) return st;
         a.scratch = scratch;
     }
@@ -403,8 +402,6 @@ int32_t swc_lz4_multi_decompress(const uint8_t *in, size_t in_len, const uint8_t
 
 namespace {
 
-constexpr u64 kCompressPoolLimit = 16ull << 30;      // library-pool scratch per slice of a compress batch
-
 inline u64 window_of(u64 in_len, u64 dict_len) {
     if (in_len > lz4c::MAX_BLOCK || (dict_len >= 1 && dict_len <= 3)) return 0;       // rejected units need no scratch
     return in_len + (dict_len > lz4c::MAX_DICT ? lz4c::MAX_DICT : dict_len);
@@ -414,8 +411,6 @@ inline u64 need_of(u64 in_len, u64 dict_len) {
     return lz4c::unit_scratch(w, w ? in_len : 0);
 }
 inline u64 meta_bytes(u64 count) { return (count * 8 + 255) & ~(u64)255; }
-
-inline void put32(uint8_t *p, uint32_t v) { p[0] = (uint8_t)v; p[1] = (uint8_t)(v >> 8); p[2] = (uint8_t)(v >> 16); p[3] = (uint8_t)(v >> 24); }
 
 }  // namespace
 
@@ -438,49 +433,20 @@ int32_t swc_lz4_block_compress_batch(const uint8_t *in_base, const uint64_t *in_
     if ((dict_off == nullptr) != (dict_len == nullptr)) return SWC_ERR_INVALID_ARG;
     const cudaStream_t s = (cudaStream_t)cuda_stream;
     // the scratch layout is planned on the host from the unit sizes (n x 16 bytes)
-    std::vector<uint64_t> lens(n), dlens(n, 0), offs(n);
-    SWC_CUDA_TRY(cudaMemcpyAsync(lens.data(), in_len, n * 8, cudaMemcpyDeviceToHost, s));
-    if (dict_len) SWC_CUDA_TRY(cudaMemcpyAsync(dlens.data(), dict_len, n * 8, cudaMemcpyDeviceToHost, s));
-    SWC_CUDA_TRY(cudaStreamSynchronize(s));
-    u64 total = meta_bytes(n), biggest = 0;
-    for (uint64_t i = 0; i < n; i++) {
-        const u64 need = need_of(lens[i], dlens[i]);
-        total += need;
-        if (need > biggest) biggest = need;
-    }
-    size_t cap = scratch_bytes;
-    if (!scratch) {
-        cap = (size_t)(total < kCompressPoolLimit ? total : kCompressPoolLimit);
-        if (cap < meta_bytes(1) + biggest) cap = (size_t)(meta_bytes(1) + biggest);
-        int st = scratch_get(cap, &scratch, s);
-        if (st) return st;
-    }
-    lz4c::Args a;
-    a.in_base = in_base; a.in_off = in_off; a.in_len = in_len; a.dict_off = dict_off; a.dict_len = dict_len;
-    a.out_base = out_base; a.out_off = out_off; a.out_cap = out_cap; a.out_len = out_len; a.status = status;
-    a.stored = nullptr; a.n = n;
-    u8 *scr = (u8 *)scratch;
-    // units go in slices whose scratch fits: a slice's table of offsets first, then each unit's region
-    for (uint64_t first = 0; first < n;) {
-        uint64_t count = 0;
-        u64 used = 0;
-        while (first + count < n) {
-            const u64 need = need_of(lens[first + count], dlens[first + count]);
-            if (meta_bytes(count + 1) + used + need > cap) break;
-            offs[first + count] = used;
-            used += need;
-            count++;
-        }
-        if (count == 0) return SWC_ERR_INVALID_ARG;                       // caller scratch smaller than one unit needs
-        const u64 mb = meta_bytes(count);
-        for (uint64_t j = 0; j < count; j++) offs[first + j] += mb;
+    std::vector<u64> lens, dlens(n, 0), offs(n);
+    int st = read_lens(in_len, n, s, lens);
+    if (!st && dict_len) st = read_lens(dict_len, n, s, dlens);
+    if (st) return st;
+    const lz4c::Args a{{in_base, in_off, in_len, out_base, out_off, out_cap, out_len, status, n}, dict_off, dict_len, nullptr};
+    auto need = [&](u64 i) { return need_of(lens[i], dlens[i]); };
+    return run_in_slices(n, need, meta_bytes, scratch, scratch_bytes, s, [&](u64 first, u64 count, u8 *scr, size_t) -> int {
+        // the slice's table of offsets first, then each unit's region
+        u64 at = meta_bytes(count);
+        for (u64 j = 0; j < count; j++) { offs[first + j] = at; at += need(first + j); }
         SWC_CUDA_TRY(cudaMemcpyAsync(scr, offs.data() + first, count * 8, cudaMemcpyHostToDevice, s));
         int st = lz4c::parse(a, first, count, scr, (const u64 *)scr, s);
-        if (!st) st = lz4c::emit(a, first, count, scr, (const u64 *)scr, s);
-        if (st) return st;
-        first += count;
-    }
-    return SWC_OK;
+        return st ? st : lz4c::emit(a, first, count, scr, (const u64 *)scr, s);
+    });
 }
 
 // LZ4.compress(data:independentBlocks:blockChecksums:contentChecksum:contentSize:blockSize:dictionary:dictionaryID:)
@@ -591,11 +557,11 @@ int32_t swc_lz4_compress(const uint8_t *in, size_t in_len, int32_t independent_b
     }
     memcpy(host, hdr, h);
     for (u64 k = 0; k < nb; k++) {                                                                       // :113-139
-        put32(host + pay_off[k] - 4, (stored[k] ? 0x80000000u : 0u) | (uint32_t)pay_len[k]);
-        if (block_checksums) put32(host + pay_off[k] + pay_len[k], cks[k]);
+        put_le32(host + pay_off[k] - 4, (stored[k] ? 0x80000000u : 0u) | (uint32_t)pay_len[k]);
+        if (block_checksums) put_le32(host + pay_off[k] + pay_len[k], cks[k]);
     }
-    put32(host + payload_end, 0);
-    if (content_checksum) put32(host + payload_end + 4, content_ck);
+    put_le32(host + payload_end, 0);
+    if (content_checksum) put_le32(host + payload_end + 4, content_ck);
     *out = host; *out_len = frame_len;
     return SWC_OK;
 }

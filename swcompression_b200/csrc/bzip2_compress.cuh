@@ -9,14 +9,7 @@ constexpr u32 RAW_PER_LEVEL = 80000;     // BZip2+Compress.swift:47: a raw block
 constexpr u32 MAX_SYMBOLS = 258;         // RUNA, RUNB, 255 MTF indices and EOB
 constexpr u32 MAX_LEN = 11;              // every code length of a 50-symbol group (DESIGN §4.11, lemma 4)
 
-struct Args {
-    const u8 *in_base;
-    const u64 *in_off, *in_len;
-    u8 *out_base;
-    const u64 *out_off, *out_cap;
-    u64 *out_len;                        // the exact size of the .bz2 stream, also for a unit that overflows
-    int32_t *status;
-    u64 n;
+struct Args : UnitIO {                  // out_len: the exact size of the .bz2 stream, also for a unit that overflows
     u32 level;                           // BlockSize.rawValue, 1...9
 };
 

@@ -20,6 +20,18 @@ namespace swc {
 
 __device__ __forceinline__ u32 lane_id() { return threadIdx.x & 31; }
 
+// the unit table of a batched compressor: unit i reads in_base[in_off[i], in_off[i] + in_len[i]) and writes
+// out_base[out_off[i], out_off[i] + out_cap[i]); out_len[i] and status[i] are its results.  Each codec's Args extends it.
+struct UnitIO {
+    const u8 *in_base;
+    const u64 *in_off, *in_len;
+    u8 *out_base;
+    const u64 *out_off, *out_cap;
+    u64 *out_len;
+    int32_t *status;
+    u64 n;
+};
+
 // launch bookkeeping (swc_kernel_launches)
 void count_launch(int n = 1);
 // record a CUDA failure; returns SWC_ERR_CUDA

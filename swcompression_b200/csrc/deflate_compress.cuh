@@ -11,15 +11,7 @@ constexpr u32 REACH = 32768;             // Deflate+Compress.swift:166 (`distanc
 constexpr u32 TILE = 64u << 10;          // positions per link-builder tile; each tile reads REACH bytes of halo in front
 constexpr u32 CHUNK = 4096;              // input bytes per emit checkpoint (> 258, so every chunk but the last starts a symbol)
 
-struct Args {
-    const u8 *in_base;
-    const u64 *in_off, *in_len;
-    u8 *out_base;
-    const u64 *out_off, *out_cap;
-    u64 *out_len;                        // parse: the exact size of the Deflate stream
-    int32_t *status;
-    u64 n;
-};
+struct Args : UnitIO {};                // out_len: the exact size of the Deflate stream
 
 // one slice of units [first, first + count): per-unit scratch offsets, and prefix sums of link tiles and emit chunks
 // (count + 1 entries each), all in device memory

@@ -73,6 +73,14 @@ struct DevBuf {
 
 inline size_t round16(size_t v) { return (v + 15) & ~(size_t)15; }
 
+// a batch's n u64 lengths (device) into `v` on the host, for planning the batch (blocking: waits for `s`)
+inline int read_lens(const u64 *d, u64 n, cudaStream_t s, std::vector<u64> &v) {
+    v.resize(n);
+    SWC_CUDA_TRY(cudaMemcpyAsync(v.data(), d, n * 8, cudaMemcpyDeviceToHost, s));
+    SWC_CUDA_TRY(cudaStreamSynchronize(s));
+    return SWC_OK;
+}
+
 // ---- unit tables: the per-unit metadata of one batch, as typed columns in one device allocation ----
 // Declare every column first, then seat the table with alloc() (its own cudaMalloc) or place() (memory the caller owns);
 // host() pointers stay valid from the last declaration on.  in<T>() columns have a zero-filled host side that upload()
@@ -211,6 +219,7 @@ int copy_back_regions(uint8_t *out_base, const u8 *d_out, const uint64_t *out_of
 
 // ---- container framing (a few bytes per header / block mark) read on the host ----
 inline uint32_t le32(const uint8_t *p) { return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24; }
+inline void put_le32(uint8_t *p, uint32_t v) { for (int k = 0; k < 4; k++) p[k] = (uint8_t)(v >> (8 * k)); }
 // bitwise CRC-32 of header / index / footer fields; payload CRCs run on the device
 inline uint32_t crc32_framing(const uint8_t *p, size_t n) {
     uint32_t c = 0xFFFFFFFFu;

@@ -8,16 +8,9 @@ namespace lz4c {
 constexpr u64 MAX_BLOCK = 4u << 20;      // the largest block a frame holds (LZ4+Compress.swift:51); longer units are unsupported
 constexpr u64 MAX_DICT = 64u << 10;      // longer dictionary windows behave exactly as their last 64 KiB (see DESIGN §4.9)
 
-struct Args {
-    const u8 *in_base;
-    const u64 *in_off, *in_len;          // the block of unit i
-    const u64 *dict_off, *dict_len;      // its dictionary window inside in_base (both null: no dictionary)
-    u8 *out_base;
-    const u64 *out_off, *out_cap;
-    u64 *out_len;                        // parse: exact compressed size of the raw block
-    int32_t *status;
+struct Args : UnitIO {                  // out_len: parse: exact compressed size of the raw block
+    const u64 *dict_off, *dict_len;      // unit i's dictionary window inside in_base (both null: no dictionary)
     const u8 *stored;                    // emit only, may be null: 1 = copy the block uncompressed (frame stored blocks)
-    u64 n;
 };
 
 // scratch of one unit with a window of `w` bytes (dictionary + block) and a block of `l` bytes

@@ -195,11 +195,12 @@ def pack_hostile(units, rng, heads=None, tails=None, residues=None):
     return np.frombuffer(bytes(buf), dtype=np.uint8).copy(), offs, lens
 
 
-def fenced_layout(sizes, spare=4096):
+def fenced_layout(sizes, spare=4096, align=16):
     """Output regions for units that decode to `sizes` bytes (None: unknown, e.g. a damaged unit, which gets `spare` bytes).
     Caps cycle through the exact size, 1..15 bytes short of it (overflow) and 1..15 bytes beyond it; regions start on
-    16-byte multiples, GUARD bytes in front of the first one, at least one byte between two regions and GUARD bytes behind
-    the last one.  -> (out_off u64, out_cap u64, total buffer bytes)"""
+    multiples of `align` (a power of two up to 16) and cycle through every such residue mod 16, GUARD bytes in front of
+    the first one, at least one byte between two regions and GUARD bytes behind the last one.
+    -> (out_off u64, out_cap u64, total buffer bytes)"""
     n = len(sizes)
     offs = np.zeros(n, dtype=np.uint64)
     caps = np.zeros(n, dtype=np.uint64)
@@ -211,7 +212,7 @@ def fenced_layout(sizes, spare=4096):
         else:
             cap = s if i % 3 == 0 else max(s - d, 0) if i % 3 == 1 else s + d
         offs[i], caps[i] = pos, cap
-        pos = (pos + cap + 1 + 15) // 16 * 16 + (16 if i % 2 else 0)
+        pos = (pos + cap + 1 + 15) // 16 * 16 + (16 if i % 2 else 0) + (i + 1) % (16 // align) * align
     return offs, caps, pos + GUARD
 
 

@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 import bzip2c_cases as K
+import compress_batch as CB
 import helpers as H
 
 pytestmark = pytest.mark.gpu
@@ -71,87 +72,29 @@ def test_default_block_size_and_invalid(gpu):
         assert L.swc_bzip2_compress_batch(None, None, None, bad, None, None, None, None, None, 1, None, 0, None) == 4
 
 
-def run_batch(units, in_offs, in_buf, out_off, out_cap, out_total, k, scratch=None, fill=0xA5):
-    import torch
-    from swcompression_b200 import _lib
-    dev = torch.device("cuda:0")
-    t = lambda a: torch.from_numpy(np.asarray(a, dtype=np.uint64).view(np.int64)).to(dev)
-    n = len(units)
-    d_in = torch.from_numpy(in_buf).to(dev)
-    d_out = torch.full((out_total,), fill, dtype=torch.uint8, device=dev)
-    lens = np.array([len(u) for u in units], dtype=np.uint64)
-    d_len, d_st = torch.zeros(n, dtype=torch.int64, device=dev), torch.full((n,), -1, dtype=torch.int32, device=dev)
-    L = _lib.lib()
-    nb = L.swc_bzip2_compress_batch_scratch_bytes(n, int(lens.sum()), k) if scratch is None else scratch
-    scr = torch.empty(nb, dtype=torch.uint8, device=dev)
-    keep = [t(in_offs), t(lens), t(out_off), t(out_cap)]
-    p = lambda x: C.c_void_p(x.data_ptr())
-    st = L.swc_bzip2_compress_batch(p(d_in), p(keep[0]), p(keep[1]), k, p(d_out), p(keep[2]), p(keep[3]), p(d_len), p(d_st),
-                                    n, p(scr), scr.numel(), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-    assert st == 0
-    torch.cuda.synchronize()
-    return d_st.cpu().numpy(), d_len.cpu().numpy(), d_out.cpu().numpy()
+# ---- the batch layout and slice contract it shares with LZ4 and Deflate (compress_batch.py) ----------------------------
+
+def test_batch_fenced(gpu):
+    CB.one_slice("bzip2_compress", 1)
 
 
-def fenced(oc, scratch=None, k=1):
-    """unaligned back-to-back inputs; output regions at any alignment with capacities exact, 1-15 short and 1-15 long"""
-    rng = random.Random(17)
-    text = H.textlike(200000, 21)
-    units = [b"", b"a", b"abcabcabcabc", text[:1000], bytes(5000), text[3:90000], bytes(range(200, 256))]
-    units += [bytes(rng.getrandbits(8) for _ in range(rng.randint(0, 3000))) for _ in range(8)]
-    units += [text[rng.randint(0, 10000):][:rng.randint(1, 9000)] for _ in range(30)]
-    expected = [oc.bzip2_compress(u, k)[1] for u in units]
-    in_buf, in_offs, _ = H.pack_hostile(units, rng)
-    out_off, out_cap, pos = [], [], 7
-    for j, e in enumerate(expected):
-        d = j % 31 - 15
-        cap = max(len(e) + d, 0)
-        out_off.append(pos); out_cap.append(cap)
-        pos += cap + 1 + j % 5
-    st, ln, out = run_batch(units, in_offs, in_buf, out_off, out_cap, pos + 64, k, scratch)
-    touched = np.zeros(len(out), dtype=bool)
-    for j, e in enumerate(expected):
-        assert ln[j] == len(e), j
-        if out_cap[j] < len(e):
-            assert st[j] == 1                                            # SWC_ERR_OUTPUT_OVERFLOW, nothing written
-        else:
-            assert st[j] == 0 and bytes(out[out_off[j]:out_off[j] + len(e)]) == e, j
-            touched[out_off[j]:out_off[j] + len(e)] = True
-    assert (out[~touched] == 0xA5).all()
-    return st, ln, out
+def test_batch_fenced_in_slices(gpu):
+    """the two-block unit (about 3.5 MiB of scratch) fits a slice alone, the batch does not"""
+    CB.in_slices("bzip2_compress", 1)
 
 
-def test_batch_fenced(gpu, oc):
-    fenced(oc)
+def test_scratch_bytes_run_one_slice(gpu):
+    CB.tiny_units_one_slice("bzip2_compress", 1)
 
 
-def test_batch_fenced_in_slices(gpu, oc):
-    """a 6 MiB caller scratch holds the largest unit (two blocks, about 3.5 MiB) but not the batch, which then runs in
-    slices: the results must not change"""
-    from swcompression_b200 import _lib
-    assert _lib.lib().swc_bzip2_compress_batch_scratch_bytes(45, 300000, 1) > 6 << 20
-    a = fenced(oc)
-    b = fenced(oc, scratch=6 << 20)
-    for x, y in zip(a, b):
-        assert (x == y).all()
+@pytest.mark.parametrize("k", [1, 5])
+def test_scratch_below_largest_unit_is_invalid(gpu, k):
+    CB.below_largest_unit_is_invalid("bzip2_compress", k)
 
 
-def test_scratch_bytes_run_one_slice(gpu, oc):
-    """swc_bzip2_compress_batch_scratch_bytes is enough for one slice, also for batches of tiny units: one slice is
-    9 kernel launches"""
-    from swcompression_b200 import _lib
-    L = _lib.lib()
-    rng = random.Random(23)
-    for units in ([bytes(rng.getrandbits(8) for _ in range(rng.randint(0, 84))) for _ in range(300)],
-                  [b"x"] * 50 + [H.textlike(80001, 3)] + [bytes(200)] * 50):
-        expected = [oc.bzip2_compress(u, 1)[1] for u in units]
-        in_buf, in_offs, _ = H.pack_hostile(units, rng)
-        out_off = np.cumsum([0] + [len(e) + 3 for e in expected[:-1]]) + 5
-        before = L.swc_kernel_launches()
-        st, ln, out = run_batch(units, in_offs, in_buf, out_off, [len(e) for e in expected], int(out_off[-1]) + len(expected[-1]) + 64, 1)
-        assert L.swc_kernel_launches() - before == 9
-        for j, e in enumerate(expected):
-            assert st[j] == 0 and bytes(out[out_off[j]:out_off[j] + len(e)]) == e, j
+def test_batch_contract_at_block_size_5(gpu):
+    CB.in_slices("bzip2_compress", 5)
+    CB.tiny_units_one_slice("bzip2_compress", 5)
 
 
 def test_benched_shape_tiled(gpu, oc):

@@ -8,6 +8,7 @@ import struct
 import numpy as np
 import pytest
 
+import compress_batch as CB
 import deflatec_cases as K
 import helpers as H
 
@@ -96,72 +97,22 @@ def test_gzip_errors(gpu):
     assert S.GzipArchive.unarchive(ok) == b"x"
 
 
-def run_batch(units, in_offs, in_buf, out_off, out_cap, out_total, scratch=None, fill=0xA5):
-    import torch
-    from swcompression_b200 import _lib
-    dev = torch.device("cuda:0")
-    t = lambda a: torch.from_numpy(np.asarray(a, dtype=np.uint64).view(np.int64)).to(dev)
-    n = len(units)
-    d_in = torch.from_numpy(in_buf).to(dev)
-    d_out = torch.full((out_total,), fill, dtype=torch.uint8, device=dev)
-    lens = np.array([len(u) for u in units], dtype=np.uint64)
-    d_len, d_st = torch.zeros(n, dtype=torch.int64, device=dev), torch.full((n,), -1, dtype=torch.int32, device=dev)
-    L = _lib.lib()
-    nb = L.swc_deflate_compress_batch_scratch_bytes(n, int(lens.sum())) if scratch is None else scratch
-    scr = torch.empty(nb, dtype=torch.uint8, device=dev)
-    keep = [t(in_offs), t(lens), t(out_off), t(out_cap)]
-    p = lambda x: C.c_void_p(x.data_ptr())
-    st = L.swc_deflate_compress_batch(p(d_in), p(keep[0]), p(keep[1]), p(d_out), p(keep[2]), p(keep[3]), p(d_len), p(d_st),
-                                      n, p(scr), scr.numel(), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-    assert st == 0
-    torch.cuda.synchronize()
-    return d_st.cpu().numpy(), d_len.cpu().numpy(), d_out.cpu().numpy()
+# ---- the batch layout and slice contract it shares with LZ4 and BZip2 (compress_batch.py) ------------------------------
+
+def test_batch_fenced(gpu):
+    CB.one_slice("deflate_compress")
 
 
-def fenced(oc, scratch=None):
-    rng = random.Random(17)
-    text = H.textlike(200000, 21)
-    units = [b"", b"a", b"abcabcabcabc", text[:1000], bytes(5000), text[3:70000], text[:K.TILE + 1], bytes(range(200, 256))]
-    units += [bytes(rng.getrandbits(8) for _ in range(rng.randint(0, 3000))) for _ in range(10)]
-    units += [text[rng.randint(0, 10000):][:rng.randint(1, 9000)] for _ in range(40)]
-    expected = [oc.deflate_compress(u)[1] for u in units]
-    in_offs, pos = [], 3
-    for u in units:
-        in_offs.append(pos)
-        pos += len(u)
-    in_buf = np.zeros(pos + 64, dtype=np.uint8)
-    for u, o in zip(units, in_offs):
-        in_buf[o:o + len(u)] = np.frombuffer(u, dtype=np.uint8)
-    # capacities at every residue: exact, 1-15 short, 1-15 long; regions 16-aligned with 0xA5 gaps between them
-    out_off, out_cap, pos = [], [], 16
-    for k, e in enumerate(expected):
-        d = k % 31 - 15
-        cap = max(len(e) + d, 0)
-        out_off.append(pos); out_cap.append(cap)
-        pos += (cap + 15) // 16 * 16 + 16
-    st, ln, out = run_batch(units, in_offs, in_buf, out_off, out_cap, pos + 64, scratch)
-    touched = np.zeros(len(out), dtype=bool)
-    for k, e in enumerate(expected):
-        assert ln[k] == len(e), k
-        if out_cap[k] < len(e):
-            assert st[k] == 1                                            # SWC_ERR_OUTPUT_OVERFLOW, nothing written
-        else:
-            assert st[k] == 0 and bytes(out[out_off[k]:out_off[k] + len(e)]) == e, k
-            touched[out_off[k]:out_off[k] + len(e)] = True
-    assert (out[~touched] == 0xA5).all()
-    return st, ln, out
+def test_batch_fenced_in_slices(gpu):
+    CB.in_slices("deflate_compress")
 
 
-def test_batch_fenced(gpu, oc):
-    fenced(oc)
+def test_scratch_bytes_run_one_slice(gpu):
+    CB.tiny_units_one_slice("deflate_compress")
 
 
-def test_batch_fenced_in_slices(gpu, oc):
-    """a caller scratch that holds only a few units forces slices: the results must not change"""
-    a = fenced(oc)
-    b = fenced(oc, scratch=2 << 20)
-    for x, y in zip(a, b):
-        assert (x == y).all()
+def test_scratch_below_largest_unit_is_invalid(gpu):
+    CB.below_largest_unit_is_invalid("deflate_compress")
 
 
 def test_benched_shape_and_bgzf_round_trip(gpu, oc):

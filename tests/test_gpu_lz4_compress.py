@@ -1,11 +1,11 @@
 """The CUDA LZ4 compressor (lz4_compress.cu through swc_lz4_compress / swc_lz4_block_compress_batch) byte for byte
 against the CPU restatement of LZ4+Compress.swift, and back through the GPU decoder."""
-import ctypes as C
 import random
 
 import numpy as np
 import pytest
 
+import compress_batch as CB
 import helpers as H
 import lz4c_cases as K
 
@@ -110,61 +110,22 @@ def test_option_sweep(gpu, oc, bs):
                                     contentSize=cs, blockSize=bs)
 
 
-# ---- the batched raw form --------------------------------------------------------------------------------------------
+# ---- the batched raw form: the layout and slice contract it shares with Deflate and BZip2 (compress_batch.py) ----------
 
-def run_batch(units, in_offs, in_buf, out_off, out_cap, out_total, dict_off=None, dict_len=None, fill=0xA5):
-    import torch
-    from swcompression_b200 import _lib
-    dev = torch.device("cuda:0")
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(np.asarray(a, dtype=np.uint64)).view(np.int64)).to(dev)
-    n = len(units)
-    d_in = torch.from_numpy(in_buf).to(dev)
-    d_out = torch.full((out_total,), fill, dtype=torch.uint8, device=dev)
-    lens = np.array([len(u) for u in units], dtype=np.uint64)
-    d_len, d_st = torch.zeros(n, dtype=torch.int64, device=dev), torch.full((n,), -1, dtype=torch.int32, device=dev)
-    window = int(lens.sum()) + (0 if dict_len is None else int(np.minimum(np.asarray(dict_len, dtype=np.uint64), 65536).sum()))
-    L = _lib.lib()
-    scr = torch.empty(L.swc_lz4_compress_batch_scratch_bytes(n, window), dtype=torch.uint8, device=dev)
-    keep = [t(in_offs), t(lens), t(out_off), t(out_cap)] + ([t(dict_off), t(dict_len)] if dict_off is not None else [None, None])
-    p = lambda x: None if x is None else C.c_void_p(x.data_ptr())
-    st = L.swc_lz4_block_compress_batch(p(d_in), p(keep[0]), p(keep[1]), p(keep[4]), p(keep[5]), p(d_out), p(keep[2]),
-                                        p(keep[3]), p(d_len), p(d_st), n, p(scr), scr.numel(),
-                                        C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-    assert st == 0
-    torch.cuda.synchronize()
-    return d_st.cpu().numpy(), d_len.cpu().numpy(), d_out.cpu().numpy()
+def test_batch_unaligned_fenced(gpu):
+    CB.one_slice("lz4_block_compress")
 
 
-def test_batch_unaligned_fenced(gpu, oc):
-    rng = random.Random(17)
-    text = dict(K.frame_inputs())["text"]
-    units = [b"", b"a", b"abcdabcdabcdabcd", text[:1000], bytes(5000), text[3:70000]]
-    units += [bytes(rng.getrandbits(8) for _ in range(rng.randint(0, 3000))) for _ in range(10)]
-    units += [text[rng.randint(0, 10000):][:rng.randint(1, 9000)] for _ in range(30)]
-    expected = [oc.lz4_block_compress(u)[1] for u in units]
-    # inputs back to back at odd offsets; outputs at every capacity residue with 0xA5 gaps between them
-    in_offs, pos = [], 3
-    for u in units:
-        in_offs.append(pos)
-        pos += len(u)
-    in_buf = np.zeros(pos + 64, dtype=np.uint8)
-    for u, o in zip(units, in_offs):
-        in_buf[o:o + len(u)] = np.frombuffer(u, dtype=np.uint8)
-    out_off, out_cap, pos = [], [], 5
-    for k, e in enumerate(expected):
-        cap = len(e) + k % 17 if k % 5 else max(len(e) - 1, 0)       # every fifth unit is one byte short
-        out_off.append(pos); out_cap.append(cap)
-        pos += cap + 7
-    st, ln, out = run_batch(units, in_offs, in_buf, out_off, out_cap, pos + 64)
-    touched = np.zeros(len(out), dtype=bool)
-    for k, e in enumerate(expected):
-        assert ln[k] == len(e), k
-        if k % 5 == 0 and len(e) > 0:
-            assert st[k] == 1                                            # SWC_ERR_OUTPUT_OVERFLOW, required size in out_len
-        else:
-            assert st[k] == 0 and bytes(out[out_off[k]:out_off[k] + len(e)]) == e, k
-        touched[out_off[k]:out_off[k] + out_cap[k]] = True
-    assert (out[~touched] == 0xA5).all()
+def test_batch_fenced_in_slices(gpu):
+    CB.in_slices("lz4_block_compress")
+
+
+def test_scratch_bytes_run_one_slice(gpu):
+    CB.tiny_units_one_slice("lz4_block_compress")
+
+
+def test_scratch_below_largest_unit_is_invalid(gpu):
+    CB.below_largest_unit_is_invalid("lz4_block_compress")
 
 
 def test_batch_dictionary_windows(gpu, oc):
@@ -184,15 +145,18 @@ def test_batch_dictionary_windows(gpu, oc):
             d_off.append(len(small) + o - w); d_len.append(w); dicts.append(text[o - w:o])
     units.append(text[:3000]); in_offs.append(len(small)); d_off.append(0); d_len.append(len(buf)); dicts.append(buf)
     units.append(text[:100]); in_offs.append(len(small)); d_off.append(0); d_len.append(2); dicts.append(buf[:2])
+    from swcompression_b200.batch import Batch
     in_buf = np.frombuffer(buf + bytes(64), dtype=np.uint8).copy()
-    caps = [len(u) + len(u) // 200 + 64 for u in units]
-    offs = list(np.cumsum([0] + caps[:-1]))
-    st, ln, out = run_batch(units, in_offs, in_buf, offs, caps, sum(caps) + 64, d_off, d_len)
+    b = Batch("lz4_block_compress", in_buf, in_offs, [len(u) for u in units], [len(u) + len(u) // 200 + 64 for u in units],
+              aux=(d_off, d_len))
+    b.run()
+    st, ln, _ = b.results()
+    outs = b.outputs()
     for k, (u, d) in enumerate(zip(units, dicts)):
         ost, exp, _ = oc.lz4_block_compress(u, d)
         assert st[k] == ost, k
         if ost == 0:
-            assert ln[k] == len(exp) and bytes(out[offs[k]:offs[k] + ln[k]]) == exp, k
+            assert ln[k] == len(exp) and outs[k] == exp, k
     assert st[-1] == 2
 
 

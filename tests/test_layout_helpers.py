@@ -85,6 +85,15 @@ def test_fenced_layout_caps_and_guards():
     assert (offs[1:] > ends[:-1]).all() and total - int(ends[-1]) >= H.GUARD
 
 
+@pytest.mark.parametrize("align", [1, 4, 16])
+def test_fenced_layout_alignment(align):
+    sizes = [1000 + 37 * i for i in range(96)]
+    offs, caps, total = H.fenced_layout(sizes, align=align)
+    assert set((offs % 16).tolist()) == set(range(0, 16, align))
+    ends = offs + caps
+    assert (offs[1:] > ends[:-1]).all() and total - int(ends[-1]) >= H.GUARD
+
+
 def test_fence_violations_finds_a_stray_byte():
     offs, caps, total = H.fenced_layout([100, 200, 300])
     out = np.full(total, H.SENTINEL, dtype=np.uint8)
