@@ -24,25 +24,29 @@ namespace inflate {
 // One warp per unit, the only writer of the unit's output, which it builds in order in a per-warp ring of RING bytes of
 // shared memory (output byte p lives at ring[(p + phase) % RING], phase = the output's address mod 16, so that aligned
 // 16-byte chunks of the output are aligned 16-byte chunks of the ring).  A batch is a run of consecutive records whose
-// output ends at most SPAN bytes past the batch start; lane j holds record j, loaded one batch ahead.  Per batch:
-//   scan     : inclusive warp scans of (literal run + length) and of the literal run give every record its position and
-//              the offset of its literals in the batch's part of the literal stream;
+// output ends at most SPAN bytes past the batch start, at most BATCH = 64 of them; lane j holds records 2j and 2j + 1,
+// loaded one batch ahead.  Per batch:
+//   scan     : inclusive scans of (literal run + length) and of the literal run — each lane adds its pair, a warp scan
+//              adds the pair sums — give every record its position and the offset of its literals in the batch's part of
+//              the literal stream;
 //   gather   : one round of 16-byte cp.async copies brings in the batch's literals from the packed stream and the sources
-//              of its FAR matches from the output.  A match is far when its first source byte is more than RING bytes behind
-//              the batch end (bend): with len <= 258 and bend - RING <= done - SPAN, its whole source then lies in output this
-//              warp has already flushed, and dist > RING - SPAN >= len.  Every other match reads only bytes that are still
-//              in the ring.  A far source takes at most len/16 + 2 aligned chunks, so a batch (<= 32 records, their lengths
-//              summing to <= SPAN) needs at most 128 of them, which a warp-wide scan packs into a 2 KiB staging buffer;
-//              the part of the output's first chunk that lies before out[0] is never read (that chunk is copied byte by
-//              byte);
-//   literals : every lane places literals: a binary search over the records' literal offsets (shuffles) finds each
-//              one's position;
-//   matches  : replayed 8 at a time by 4-lane sub-groups, reading shared memory only (far ones from the staging buffer,
-//              the others from the ring).  A record is READY when everything it reads is final: its source ends at or
-//              before the start of the oldest still-pending record of the 8 (bytes before that point are literals, older
-//              matches or earlier batches) — or it IS that oldest record.  Far matches therefore run 8-wide in one pass,
-//              chains of near matches (RLE-like data) degrade to in-order execution.  Overlapping copies (dist < len)
-//              replicate the period: every source byte lies in [start-dist, start), never in what the match itself writes;
+//              of its FAR matches from the output, both into one staging buffer (literals first, far sources behind
+//              them).  A match is far when its first source byte is more than RING bytes behind the batch end (bend):
+//              with len <= 258 and bend - RING <= done - SPAN, its whole source then lies in output this warp has already
+//              flushed, and dist > RING - SPAN >= len.  Every other match reads only bytes that are still in the ring.
+//              The nl literals take at most (nl + 30)/16 aligned chunks, a far source of len bytes at most
+//              (len + 30)/16; the batch's literal runs and lengths sum to <= SPAN, so with <= 64 records the buffer needs
+//              at most (SPAN + 30 + 30 * 64)/16, i.e. 185 chunks.  A warp-wide scan packs the far sources; the part
+//              of the output's first chunk that lies before out[0] is never read (that chunk is copied byte by byte);
+//   literals : each lane copies the literal runs of its two records into the ring, eight bytes per trip (a binary
+//              search over the records for every literal, one per lane and round, was slower);
+//   matches  : replayed PASS = 16 at a time by 2-lane sub-groups, reading shared memory only (far ones from the staging
+//              buffer, the others from the ring).  A record is READY when everything it reads is final: its source ends
+//              at or before the start of the oldest still-pending record of the pass (bytes before that point are
+//              literals, older matches or earlier batches) — or it IS that oldest record.  Far matches therefore run
+//              16-wide in one pass, chains of near matches (RLE-like data) degrade to in-order execution.  Overlapping
+//              copies (dist < len) replicate the period: every source byte lies in [start-dist, start), never in what
+//              the match itself writes;
 //   flush    : every whole 16-byte chunk of the output below the batch end goes out with one 16-byte store; the output's
 //              first and last partial chunks are written byte by byte, so no byte outside [0, out_len) is touched.
 // A batch stays within SPAN + 15 bytes of the first unflushed byte, so nothing is overwritten in the ring before it is
@@ -54,14 +58,16 @@ constexpr int WARPS = 8;
 constexpr int CTAS_PER_SM = 4;
 constexpr u32 RING = 2048;
 constexpr u32 SPAN = RING / 2;       // >= 255 + 258: one record of any kind but an escape fits a batch
-constexpr u32 LITBUF = SPAN + 32;    // a batch's literals plus the 16-byte alignment slack at both ends
-constexpr u32 FARBUF = 128 * 16;     // the far sources of a batch: at most 32 * 2 + SPAN / 16 chunks
+constexpr u32 BATCH = 64;            // records per batch at most: two per lane
+constexpr u32 SUBW = 2;              // lanes per replay sub-group (4-lane sub-groups, 8 records per pass: slower)
+constexpr u32 PASS = 32 / SUBW;      // records replayed per pass
+constexpr u32 BPL = 16 / SUBW;       // bytes per lane and trip of a copy
+constexpr u32 STAGEBUF = (SPAN + 30 + 30 * BATCH) / 16 * 16;   // a batch's literals, then its far sources
 constexpr u32 NEAR = 0xFFFFFFFFu;    // staging offset of a match that reads the ring
 struct __align__(16) WarpSmem {
-    uint4 stage[32];                 // {start, length, distance, staging offset of the first source byte | NEAR}
+    uint4 stage[BATCH];              // {start, length, distance, staging offset of the first source byte | NEAR}
     u8 ring[RING];
-    u8 lit[LITBUF];
-    u8 far[FARBUF];
+    u8 buf[STAGEBUF];
 };
 __device__ __forceinline__ void cp_async16(void *dst, const void *src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"((u32)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
@@ -80,7 +86,7 @@ lz_resolve_kernel(BatchArgs a) {
     if (nrec == REC_DIRECT) return;
     WarpSmem &S = smem[(threadIdx.x >> 5) & (WARPS - 1)];
     const u32 lane = threadIdx.x & 31;
-    const u32 sub = lane >> 2, t = lane & 3;
+    const u32 sub = lane / SUBW, t = lane % SUBW;
     const u64 off = a.out_off[unit];
     const u32 len = (u32)a.out_len[unit];
     u8 *out = a.out_base + off;
@@ -107,131 +113,158 @@ lz_resolve_kernel(BatchArgs a) {
         }
         flushed = to;
     };
-    u32 rv = lane < nrec ? __ldg(rec - 1 - lane) : REC_ESC;              // record g + lane
+    // records g + 2 lane (x) and g + 2 lane + 1 (y)
+    auto load = [&](u32 i) -> u32 { return i < nrec ? __ldg(rec - 1 - i) : REC_ESC; };
+    u32 rx = load(2 * lane), ry = load(2 * lane + 1);
     for (;;) {
-        // ---- the batch: records g.. whose output ends within SPAN bytes of `done`
-        const bool real = g + lane < nrec;
-        const Match m = get_match(rv);
-        const u32 adv = m.adv - (lane == 0 ? part : 0u);
-        const u32 run = adv - m.len;
-        u32 end = adv, lend = run;
+        // ---- the batch: records g.. whose output ends within SPAN bytes of `done`, at most BATCH of them
+        const u32 ix = 2 * lane, iy = ix + 1;                    // record indices within the batch
+        const Match mx = get_match(rx), my = get_match(ry);
+        const u32 advx = mx.adv - (lane == 0 ? part : 0u), advy = my.adv;
+        const u32 runx = advx - mx.len, runy = advy - my.len;
+        u32 end = advx + advy, lend = runx + runy;               // inclusive scans over the pairs: record y's values
 #pragma unroll
         for (int d = 1; d < 32; d <<= 1) {
             const u32 v = __shfl_up_sync(SWC_FULL, end, d), w = __shfl_up_sync(SWC_FULL, lend, d);
             if (lane >= (u32)d) { end += v; lend += w; }
         }
-        const u32 k = __popc(__ballot_sync(SWC_FULL, real && end <= SPAN));   // a prefix: `end` does not decrease
+        const u32 endx = end - advy, lendx = lend - runy;        // record x's
+        // a prefix: `end` does not decrease along the records
+        const u32 k = __popc(__ballot_sync(SWC_FULL, g + ix < nrec && endx <= SPAN)) +
+                      __popc(__ballot_sync(SWC_FULL, g + iy < nrec && end <= SPAN));
         u32 span, nl;
-        u32 delta;         // output position of a literal minus its index in the batch's literals (the lane's record)
+        u32 deltax, deltay;  // output position of a literal minus its index in the batch's literals (records x, y)
+        u32 litx, lity, nx, ny;   // first literal (index in the batch's literals) and literal count of records x, y
         if (k > 0) {
-            span = __shfl_sync(SWC_FULL, end, k - 1);
-            nl = __shfl_sync(SWC_FULL, lend, k - 1);
-            delta = done + end - adv - (lend - run);
-            if (lane >= k) lend = 0xFFFFFFFFu;
+            const bool ly = ((k - 1) & 1) != 0;                  // the batch's last record is a y
+            span = __shfl_sync(SWC_FULL, ly ? end : endx, (k - 1) >> 1);
+            nl = __shfl_sync(SWC_FULL, ly ? lend : lendx, (k - 1) >> 1);
+            deltax = done + endx - advx - (lendx - runx);
+            deltay = done + end - advy - (lend - runy);
+            litx = lendx - runx;
+            lity = lendx;
+            nx = ix < k ? runx : 0u;
+            ny = iy < k ? runy : 0u;
             g += k;
             part = 0;
         } else {
             // a literal run longer than SPAN: an escape (g < nrec) or the literals after the last match
-            const u32 adv0 = __shfl_sync(SWC_FULL, adv, 0);      // what is left of escape g
+            const u32 adv0 = __shfl_sync(SWC_FULL, advx, 0);     // what is left of escape g
             const u32 rem = g < nrec ? adv0 : len - done;
             if (rem == 0) break;
             span = nl = rem < SPAN ? rem : SPAN;
             if (g < nrec) part += span;
-            delta = done;
-            lend = lane == 0 ? nl : 0xFFFFFFFFu;
+            deltax = deltay = done;
+            litx = lity = 0;
+            nx = lane == 0 ? nl : 0u;
+            ny = 0;
         }
-        if (k > 0) rv = g + lane < nrec ? __ldg(rec - 1 - (g + lane)) : REC_ESC;   // the next batch's records
+        if (k > 0) {                                             // the next batch's records
+            rx = load(g + ix);
+            ry = load(g + iy);
+        }
         const u32 bend = done + span;                            // batch end
         // ---- gather: the literals (packed stream) and the far match sources (flushed output) -> shared memory
         const uintptr_t lsrc = (uintptr_t)(lits + lit);
         const u8 *lchunk = (const u8 *)(lsrc & ~(uintptr_t)15);
         const u32 lofs = (u32)(lsrc & 15), nch = (lofs + nl + 15) >> 4;
-        for (u32 c = lane; c < nch; c += 32) cp_async16(S.lit + c * 16, lchunk + c * 16);
-        const u32 ms = done + end - m.len, mq = ms - m.dist;      // the lane's match: start, first source byte
-        const bool far = lane < k && m.len != 0 && mq + RING < bend;
-        const u32 c0 = (mq + ph) >> 4;                           // first source chunk (output chunk index)
-        const u32 fch = far ? ((mq + m.len - 1 + ph) >> 4) - c0 + 1 : 0u;
-        u32 fend = fch;                                          // inclusive scan: staging chunks up to this record
+        for (u32 c = lane; c < nch; c += 32) cp_async16(S.buf + c * 16, lchunk + c * 16);
+        const u32 msx = done + endx - mx.len, mqx = msx - mx.dist;      // the lane's matches: start, first source byte
+        const u32 msy = done + end - my.len, mqy = msy - my.dist;
+        const bool farx = ix < k && mx.len != 0 && mqx + RING < bend;
+        const bool fary = iy < k && my.len != 0 && mqy + RING < bend;
+        const u32 c0x = (mqx + ph) >> 4, c0y = (mqy + ph) >> 4;          // first source chunks (output chunk index)
+        const u32 fchx = farx ? ((mqx + mx.len - 1 + ph) >> 4) - c0x + 1 : 0u;
+        const u32 fchy = fary ? ((mqy + my.len - 1 + ph) >> 4) - c0y + 1 : 0u;
+        u32 fend = fchx + fchy;                                  // inclusive scan: staging chunks up to this pair
 #pragma unroll
         for (int d = 1; d < 32; d <<= 1) {
             const u32 v = __shfl_up_sync(SWC_FULL, fend, d);
             if (lane >= (u32)d) fend += v;
         }
-        const u32 fbeg = fend - fch;
+        const u32 fbx = nch + fend - fchx - fchy, fby = fbx + fchx;      // first staging chunks of x and y
         const u8 *outa = out - ph;                               // 16-byte aligned: output chunk c starts at outa + 16 c
-        for (u32 c = 0; c < fch; c++) {
-            u8 *dst = S.far + (fbeg + c) * 16;
-            if (c0 + c > 0 || ph == 0) {
-                cp_async16(dst, outa + (c0 + c) * 16);
+        for (u32 c = 0; c < fchx + fchy; c++) {
+            const u32 oc = c < fchx ? c0x + c : c0y + c - fchx;  // output chunk
+            u8 *dst = S.buf + (fbx + c) * 16;
+            if (oc > 0 || ph == 0) {
+                cp_async16(dst, outa + oc * 16);
             } else {
                 for (u32 b = ph; b < 16; b++) dst[b] = outa[b];  // the output's first chunk starts before out[0]
             }
         }
-        S.stage[lane] = make_uint4(ms, lane < k ? m.len : 0u, m.dist, far ? fbeg * 16 + ((mq + ph) & 15) : NEAR);
+        S.stage[ix] = make_uint4(msx, ix < k ? mx.len : 0u, mx.dist, farx ? fbx * 16 + ((mqx + ph) & 15) : NEAR);
+        S.stage[iy] = make_uint4(msy, iy < k ? my.len : 0u, my.dist, fary ? fby * 16 + ((mqy + ph) & 15) : NEAR);
         cp_async_wait_all();
         __syncwarp();
-        // ---- literals -> their positions in the ring
-        for (u32 j0 = 0; j0 < nl; j0 += 32) {
-            const u32 j = j0 + lane;
-            u32 r = 0;                                           // records whose literals all precede literal j
+        // ---- literals -> their positions in the ring: each lane copies the literal runs of its two records, eight
+        // bytes per trip, all loads before the first store
+        auto place = [&](u32 li, u32 delta, u32 n, u32 i) {
+            if (i >= n) return;
+            const u8 *src = S.buf + lofs + li + i;
+            const u32 b = (li + delta + i + ph) & M;
+            u32 v[8];
 #pragma unroll
-            for (u32 step = 16; step > 0; step >>= 1)
-                if (__shfl_sync(SWC_FULL, lend, r + step - 1) <= j) r += step;
-            const u32 p = j + __shfl_sync(SWC_FULL, delta, r);
-            if (j < nl) S.ring[(p + ph) & M] = S.lit[lofs + j];
+            for (u32 q = 0; q < 8; q++) v[q] = i + q < n ? src[q] : 0u;
+            if (b <= M - 7) {
+#pragma unroll
+                for (u32 q = 0; q < 8; q++)
+                    if (i + q < n) S.ring[b + q] = (u8)v[q];
+            } else {
+#pragma unroll
+                for (u32 q = 0; q < 8; q++)
+                    if (i + q < n) S.ring[(b + q) & M] = (u8)v[q];
+            }
+        };
+        for (u32 i = 0; i < (nx > ny ? nx : ny); i += 8) {
+            place(litx, deltax, nx, i);
+            place(lity, deltay, ny, i);
         }
         lit += nl;
         __syncwarp();
         // ---- matches
 #pragma unroll 1
-        for (u32 b0 = 0; b0 < k; b0 += 8) {
+        for (u32 b0 = 0; b0 < k; b0 += PASS) {
             const uint4 rc = S.stage[b0 + sub];                  // this sub-group's record
             const u32 s = rc.x, l = rc.y, d = rc.z;
             const u32 src_end = s - d + (l < d ? l : d);
             // source byte i of the match: a far one from the staging buffer, a near one from the ring
             const bool fr = rc.w != NEAR;
-            const u8 *sb = fr ? S.far : S.ring;
+            const u8 *sb = fr ? S.buf : S.ring;
             const u32 s0 = fr ? rc.w : s - d + ph, sm = fr ? 0xFFFFFFFFu : M;
-            const u32 alim = fr ? FARBUF : M - 3;               // source index of 4 bytes that do not wrap around
+            const u32 alim = fr ? STAGEBUF : M - (BPL - 1);     // source index of BPL bytes that do not wrap around
             auto src_byte = [&](u32 i) -> u8 { return sb[(s0 + i) & sm]; };
             bool pend = l != 0;
-            u32 pmask = __ballot_sync(SWC_FULL, pend && t == 0); // bit 4*sub per pending record
+            u32 pmask = __ballot_sync(SWC_FULL, pend && t == 0); // bit SUBW*sub per pending record
             while (pmask) {
-                const u32 oldest = (__ffs(pmask) - 1) >> 2;       // sub-group index of the oldest pending record
+                const u32 oldest = (__ffs(pmask) - 1) / SUBW;     // sub-group index of the oldest pending record
                 const u32 frontier = S.stage[b0 + oldest].x;
                 const bool ready = pend && (sub == oldest || src_end <= frontier);
                 if (ready) {
                     if (d >= l) {
-                        // four consecutive bytes per lane and trip, all four loads issued before the first store; one
-                        // source and one ring address per trip unless the four bytes wrap around the ring
-                        for (u32 i = 4 * t; i < l; i += 16) {
-                            const bool p1 = i + 1 < l, p2 = i + 2 < l, p3 = i + 3 < l;
+                        // BPL consecutive bytes per lane and trip, all loads issued before the first store; one source
+                        // and one ring address per trip unless the bytes wrap around the ring
+                        for (u32 i = BPL * t; i < l; i += 16) {
                             const u32 a = (s0 + i) & sm, b = (s + i + ph) & M;
-                            u32 v0, v1 = 0, v2 = 0, v3 = 0;
-                            if (a <= alim && b <= M - 3) {
+                            u32 v[BPL];
+                            if (a <= alim && b <= M - (BPL - 1)) {
                                 const u8 *src = sb + a;
                                 u8 *dst = S.ring + b;
-                                v0 = src[0];
-                                if (p1) v1 = src[1];
-                                if (p2) v2 = src[2];
-                                if (p3) v3 = src[3];
-                                dst[0] = v0;
-                                if (p1) dst[1] = v1;
-                                if (p2) dst[2] = v2;
-                                if (p3) dst[3] = v3;
+#pragma unroll
+                                for (u32 q = 0; q < BPL; q++) v[q] = i + q < l ? src[q] : 0u;
+#pragma unroll
+                                for (u32 q = 0; q < BPL; q++)
+                                    if (i + q < l) dst[q] = (u8)v[q];
                             } else {
-                                v0 = src_byte(i);
-                                if (p1) v1 = src_byte(i + 1);
-                                if (p2) v2 = src_byte(i + 2);
-                                if (p3) v3 = src_byte(i + 3);
-                                S.ring[b] = v0;
-                                if (p1) S.ring[(b + 1) & M] = v1;
-                                if (p2) S.ring[(b + 2) & M] = v2;
-                                if (p3) S.ring[(b + 3) & M] = v3;
+#pragma unroll
+                                for (u32 q = 0; q < BPL; q++) v[q] = i + q < l ? src_byte(i + q) : 0u;
+#pragma unroll
+                                for (u32 q = 0; q < BPL; q++)
+                                    if (i + q < l) S.ring[(b + q) & M] = (u8)v[q];
                             }
                         }
                     } else {
-                        for (u32 i = t; i < l; i += 4) S.ring[(s + i + ph) & M] = src_byte(i % d);
+                        for (u32 i = t; i < l; i += SUBW) S.ring[(s + i + ph) & M] = src_byte(i % d);
                     }
                     pend = false;
                 }
