@@ -10,29 +10,30 @@ using namespace swc;
 
 namespace {
 
-int bzip2_batch_impl(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
-                     uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
-                     uint64_t *out_len, uint64_t *consumed_bits, int32_t *status, uint64_t n, cudaStream_t stream) {
-    if (n == 0) return SWC_OK;
-    if (!in_base || !in_off || !in_len || !out_base || !out_off || !out_cap || !out_len || !consumed_bits || !status)
-        return SWC_ERR_INVALID_ARG;
-    // per-unit scratch sizes depend on the capacities: fetch them (n x 8 bytes), lay the scratch out on the host
-    std::vector<uint64_t> caps(n), soff(n);
-    SWC_CUDA_TRY(cudaMemcpyAsync(caps.data(), out_cap, n * 8, cudaMemcpyDeviceToHost, stream));
-    SWC_CUDA_TRY(cudaStreamSynchronize(stream));
-    size_t total = (n * 8 + 255) & ~(size_t)255;
-    for (uint64_t i = 0; i < n; i++) { soff[i] = total; total += bzip2::scratch_per_unit(caps[i]); }
+// Lays the scratch out for units of output capacity caps[0, a.n) (host): a table of a.n offsets rounded up to 256 bytes,
+// then scratch_per_unit(cap) bytes per unit.  Uploads the table into the front of the scratch and launches.  When the pool
+// cannot supply the scratch, *no_scratch is set and its status returned without a launch.
+int launch_with_scratch(bzip2::Args a, const u64 *caps, cudaStream_t stream, bool *no_scratch = nullptr) {
+    std::vector<u64> soff(a.n);
+    size_t total = (a.n * 8 + 255) & ~(size_t)255;
+    for (u64 i = 0; i < a.n; i++) { soff[i] = total; total += bzip2::scratch_per_unit(caps[i]); }
     void *scratch = nullptr;
     int st = scratch_get(total, &scratch, stream);
+    if (no_scratch) *no_scratch = st != SWC_OK;
     if (st) return st;
-    SWC_CUDA_TRY(cudaMemcpyAsync(scratch, soff.data(), n * 8, cudaMemcpyHostToDevice, stream));
+    SWC_CUDA_TRY(cudaMemcpyAsync(scratch, soff.data(), a.n * 8, cudaMemcpyHostToDevice, stream));
     SWC_CUDA_TRY(cudaStreamSynchronize(stream));     // soff lives on this stack frame
-    bzip2::Args a;
-    a.in_base = in_base; a.in_off = in_off; a.in_len = in_len;
-    a.out_base = out_base; a.out_off = out_off; a.out_cap = out_cap;
-    a.out_len = out_len; a.consumed_bits = consumed_bits; a.status = status; a.n = n;
     a.scratch = (u8 *)scratch; a.scr_off = (const u64 *)scratch;
     return bzip2::launch(a, stream);
+}
+
+// whole streams; the per-unit scratch sizes depend on the capacities: fetch them (n x 8 bytes)
+int bzip2_batch_impl(const DecodeIO &io, cudaStream_t stream) {
+    if (io.n == 0) return SWC_OK;
+    if (missing(io)) return SWC_ERR_INVALID_ARG;
+    std::vector<u64> caps;
+    int st = read_lens(io.out_cap, io.n, stream, caps);
+    return st ? st : launch_with_scratch(bzip2::Args{io}, caps.data(), stream);
 }
 
 // 32 bits at an arbitrary bit position of the host copy, MSB first (BZip2's reader order)
@@ -88,24 +89,13 @@ int bzip2_stream_by_blocks(const uint8_t *in, const u8 *d_in, size_t in_len, siz
     if (d_out.alloc(nb * cap + 64)) return SWC_OK;
     if (t.alloc()) return SWC_OK;
     if ((st = t.upload())) return st;
-    {
-        size_t total = (nb * 8 + 255) & ~(size_t)255;
-        std::vector<u64> soff(nb);
-        for (size_t k = 0; k < nb; k++) { soff[k] = total; total += bzip2::scratch_per_unit(cap); }
-        void *scratch = nullptr;
-        if (scratch_get(total, &scratch, 0)) return SWC_OK;
-        SWC_CUDA_TRY(cudaMemcpy(scratch, soff.data(), nb * 8, cudaMemcpyHostToDevice));
-        bzip2::Args a;
-        a.in_base = d_in; a.in_off = t.dev(c.in_off); a.in_len = t.dev(c.in_len);
-        a.out_base = d_out.as<u8>(); a.out_off = t.dev(c.out_off); a.out_cap = t.dev(c.out_cap);
-        a.out_len = t.dev(c.out_len); a.consumed_bits = t.dev(c.consumed); a.status = t.dev(c.status); a.n = nb;
-        a.scratch = (u8 *)scratch; a.scr_off = (const u64 *)scratch;
-        a.start_bits = t.dev(sb); a.block_mode = 1;
-        if ((st = bzip2::launch(a, 0))) return st;
-    }
-    std::vector<u64> r_len, r_used;
-    std::vector<int32_t> r_st;
-    if ((st = t.fetch(c.out_len, r_len)) || (st = t.fetch(c.consumed, r_used)) || (st = t.fetch(c.status, r_st))) return st;
+    const std::vector<u64> caps(nb, cap);
+    bool no_scratch = false;
+    if ((st = launch_with_scratch(bzip2::Args{c.bind(t, d_in, d_out.as<u8>(), 0, nb), nullptr, nullptr, t.dev(sb), 1}, caps.data(), 0,
+                                  &no_scratch)))
+        return no_scratch ? SWC_OK : st;
+    UnitCols::Results res;
+    if ((st = c.fetch(t, res))) return st;
     // the in-order walk: every block must end where the next magic starts, the last one at the end-of-stream magic
     uint32_t total_crc = 0;
     UnitTable g;
@@ -113,13 +103,13 @@ int bzip2_stream_by_blocks(const uint8_t *in, const u8 *d_in, size_t in_len, siz
     u64 *g_dst = g.host(dst);
     u64 out_total = 0;
     for (size_t k = 0; k < nb; k++) {
-        const u64 ends_at = (pos[k] & ~7ull) + r_used[k];            // consumed is counted from the unit's first byte
+        const u64 ends_at = (pos[k] & ~7ull) + res.consumed[k];            // consumed is counted from the unit's first byte
         const u64 next = k + 1 < nb ? pos[k + 1] : end_pos;
-        if (r_st[k] != SWC_OK || ends_at != next) return SWC_OK;
+        if (res.status[k] != SWC_OK || ends_at != next) return SWC_OK;
         const uint32_t block_crc = bits32_at(in, in_len, pos[k] + 48);
         total_crc = ((total_crc << 1) | (total_crc >> 31)) ^ block_crc;  // BZip2.swift:83-84
         g_dst[k] = out_total;
-        out_total += r_len[k];
+        out_total += res.out_len[k];
     }
     if (end_pos + 80 > (u64)in_len * 8) return SWC_OK;
     if (bits32_at(in, in_len, end_pos + 48) != total_crc) return SWC_OK;   // the sequential path reports wrongCRC with its payload
@@ -147,11 +137,9 @@ int bzip2_unit_device(const u8 *d_in, size_t in_len, size_t start, UnitResult &r
     UnitTable t;
     UnitCols c(t, 1);
     // BZip2 cannot report the final size before it has decoded everything: x4 per attempt
-    return decode_unit(t, c, start, in_len, (in_len - start) * 16 + (1u << 20), 8,
-                       [](size_t cap, size_t) { return cap >= ((size_t)1 << 32) ? 0 : cap * 4; }, [&](u8 *out, size_t) {
-        return bzip2_batch_impl(d_in, t.dev(c.in_off), t.dev(c.in_len), out, t.dev(c.out_off), t.dev(c.out_cap), t.dev(c.out_len),
-                                t.dev(c.consumed), t.dev(c.status), 1, 0);
-    }, r);
+    return decode_unit(t, c, d_in, start, in_len, (in_len - start) * 16 + (1u << 20), 8,
+                       [](size_t cap, size_t) { return cap >= ((size_t)1 << 32) ? 0 : cap * 4; },
+                       [](const DecodeIO &io, size_t) { return bzip2_batch_impl(io, 0); }, r);
 }
 
 }  // namespace
@@ -164,7 +152,8 @@ int32_t swc_bzip2_decompress_batch(const uint8_t *in_base, const uint64_t *in_of
                                    uint64_t n, void *cuda_stream) {
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
-    return bzip2_batch_impl(in_base, in_off, in_len, out_base, out_off, out_cap, out_len, consumed_bits, status, n, (cudaStream_t)cuda_stream);
+    const DecodeIO io{{in_base, in_off, in_len, out_base, out_off, out_cap, out_len, status, n}, consumed_bits};
+    return bzip2_batch_impl(io, (cudaStream_t)cuda_stream);
 }
 
 // BZip2.decompress(data:) BZip2.swift:22-26 (+ reader form :50)
@@ -242,17 +231,16 @@ int32_t swc_bzip2_multi_decompress(const uint8_t *in, size_t in_len,
                 DevBuf d_out;
                 if ((st = d_out.alloc(out_total + 64))) return st;
                 if ((st = t.alloc()) || (st = t.upload())) return st;
-                if ((st = bzip2_batch_impl(d_in.as<u8>(), t.dev(c.in_off), t.dev(c.in_len), d_out.as<u8>(), t.dev(c.out_off), t.dev(c.out_cap),
-                                           t.dev(c.out_len), t.dev(c.consumed), t.dev(c.status), g, 0))) return st;
-                std::vector<u64> r_len, r_used;
-                std::vector<int32_t> r_st;
-                if ((st = t.fetch(c.out_len, r_len)) || (st = t.fetch(c.consumed, r_used)) || (st = t.fetch(c.status, r_st))) return st;
+                if ((st = bzip2_batch_impl(c.bind(t, d_in.as<u8>(), d_out.as<u8>(), 0, g), 0))) return st;
+                UnitCols::Results res;
+                if ((st = c.fetch(t, res))) return st;
                 for (size_t j = 0; j < g; j++) {
-                    const bool ok = r_st[j] == SWC_OK && (r_used[j] + 7) / 8 == h_len[j];
+                    const u64 r_len = res.out_len[j];
+                    const bool ok = res.status[j] == SWC_OK && (res.consumed[j] + 7) / 8 == h_len[j];
                     if (!ok) { off = cand[k0 + j]; handed_over = true; break; }   // sequential loop re-decodes this stream
-                    uint8_t *dst = o.grow(r_len[j]);
+                    uint8_t *dst = o.grow(r_len);
                     if (!dst) return SWC_ERR_OUTPUT_OVERFLOW;
-                    if (r_len[j]) SWC_CUDA_TRY(cudaMemcpy(dst, d_out.as<u8>() + h_ooff[j], r_len[j], cudaMemcpyDeviceToHost));
+                    if (r_len) SWC_CUDA_TRY(cudaMemcpy(dst, d_out.as<u8>() + h_ooff[j], r_len, cudaMemcpyDeviceToHost));
                     ends.push_back(o.len);
                     off = cand[k0 + j] + h_len[j];
                 }

@@ -7,25 +7,19 @@
 
 namespace swc {
 
-int deflate_batch_impl(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, const uint8_t *start_bits,
-                              uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t out_total,
-                              uint64_t *out_len, uint64_t *consumed_bits, int32_t *status, uint64_t n,
-                              void *scratch, size_t scratch_bytes, cudaStream_t stream) {
-    if (n == 0) return SWC_OK;
-    if (!in_base || !in_off || !in_len || !out_base || !out_off || !out_cap || !out_len || !consumed_bits || !status)
-        return SWC_ERR_INVALID_ARG;
-    const size_t need = inflate::scratch_bytes(n, out_total);
+int deflate_batch_impl(const DecodeIO &io, const uint8_t *start_bits, uint64_t out_total, void *scratch, size_t scratch_bytes,
+                       cudaStream_t stream) {
+    if (io.n == 0) return SWC_OK;
+    if (missing(io)) return SWC_ERR_INVALID_ARG;
+    const size_t need = inflate::scratch_bytes(io.n, out_total);
     if (!scratch) {
         int st = scratch_get(need, &scratch, stream);
         if (st) return st;
     } else if (scratch_bytes < need) {
         return SWC_ERR_INVALID_ARG;
     }
-    inflate::BatchArgs a;
-    a.in_base = in_base; a.in_off = in_off; a.in_len = in_len; a.start_bits = start_bits;
-    a.out_base = out_base; a.out_off = out_off; a.out_cap = out_cap;
-    a.out_len = out_len; a.consumed_bits = consumed_bits; a.status = status; a.n = n;
-    inflate::seat_scratch(a, scratch, n, 0, 1, 0);
+    inflate::BatchArgs a{io, start_bits};
+    inflate::seat_scratch(a, scratch, io.n, 0, 1, 0);
     return inflate::launch(a, stream);
 }
 
@@ -38,10 +32,8 @@ int deflate_unit_device(const u8 *d_in, size_t in_len, size_t start_bit_abs, Uni
     const Col<u8> sb = t.in<u8>(1);
     *t.host(sb) = (u8)(start_bit_abs & 7);
     const size_t first_cap = hint ? hint : (in_len - start_byte) * 4 + 65536;
-    int st = decode_unit(t, c, start_byte, in_len, first_cap, 3, [](size_t, size_t need) { return need; }, [&](u8 *out, size_t cap) {
-        return deflate_batch_impl(d_in, t.dev(c.in_off), t.dev(c.in_len), t.dev(sb), out, t.dev(c.out_off), t.dev(c.out_cap), cap,
-                                  t.dev(c.out_len), t.dev(c.consumed), t.dev(c.status), 1, nullptr, 0, 0);
-    }, r);
+    int st = decode_unit(t, c, d_in, start_byte, in_len, first_cap, 3, [](size_t, size_t need) { return need; },
+                         [&](const DecodeIO &io, size_t cap) { return deflate_batch_impl(io, t.dev(sb), cap, nullptr, 0, 0); }, r);
     if (st) return st;
     if (r.status == SWC_INTERNAL_NEEDS_SLOW) r.status = SWC_ERR_UNSUPPORTED;
     return SWC_OK;
@@ -65,8 +57,8 @@ int32_t swc_deflate_decompress_batch(const uint8_t *in_base, const uint64_t *in_
                                      uint64_t n, void *scratch, size_t scratch_bytes, void *cuda_stream) {
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
-    return deflate_batch_impl(in_base, in_off, in_len, start_bits, out_base, out_off, out_cap, out_capacity_total,
-                              out_len, consumed_bits, status, n, scratch, scratch_bytes, (cudaStream_t)cuda_stream);
+    const DecodeIO io{{in_base, in_off, in_len, out_base, out_off, out_cap, out_len, status, n}, consumed_bits};
+    return deflate_batch_impl(io, start_bits, out_capacity_total, scratch, scratch_bytes, (cudaStream_t)cuda_stream);
 }
 
 // Host-buffer batch: the units are cut into slices that flow through three CUDA streams, so the host->device copy of
@@ -80,7 +72,8 @@ int32_t swc_deflate_decompress_batch_host(const uint8_t *in_base, const uint64_t
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
     if (n == 0) return SWC_OK;
-    if (!in_base || !in_off || !in_len || !out_base || !out_off || !out_cap || !out_len || !consumed_bits || !status) return SWC_ERR_INVALID_ARG;
+    if (missing(DecodeIO{{in_base, in_off, in_len, out_base, out_off, out_cap, out_len, status, n}, consumed_bits}))
+        return SWC_ERR_INVALID_ARG;
     DeviceCtx &ctx = device_ctx();                                       // streams / event / pinned result buffer of THIS device
     cudaStream_t *streams = ctx.streams;
     if (!streams[0]) {
@@ -99,9 +92,7 @@ int32_t swc_deflate_decompress_batch_host(const uint8_t *in_base, const uint64_t
     if (monotone && n >= 4096) { S = s_env > 0 ? (uint64_t)s_env : n / 2048; if (S > 32) S = 32; if (S > 64) S = 64; }
     // the unit table lives in an arena; its columns are filled straight from the caller's arrays
     UnitTable t;
-    const Col<u64> d_in_off = t.out<u64>(n), d_in_len = t.out<u64>(n), d_out_off = t.out<u64>(n), d_out_cap = t.out<u64>(n);
-    const Col<u64> d_out_len = t.out<u64>(n), d_cons = t.out<u64>(n);
-    const Col<int32_t> d_status = t.out<int32_t>(n);
+    const UnitCols c(t, n, false);
     void *p_in = nullptr, *p_out = nullptr, *p_meta = nullptr, *p_scr = nullptr;
     const size_t tb = n * 8;
     const int tickets = 64;                                              // up to 64 slices, one ticket block each
@@ -122,10 +113,10 @@ int32_t swc_deflate_decompress_batch_host(const uint8_t *in_base, const uint64_t
     u8 *h_res = ctx.h_res;
     u64 *h_out_len = (u64 *)h_res, *h_cons = h_out_len + n;
     int32_t *h_status = (int32_t *)(h_cons + n);
-    SWC_CUDA_TRY(cudaMemcpyAsync(t.dev(d_in_off), in_off, tb, cudaMemcpyHostToDevice, streams[0]));
-    SWC_CUDA_TRY(cudaMemcpyAsync(t.dev(d_in_len), in_len, tb, cudaMemcpyHostToDevice, streams[0]));
-    SWC_CUDA_TRY(cudaMemcpyAsync(t.dev(d_out_off), out_off, tb, cudaMemcpyHostToDevice, streams[0]));
-    SWC_CUDA_TRY(cudaMemcpyAsync(t.dev(d_out_cap), out_cap, tb, cudaMemcpyHostToDevice, streams[0]));
+    SWC_CUDA_TRY(cudaMemcpyAsync(t.dev(c.in_off), in_off, tb, cudaMemcpyHostToDevice, streams[0]));
+    SWC_CUDA_TRY(cudaMemcpyAsync(t.dev(c.in_len), in_len, tb, cudaMemcpyHostToDevice, streams[0]));
+    SWC_CUDA_TRY(cudaMemcpyAsync(t.dev(c.out_off), out_off, tb, cudaMemcpyHostToDevice, streams[0]));
+    SWC_CUDA_TRY(cudaMemcpyAsync(t.dev(c.out_cap), out_cap, tb, cudaMemcpyHostToDevice, streams[0]));
     SWC_CUDA_TRY(cudaEventRecord(tables_ready, streams[0]));
     for (uint64_t k = 0; k < S; k++) {
         const uint64_t b = n * k / S, e = n * (k + 1) / S;
@@ -134,16 +125,13 @@ int32_t swc_deflate_decompress_batch_host(const uint8_t *in_base, const uint64_t
         SWC_CUDA_TRY(cudaStreamWaitEvent(s, tables_ready, 0));
         const uint64_t i0 = S == 1 ? 0 : in_off[b], i1 = S == 1 ? in_total : in_off[e - 1] + in_len[e - 1];
         SWC_CUDA_TRY(cudaMemcpyAsync((u8 *)p_in + i0, in_base + i0, i1 - i0, cudaMemcpyHostToDevice, s));
-        inflate::BatchArgs a;
-        a.in_base = (const u8 *)p_in; a.in_off = t.dev(d_in_off) + b; a.in_len = t.dev(d_in_len) + b; a.start_bits = nullptr;
-        a.out_base = (u8 *)p_out; a.out_off = t.dev(d_out_off) + b; a.out_cap = t.dev(d_out_cap) + b;
-        a.out_len = t.dev(d_out_len) + b; a.consumed_bits = t.dev(d_cons) + b; a.status = t.dev(d_status) + b; a.n = e - b;
+        inflate::BatchArgs a{c.bind(t, (const u8 *)p_in, (u8 *)p_out, b, e - b), nullptr};
         inflate::seat_scratch(a, p_scr, n, b, tickets, (int)k);
         if ((st = inflate::launch(a, s))) return st;
         if ((st = copy_back_regions(out_base, (const u8 *)p_out, out_off, out_cap, b, e, s))) return st;
-        SWC_CUDA_TRY(cudaMemcpyAsync(h_out_len + b, t.dev(d_out_len) + b, (e - b) * 8, cudaMemcpyDeviceToHost, s));
-        SWC_CUDA_TRY(cudaMemcpyAsync(h_cons + b, t.dev(d_cons) + b, (e - b) * 8, cudaMemcpyDeviceToHost, s));
-        SWC_CUDA_TRY(cudaMemcpyAsync(h_status + b, t.dev(d_status) + b, (e - b) * 4, cudaMemcpyDeviceToHost, s));
+        SWC_CUDA_TRY(cudaMemcpyAsync(h_out_len + b, a.out_len, (e - b) * 8, cudaMemcpyDeviceToHost, s));
+        SWC_CUDA_TRY(cudaMemcpyAsync(h_cons + b, a.consumed, (e - b) * 8, cudaMemcpyDeviceToHost, s));
+        SWC_CUDA_TRY(cudaMemcpyAsync(h_status + b, a.status, (e - b) * 4, cudaMemcpyDeviceToHost, s));
     }
     for (int i = 0; i < 3; i++) SWC_CUDA_TRY(cudaStreamSynchronize(streams[i]));
     memcpy(out_len, h_out_len, n * 8);

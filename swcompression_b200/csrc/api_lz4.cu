@@ -80,14 +80,11 @@ int run_blocks(DeviceInput &dev, const std::vector<Block> &blocks, int mode, boo
     for (int attempt = 0; attempt < 2; attempt++) {
         if ((st = d_out_keep.alloc(total))) return st;
         if ((st = t.upload())) return st;
-        lz4::Args a;
-        a.in_base = dev.in.as<u8>(); a.blk_off = t.dev(blk_off); a.blk_len = t.dev(blk_len); a.first_blk = t.dev(first); a.n_blk = t.dev(count);
-        a.dict = use_dict && dev.have_dict ? dev.dict.as<u8>() : nullptr;
-        a.dict_len = use_dict && dev.have_dict ? dev.dict_len : 0;
+        lz4::Args a{{dev.in.as<u8>(), t.dev(blk_off), t.dev(blk_len), d_out_keep.as<u8>(), t.dev(unit_off), t.dev(unit_cap),
+                     t.dev(unit_len), t.dev(status), nunits},
+                    t.dev(first), t.dev(count), use_dict && dev.have_dict ? dev.dict.as<u8>() : nullptr,
+                    use_dict && dev.have_dict ? dev.dict_len : 0, nullptr};
         if (mode == 1 && a.dict_len > 65536) { a.dict += a.dict_len - 65536; a.dict_len = 65536; }    // LZ4.swift:309
-        a.out_base = d_out_keep.as<u8>(); a.out_off = t.dev(unit_off); a.out_cap = t.dev(unit_cap); a.out_len = t.dev(unit_len);
-        a.status = t.dev(status); a.n = nunits;
-        a.scratch = nullptr;
         if (mode == 0) {               // one block per unit: take the two-phase (parse + 8-wide execute) path
             uint64_t tot = 0;
             for (size_t i = 0; i < nb; i++) tot += blocks[i].len;
@@ -262,11 +259,8 @@ int32_t swc_lz4_block_decompress_batch(const uint8_t *in_base, const uint64_t *i
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
     if (n == 0) return SWC_OK;
-    if (!in_base || !in_off || !in_len || !out_base || !out_off || !out_cap || !out_len || !status) return SWC_ERR_INVALID_ARG;
-    lz4::Args a;
-    a.in_base = in_base; a.blk_off = in_off; a.blk_len = in_len; a.first_blk = nullptr; a.n_blk = nullptr;
-    a.dict = dict; a.dict_len = dict ? dict_len : 0;
-    a.out_base = out_base; a.out_off = out_off; a.out_cap = out_cap; a.out_len = out_len; a.status = status; a.n = n;
+    lz4::Args a{{in_base, in_off, in_len, out_base, out_off, out_cap, out_len, status, n}, nullptr, nullptr, dict, dict ? dict_len : 0, nullptr};
+    if (missing(a)) return SWC_ERR_INVALID_ARG;
     // two-phase path needs a record scratch sized from the compressed lengths: fetch them once (n x 8 bytes)
     {
         std::vector<u64> lens;
@@ -290,7 +284,7 @@ int32_t swc_lz4_block_decompress_batch_host(const uint8_t *in_base, const uint64
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
     if (n == 0) return SWC_OK;
-    if (!in_base || !in_off || !in_len || !out_base || !out_off || !out_cap || !out_len || !status) return SWC_ERR_INVALID_ARG;
+    if (missing(UnitIO{in_base, in_off, in_len, out_base, out_off, out_cap, out_len, status, n})) return SWC_ERR_INVALID_ARG;
     bool monotone;
     int st = check_host_units(in_off, in_len, in_total, out_off, out_cap, out_total, n, &monotone);
     if (st) return st;

@@ -34,13 +34,9 @@ int lzma_unit_device(const u8 *d_in, size_t in_len, size_t start, const LzmaJob 
     const Col<i64> dict_size = t.in<i64>(1), usize = t.in<i64>(1);
     *t.host(dict_byte) = job.dict_byte; *t.host(props) = job.props; *t.host(dict_size) = job.dict_size; *t.host(usize) = job.usize;
     // LZMA cannot size its output without decoding it (the dictionary IS the output): x4 per attempt
-    return decode_unit(t, c, start, in_len, cap_hint ? cap_hint : (in_len - start) * 8 + (1u << 20), 8,
-                       [](size_t cap, size_t) { return cap >= ((size_t)1 << 33) ? 0 : cap * 4; }, [&](u8 *out, size_t) {
-        lzma::Args a;
-        a.mode = job.mode; a.in_base = d_in; a.in_off = t.dev(c.in_off); a.in_len = t.dev(c.in_len);
-        a.dict_bytes = t.dev(dict_byte); a.props = t.dev(props); a.dict_size = t.dev(dict_size); a.usize = t.dev(usize);
-        a.out_base = out; a.out_off = t.dev(c.out_off); a.out_cap = t.dev(c.out_cap); a.out_len = t.dev(c.out_len);
-        a.consumed = t.dev(c.consumed); a.status = t.dev(c.status); a.n = 1; a.lit_scratch = lit.as<u16>();
+    return decode_unit(t, c, d_in, start, in_len, cap_hint ? cap_hint : (in_len - start) * 8 + (1u << 20), 8,
+                       [](size_t cap, size_t) { return cap >= ((size_t)1 << 33) ? 0 : cap * 4; }, [&](const DecodeIO &io, size_t) {
+        const lzma::Args a{io, job.mode, t.dev(dict_byte), t.dev(props), t.dev(dict_size), t.dev(usize), lit.as<u16>()};
         return lzma::launch(a, 0);
     }, r);
 }
@@ -349,17 +345,13 @@ int xz_prefetch(const uint8_t *in, size_t n, const u8 *d_in, Prefetch &pf) {
     if (pf.out.alloc(run + 64) || t.alloc()) return SWC_OK;       // no room: the in-order parser decodes block by block
     int st = t.upload();
     if (st) return st;
-    lzma::Args a;
-    a.mode = lzma::MODE_LZMA2; a.in_base = d_in; a.in_off = t.dev(c.in_off); a.in_len = t.dev(c.in_len); a.dict_bytes = t.dev(dict);
-    a.props = nullptr; a.dict_size = nullptr; a.usize = nullptr;
-    a.out_base = pf.out.as<u8>(); a.out_off = t.dev(c.out_off); a.out_cap = t.dev(c.out_cap); a.out_len = t.dev(c.out_len);
-    a.consumed = t.dev(c.consumed); a.status = t.dev(c.status); a.n = nb; a.lit_scratch = nullptr;
+    const lzma::Args a{c.bind(t, d_in, pf.out.as<u8>(), 0, nb), lzma::MODE_LZMA2, t.dev(dict), nullptr, nullptr, nullptr, nullptr};
     if ((st = lzma::launch(a, 0))) return st;
-    std::vector<uint64_t> r_len, r_used;
-    std::vector<int32_t> r_st;
-    if ((st = t.fetch(c.out_len, r_len)) || (st = t.fetch(c.consumed, r_used)) || (st = t.fetch(c.status, r_st))) return st;
+    UnitCols::Results res;
+    if ((st = c.fetch(t, res))) return st;
     for (size_t i = 0; i < nb; i++)
-        if (r_st[i] == SWC_OK) pf.by_offset[blks[i].data_off] = PrefetchEntry{(size_t)o_off[i], (size_t)r_len[i], (size_t)r_used[i], blks[i].dict_byte};
+        if (res.status[i] == SWC_OK)
+            pf.by_offset[blks[i].data_off] = PrefetchEntry{(size_t)o_off[i], (size_t)res.out_len[i], (size_t)res.consumed[i], blks[i].dict_byte};
     return SWC_OK;
 }
 
@@ -456,14 +448,10 @@ int32_t swc_lzma_decompress_batch(const uint8_t *in_base, const uint64_t *in_off
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
     if (n == 0) return SWC_OK;
-    if (!in_base || !in_off || !in_len || !props || !dict_size || !uncompressed_size || !out_base || !out_off || !out_cap || !out_len ||
-        !consumed_bytes || !status)
-        return SWC_ERR_INVALID_ARG;
-    lzma::Args a;
-    a.mode = lzma::MODE_RAW; a.in_base = in_base; a.in_off = in_off; a.in_len = in_len; a.dict_bytes = nullptr;
-    a.props = props; a.dict_size = (const i64 *)dict_size; a.usize = (const i64 *)uncompressed_size;
-    a.out_base = out_base; a.out_off = out_off; a.out_cap = out_cap; a.out_len = out_len; a.consumed = consumed_bytes;
-    a.status = status; a.n = n; a.lit_scratch = nullptr;      // lc + lp > 4 would need 6 MB of literal coders per unit: refused here
+    // no lit_scratch: lc + lp > 4 would need 6 MB of literal coders per unit, such units are refused here
+    const lzma::Args a{{{in_base, in_off, in_len, out_base, out_off, out_cap, out_len, status, n}, consumed_bytes},
+                       lzma::MODE_RAW, nullptr, props, (const i64 *)dict_size, (const i64 *)uncompressed_size, nullptr};
+    if (missing(a) || !props || !dict_size || !uncompressed_size) return SWC_ERR_INVALID_ARG;
     return lzma::launch(a, (cudaStream_t)cuda_stream);
 }
 
@@ -475,13 +463,10 @@ int32_t swc_lzma2_decompress_batch(const uint8_t *in_base, const uint64_t *in_of
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
     if (n == 0) return SWC_OK;
-    if (!in_base || !in_off || !in_len || !dict_bytes || !out_base || !out_off || !out_cap || !out_len || !consumed_bytes || !status)
-        return SWC_ERR_INVALID_ARG;
-    lzma::Args a;
-    a.mode = lzma::MODE_LZMA2; a.in_base = in_base; a.in_off = in_off; a.in_len = in_len; a.dict_bytes = dict_bytes;
-    a.props = nullptr; a.dict_size = nullptr; a.usize = nullptr;
-    a.out_base = out_base; a.out_off = out_off; a.out_cap = out_cap; a.out_len = out_len; a.consumed = consumed_bytes;
-    a.status = status; a.n = n; a.lit_scratch = nullptr;      // a chunk with lc + lp > 4 would need 6 MB of literal coders: refused here
+    // no lit_scratch: a chunk with lc + lp > 4 would need 6 MB of literal coders, such units are refused here
+    const lzma::Args a{{{in_base, in_off, in_len, out_base, out_off, out_cap, out_len, status, n}, consumed_bytes},
+                       lzma::MODE_LZMA2, dict_bytes, nullptr, nullptr, nullptr, nullptr};
+    if (missing(a) || !dict_bytes) return SWC_ERR_INVALID_ARG;
     return lzma::launch(a, (cudaStream_t)cuda_stream);
 }
 

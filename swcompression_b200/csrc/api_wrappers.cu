@@ -198,8 +198,7 @@ int gzip_multi_batch(const uint8_t *in, size_t n, const u8 *d_in, HostOut &o, st
             h_outoff[c.unit] = run; t.host(uc.out_cap)[c.unit] = c.isize;
             run += round16((size_t)c.isize);
         }
-        std::vector<u64> h_outlen, h_cons;
-        std::vector<int32_t> h_status;
+        UnitCols::Results res;
         std::vector<uint32_t> h_crc;
         DevBuf d_out;
         if (nu) {
@@ -209,11 +208,9 @@ int gzip_multi_batch(const uint8_t *in, size_t n, const u8 *d_in, HostOut &o, st
             { void *scr = nullptr; if (scratch_get(inflate_scratch_bytes(nu, out_total), &scr, stream)) return SWC_OK; }
             int st = t.upload(stream);
             if (st) return st;
-            if ((st = deflate_batch_impl(d_in, t.dev(uc.in_off), t.dev(uc.in_len), nullptr, d_out.as<u8>(), t.dev(uc.out_off), t.dev(uc.out_cap),
-                                         out_total, t.dev(uc.out_len), t.dev(uc.consumed), t.dev(uc.status), nu, nullptr, 0, stream))) return st;
+            if ((st = deflate_batch_impl(uc.bind(t, d_in, d_out.as<u8>(), 0, nu), nullptr, out_total, nullptr, 0, stream))) return st;
             if ((st = checks::crc32_units(d_out.as<u8>(), t.dev(uc.out_off), t.dev(uc.out_len), t.dev(uc.status), t.dev(crc), nu, stream))) return st;
-            if ((st = t.fetch(uc.out_len, h_outlen, stream)) || (st = t.fetch(uc.consumed, h_cons, stream)) ||
-                (st = t.fetch(uc.status, h_status, stream)) || (st = t.fetch(crc, h_crc, stream))) return st;
+            if ((st = uc.fetch(t, res, stream)) || (st = t.fetch(crc, h_crc, stream))) return st;
         }
         if (trace) fprintf(stderr, "[swc] gzip round: %zu units, %.1f MB out, decode+crc done at %.1f ms\n", nu, out_total / 1e6, now() - t0);
         // ---- the in-order walk: accept the longest validated prefix
@@ -222,7 +219,7 @@ int gzip_multi_batch(const uint8_t *in, size_t n, const u8 *d_in, HostOut &o, st
             const Cand &c = cs[accepted];
             if (c.unit < 0) break;
             const size_t u = (size_t)c.unit;
-            if (h_status[u] != SWC_OK || c.dstart + (h_cons[u] + 7) / 8 + 8 != c.next || h_outlen[u] != c.isize) break;
+            if (res.status[u] != SWC_OK || c.dstart + (res.consumed[u] + 7) / 8 + 8 != c.next || res.out_len[u] != c.isize) break;
             if (h_crc[u] != c.crc) { *result = SWC_GZIP_WRONG_CRC; *stop = true; accepted++; break; }   // the member is still returned
         }
         if (accepted) {
@@ -231,8 +228,8 @@ int gzip_multi_batch(const uint8_t *in, size_t n, const u8 *d_in, HostOut &o, st
             size_t acc_bytes = 0;
             for (size_t i = 0; i < accepted; i++) {
                 const size_t u = (size_t)cs[i].unit;
-                g.host(src)[i] = h_outoff[u]; g.host(len)[i] = h_outlen[u]; g.host(dst)[i] = acc_bytes;
-                acc_bytes += h_outlen[u];
+                g.host(src)[i] = h_outoff[u]; g.host(len)[i] = res.out_len[u]; g.host(dst)[i] = acc_bytes;
+                acc_bytes += res.out_len[u];
             }
             DevBuf d_g;
             if (g.alloc()) return SWC_OK;

@@ -577,7 +577,7 @@ done:
 #undef FAIL
     if (lane == 0) {
         a.out_len[unit] = op;
-        a.consumed_bits[unit] = (u64)(total_bits - br.avail);
+        a.consumed[unit] = (u64)(total_bits - br.avail);
         a.status[unit] = status;
     }
 }

@@ -5,14 +5,7 @@
 namespace swc {
 namespace bzip2 {
 
-struct Args {
-    const u8 *in_base;
-    const u64 *in_off, *in_len;
-    u8 *out_base;
-    const u64 *out_off, *out_cap;
-    u64 *out_len, *consumed_bits;
-    int32_t *status;
-    u64 n;
+struct Args : DecodeIO {
     u8 *scratch;
     const u64 *scr_off;      // per unit, bytes into scratch
     const u8 *start_bits = nullptr;   // block mode: bit offset (0..7) of the block magic inside the unit's first byte

@@ -20,7 +20,7 @@ namespace swc {
 
 __device__ __forceinline__ u32 lane_id() { return threadIdx.x & 31; }
 
-// the unit table of a batched compressor: unit i reads in_base[in_off[i], in_off[i] + in_len[i]) and writes
+// the unit table of a batched kernel: unit i reads in_base[in_off[i], in_off[i] + in_len[i]) and writes
 // out_base[out_off[i], out_off[i] + out_cap[i]); out_len[i] and status[i] are its results.  Each codec's Args extends it.
 struct UnitIO {
     const u8 *in_base;
@@ -30,6 +30,11 @@ struct UnitIO {
     u64 *out_len;
     int32_t *status;
     u64 n;
+};
+// the unit table of a batched decoder: consumed[i] is how much of its input unit i read, in bits for Deflate and BZip2,
+// in bytes for LZMA
+struct DecodeIO : UnitIO {
+    u64 *consumed;
 };
 
 // launch bookkeeping (swc_kernel_launches)

@@ -114,13 +114,39 @@ class UnitTable {
     DevBuf dev_;
 };
 
-// the columns every batched decoder takes: the unit's input and output regions in, its results out
+// a null pointer among a caller's unit table: the call returns SWC_ERR_INVALID_ARG
+inline bool missing(const UnitIO &a) {
+    return !a.in_base || !a.in_off || !a.in_len || !a.out_base || !a.out_off || !a.out_cap || !a.out_len || !a.status;
+}
+inline bool missing(const DecodeIO &a) { return missing((const UnitIO &)a) || !a.consumed; }
+
+// the columns every batched decoder takes: the unit's input and output regions in, its results out.  With
+// in_on_host = false the input columns are device-only too, for a table the caller's own copies fill.
 struct UnitCols {
     Col<u64> in_off, in_len, out_off, out_cap, out_len, consumed;
     Col<int32_t> status;
-    UnitCols(UnitTable &t, size_t n)
-        : in_off(t.in<u64>(n)), in_len(t.in<u64>(n)), out_off(t.in<u64>(n)), out_cap(t.in<u64>(n)),
-          out_len(t.out<u64>(n)), consumed(t.out<u64>(n)), status(t.out<int32_t>(n)) {}
+    UnitCols(UnitTable &t, size_t n, bool in_on_host = true)
+        : in_off(in_col(t, n, in_on_host)), in_len(in_col(t, n, in_on_host)), out_off(in_col(t, n, in_on_host)),
+          out_cap(in_col(t, n, in_on_host)), out_len(t.out<u64>(n)), consumed(t.out<u64>(n)), status(t.out<int32_t>(n)) {}
+    // a decoder's unit columns for units [first, first + count) of the seated table `t`, reading in_base, writing out_base
+    DecodeIO bind(const UnitTable &t, const u8 *in_base, u8 *out_base, u64 first, u64 count) const {
+        return DecodeIO{{in_base, t.dev(in_off) + first, t.dev(in_len) + first, out_base, t.dev(out_off) + first,
+                         t.dev(out_cap) + first, t.dev(out_len) + first, t.dev(status) + first, count},
+                        t.dev(consumed) + first};
+    }
+    struct Results {
+        std::vector<u64> out_len, consumed;
+        std::vector<int32_t> status;
+    };
+    // the whole table's results (blocking: waits for `s`)
+    int fetch(const UnitTable &t, Results &r, cudaStream_t s = 0) const {
+        int st;
+        if ((st = t.fetch(out_len, r.out_len, s)) || (st = t.fetch(consumed, r.consumed, s)) || (st = t.fetch(status, r.status, s)))
+            return st;
+        return SWC_OK;
+    }
+  private:
+    static Col<u64> in_col(UnitTable &t, size_t n, bool on_host) { return on_host ? t.in<u64>(n) : t.out<u64>(n); }
 };
 
 // result of decoding ONE unit that is already resident on the device
@@ -133,10 +159,10 @@ struct UnitResult {
 
 // Decodes the unit d_in[start, in_len) described by the 1-unit table `t` / `c` (the codec's own columns already declared
 // and filled) into r.out, growing the output until it fits: `cap` bytes first, then, while the unit overflows and
-// `attempts` last, grow(cap, reported out_len) bytes — 0 stops.  launch(out, cap) runs the codec on the table.
+// `attempts` last, grow(cap, reported out_len) bytes — 0 stops.  launch(io, cap) runs the codec on the table's columns io.
 template <typename Grow, typename Launch>
-int decode_unit(UnitTable &t, const UnitCols &c, size_t start, size_t in_len, size_t cap, int attempts, Grow grow,
-                Launch launch, UnitResult &r) {
+int decode_unit(UnitTable &t, const UnitCols &c, const u8 *d_in, size_t start, size_t in_len, size_t cap, int attempts,
+                Grow grow, Launch launch, UnitResult &r) {
     int st = t.alloc();
     if (st) return st;
     *t.host(c.in_off) = start;
@@ -146,13 +172,12 @@ int decode_unit(UnitTable &t, const UnitCols &c, size_t start, size_t in_len, si
         if ((st = r.out.alloc(cap))) return st;
         *t.host(c.out_cap) = cap;
         if ((st = t.upload())) return st;
-        if ((st = launch(r.out.as<u8>(), cap))) return st;
-        std::vector<u64> len, used;
-        std::vector<int32_t> status;
-        if ((st = t.fetch(c.out_len, len)) || (st = t.fetch(c.consumed, used)) || (st = t.fetch(c.status, status))) return st;
-        r.out_len = (size_t)len[0];
-        r.consumed = (size_t)used[0];
-        r.status = status[0];
+        if ((st = launch(c.bind(t, d_in, r.out.as<u8>(), 0, 1), cap))) return st;
+        UnitCols::Results res;
+        if ((st = c.fetch(t, res))) return st;
+        r.out_len = (size_t)res.out_len[0];
+        r.consumed = (size_t)res.consumed[0];
+        r.status = res.status[0];
         if (r.status != SWC_ERR_OUTPUT_OVERFLOW || !(cap = grow(cap, r.out_len))) break;
     }
     return SWC_OK;
@@ -161,11 +186,9 @@ int decode_unit(UnitTable &t, const UnitCols &c, size_t start, size_t in_len, si
 // Deflate stream starting at byte `start` + `start_bit` bits inside d_in[0..in_len)
 int deflate_unit_device(const u8 *d_in, size_t in_len, size_t start_bit_abs, UnitResult &r, size_t hint = 0);
 
-// batched Deflate on device-resident tables (api_deflate.cu); scratch == nullptr -> library pool
-int deflate_batch_impl(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, const uint8_t *start_bits,
-                       uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t out_total,
-                       uint64_t *out_len, uint64_t *consumed_bits, int32_t *status, uint64_t n,
-                       void *scratch, size_t scratch_bytes, cudaStream_t stream);
+// batched Deflate on device-resident tables (api_deflate.cu); start_bits may be null; scratch == nullptr -> library pool
+int deflate_batch_impl(const DecodeIO &io, const uint8_t *start_bits, uint64_t out_total, void *scratch, size_t scratch_bytes,
+                       cudaStream_t stream);
 
 // large transfers between pageable host memory and the device: T threads x (stream + two pinned bounce buffers) (runtime.cu)
 int copy_pageable(void *dst, const void *src, size_t bytes, bool to_device);

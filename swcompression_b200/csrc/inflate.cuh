@@ -6,15 +6,8 @@
 namespace swc {
 namespace inflate {
 
-struct BatchArgs {
-    const u8 *in_base;
-    const u64 *in_off, *in_len;
+struct BatchArgs : DecodeIO {
     const u8 *start_bits;      // may be null
-    u8 *out_base;
-    const u64 *out_off, *out_cap;
-    u64 *out_len, *consumed_bits;
-    int32_t *status;
-    u64 n;
     u32 *rec_base;             // literal + match-record scratch (format below)
     u32 *rec_count;            // n entries
     unsigned long long *ticket; // unit ticket counters of the persistent-lane kernels: [0] K1w, [1] K1L (zeroed by the launcher)

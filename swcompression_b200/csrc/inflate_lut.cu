@@ -493,7 +493,7 @@ inflate_lut_kernel(BatchArgs a) {
             const bool fits = em.finish(region_bytes(a.out_off[unit], cap64));
             if (status == SWC_OK && (u64)em.op > cap64) status = SWC_ERR_OUTPUT_OVERFLOW;
             if (status == SWC_OK && !fits) status = SWC_INTERNAL_NEEDS_SLOW;
-            a.consumed_bits[unit] = br.pos - sp.pos0;
+            a.consumed[unit] = br.pos - sp.pos0;
             a.out_len[unit] = em.op;
             a.status[unit] = status;
             a.rec_count[unit] = em.nrec;

@@ -140,7 +140,7 @@ done:
 #undef TRY
     if (status == SWC_OK && op > cap) status = SWC_ERR_OUTPUT_OVERFLOW;
     a.out_len[unit] = op;
-    a.consumed_bits[unit] = r.pos - skip;
+    a.consumed[unit] = r.pos - skip;
     a.status[unit] = status;
     a.rec_count[unit] = REC_DIRECT;      // the output is written: K2 leaves the unit alone
 }

@@ -494,7 +494,7 @@ inflate_warp_kernel(BatchArgs a) {
             if (status == SWC_OK && op > cap64) status = SWC_ERR_OUTPUT_OVERFLOW;
             // a unit of fewer than 8 literals may not fit its literals below its records (inflate.cuh)
             if (status == SWC_OK && (u64)nlit + 4ull * nrec > region_bytes(a.out_off[unit], cap64)) status = SWC_INTERNAL_NEEDS_SLOW;
-            a.consumed_bits[unit] = st.pos;
+            a.consumed[unit] = st.pos;
             a.out_len[unit] = op;
             a.status[unit] = status;
             a.rec_count[unit] = nrec;

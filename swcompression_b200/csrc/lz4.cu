@@ -83,10 +83,10 @@ __device__ __forceinline__ void lz4_block_body(const Args &a) {
 
     for (u64 b = 0; b < nb && status == SWC_OK; b++) {
         fail_blk = b;
-        const u64 blen_raw = a.blk_len[b0 + b];
+        const u64 blen_raw = a.in_len[b0 + b];
         const bool stored = (blen_raw >> 63) != 0;
         const u64 n = blen_raw & ~(1ull << 63);
-        const u8 *in = a.in_base + a.blk_off[b0 + b];
+        const u8 *in = a.in_base + a.in_off[b0 + b];
         if (stored) {                                                   // LZ4.swift:314-316
             if (op + n <= cap) warp_copy(out + op, in, n);
             op += n;
@@ -170,9 +170,9 @@ __device__ __forceinline__ u32 ext_bytes(u32 len_field_value /* length minus its
 __global__ void __launch_bounds__(128) lz4_parse_kernel(Args a, const u64 *rec_base_idx, u64 *recs, u32 *rec_count) {
     const u64 unit = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (unit >= a.n) return;
-    const u8 *in = a.in_base + a.blk_off[unit];
-    const u64 n = a.blk_len[unit] & ~(1ull << 63);
-    const bool stored = (a.blk_len[unit] >> 63) != 0;
+    const u8 *in = a.in_base + a.in_off[unit];
+    const u64 n = a.in_len[unit] & ~(1ull << 63);
+    const bool stored = (a.in_len[unit] >> 63) != 0;
     const u64 cap = a.out_cap[unit];
     u64 *rec = recs + rec_base_idx[unit];
     u32 nrec = 0;
@@ -251,7 +251,7 @@ __global__ void __launch_bounds__(256, 4) lz4_exec_kernel(Args a, const u64 *rec
     if (a.status[unit] != SWC_OK) return;
     const u32 lane = lane_id(), sub = lane >> 2, t = lane & 3;
     uint4 (*st)[32] = stage[(threadIdx.x >> 5) & 7];
-    const u8 *in = a.in_base + a.blk_off[unit];
+    const u8 *in = a.in_base + a.in_off[unit];
     u8 *out = a.out_base + a.out_off[unit];
     const u64 *rec = recs + rec_base_idx[unit];
     const u32 nrec = rec_count[unit];
@@ -366,7 +366,7 @@ int launch(const Args &a, cudaStream_t stream) {
         u32 *cnt = (u32 *)(base + a.n);
         u64 *recs = (u64 *)(((uintptr_t)(cnt + a.n) + 255) & ~(uintptr_t)255);
         timing_mark(stream);
-        lz4_rec_scan_kernel<<<1, 1024, 0, stream>>>(a.blk_len, a.n, base);
+        lz4_rec_scan_kernel<<<1, 1024, 0, stream>>>(a.in_len, a.n, base);
         lz4_parse_kernel<<<(unsigned)((a.n + 127) / 128), 128, 0, stream>>>(a, base, recs, cnt);
         timing_mark(stream);
         lz4_exec_kernel<<<(unsigned)((a.n * 32 + 255) / 256), 256, 0, stream>>>(a, base, recs, cnt);

@@ -5,17 +5,12 @@
 namespace swc {
 namespace lz4 {
 
-struct Args {
-    const u8 *in_base;
-    const u64 *blk_off, *blk_len;     // per block; bit 63 of blk_len = stored (uncompressed) block
+// in_off / in_len are indexed by block (bit 63 of in_len = stored, uncompressed block); the other columns and n by unit.
+// Unit u is block u unless first_blk / n_blk are set.
+struct Args : UnitIO {
     const u32 *first_blk, *n_blk;     // per unit chain, or both null: unit u = block u
     const u8 *dict;                   // prefix the first block of every unit may reference (may be null)
     u64 dict_len;
-    u8 *out_base;
-    const u64 *out_off, *out_cap;
-    u64 *out_len;
-    int32_t *status;
-    u64 n;                            // units
     void *scratch;                    // optional: two_phase_scratch_bytes(n, in_total) bytes enables the two-phase path
 };
 

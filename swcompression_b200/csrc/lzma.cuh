@@ -7,19 +7,12 @@ namespace lzma {
 
 enum { MODE_LZMA2 = 0, MODE_RAW = 1 };
 
-struct Args {
+struct Args : DecodeIO {
     int mode;
-    const u8 *in_base;
-    const u64 *in_off, *in_len;
     const u8 *dict_bytes;      // MODE_LZMA2: per-unit dictionary-size byte
     const u32 *props;          // MODE_RAW: lc | lp << 8 | pb << 16
     const i64 *dict_size;      // MODE_RAW
     const i64 *usize;          // MODE_RAW: < 0 = unknown (end marker required)
-    u8 *out_base;
-    const u64 *out_off, *out_cap;
-    u64 *out_len, *consumed;
-    int32_t *status;
-    u64 n;
     u16 *lit_scratch;          // optional: n x 4096 x 0x300 u16 for streams with lc+lp > 4 (else those units are refused)
 };
 
