@@ -279,6 +279,35 @@ int32_t swc_gzip_multi_unarchive_members(const uint8_t *in, size_t in_len,
 int32_t swc_gzip_multi_unarchive(const uint8_t *in, size_t in_len,
                                  uint8_t **out, size_t *out_len, size_t **member_ends, size_t *n_members);
 int32_t swc_zlib_unarchive(const uint8_t *in, size_t in_len, uint8_t **out, size_t *out_len);
+/* GzipArchive.unarchive(archive:) / ZlibArchive.unarchive(archive:) over n archives, device memory, asynchronous on
+ * `cuda_stream` (no host read, no synchronisation, and no allocation when the caller passes scratch).  Unit i is one
+ * archive in_base[in_off[i] ..+ in_len[i]) in the layout above; its first member is decoded and the bytes after it are
+ * ignored, as the reference does (multi-member archives: swc_gzip_multi_unarchive).  status[i] follows the reference's
+ * order of checks:
+ *   gzip: in_len < 20 -> wrongMagic; a header error; any Deflate status (SWC_ERR_OUTPUT_OVERFLOW with the size required in
+ *         out_len[i]); fewer than 8 bytes after the Deflate stream (after align()) -> wrongMagic; out_len mod 2^32 != ISIZE
+ *         -> wrongISize; a CRC-32 mismatch -> wrongCRC, with the data in the unit's output region;
+ *   zlib: a header error; any Deflate status; fewer than 4 bytes after the Deflate stream, or a big-endian Adler-32
+ *         mismatch -> wrongAdler32, with the data in the unit's output region.
+ * consumed_bytes[i] is how many bytes of the archive the reference read on OK and on the payload-carrying statuses (header
+ * + whole Deflate bytes + the 8-byte gzip / 4-byte zlib trailer, or no trailer for a zlib unit whose trailer is missing),
+ * and 0 on every other status.  A unit whose header fails reports out_len[i] = 0.
+ * headers (gzip, device, n entries, or NULL) receives each unit's swc_gzip_header as swc_gzip_header_parse fills it, its
+ * file name / comment / extra offsets relative to in_base (fields the header lacks stay 0); all zero when the header fails.
+ * scratch == NULL uses the library pool; a caller's scratch must hold swc_unarchive_batch_scratch_bytes(n,
+ * out_capacity_total) bytes, else the call returns SWC_ERR_INVALID_ARG. */
+size_t  swc_unarchive_batch_scratch_bytes(uint64_t n, uint64_t out_capacity_total);
+int32_t swc_gzip_unarchive_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                                 uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                 uint64_t out_capacity_total,
+                                 uint64_t *out_len, uint64_t *consumed_bytes, int32_t *status,
+                                 swc_gzip_header *headers /* device, n entries, or NULL */,
+                                 uint64_t n, void *scratch, size_t scratch_bytes, void *cuda_stream);
+int32_t swc_zlib_unarchive_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                                 uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                 uint64_t out_capacity_total,
+                                 uint64_t *out_len, uint64_t *consumed_bytes, int32_t *status,
+                                 uint64_t n, void *scratch, size_t scratch_bytes, void *cuda_stream);
 int32_t swc_xz_unarchive(const uint8_t *in, size_t in_len, uint8_t **out, size_t *out_len);
 int32_t swc_xz_split_unarchive(const uint8_t *in, size_t in_len,
                                uint8_t **out, size_t *out_len, size_t **stream_ends, size_t *n_streams);
@@ -317,11 +346,13 @@ int32_t swc_adler32(const uint8_t *in, size_t n, uint32_t *result);
 int32_t swc_xxh32(const uint8_t *in, size_t n, uint32_t *result);
 int32_t swc_sha256(const uint8_t *in, size_t n, uint8_t digest[32]);
 /* batched epilogues on DEVICE buffers (asynchronous on `cuda_stream`): one result per unit in_base[off[i] .. off[i]+len[i]).
- * `status` may be NULL; units whose status[i] != 0 are not read (their result is 0). */
+ * `status` may be NULL; units whose status[i] != 0 are not read (their result is 0, for Adler-32 too). */
 int32_t swc_crc32_batch(const uint8_t *in_base, const uint64_t *off, const uint64_t *len, const int32_t *status,
                         uint32_t *result, uint64_t n, void *cuda_stream);
 int32_t swc_xxh32_batch(const uint8_t *in_base, const uint64_t *off, const uint64_t *len,
                         uint32_t *result, uint64_t n, void *cuda_stream);
+int32_t swc_adler32_batch(const uint8_t *in_base, const uint64_t *off, const uint64_t *len, const int32_t *status,
+                          uint32_t *result, uint64_t n, void *cuda_stream);
 
 #ifdef __cplusplus
 }

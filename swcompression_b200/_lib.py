@@ -94,6 +94,11 @@ def lib():
         L.swc_zip_open.argtypes = [vp, sz, C.POINTER(vp), szp, C.POINTER(vp), szp]
         L.swc_zip_info.argtypes = [vp, sz, C.POINTER(vp), szp]
         L.swc_xxh32_batch.argtypes = [vp, vp, vp, vp, u64, vp]
+        L.swc_adler32_batch.argtypes = [vp, vp, vp, vp, vp, u64, vp]
+        L.swc_unarchive_batch_scratch_bytes.restype = C.c_size_t
+        L.swc_unarchive_batch_scratch_bytes.argtypes = [C.c_uint64, C.c_uint64]
+        L.swc_gzip_unarchive_batch.argtypes = [vp, vp, vp, vp, vp, vp, u64, vp, vp, vp, vp, u64, vp, sz, vp]
+        L.swc_zlib_unarchive_batch.argtypes = [vp, vp, vp, vp, vp, vp, u64, vp, vp, vp, u64, vp, sz, vp]
         L.swc_zlib_unarchive.argtypes = [vp, sz, C.POINTER(vp), szp]
         L.swc_xz_unarchive.argtypes = [vp, sz, C.POINTER(vp), szp]
         L.swc_xz_split_unarchive.argtypes = [vp, sz, C.POINTER(vp), szp, C.POINTER(vp), szp]

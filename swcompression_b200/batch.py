@@ -53,8 +53,12 @@ def pack_units(units, align=16):
 
 
 class Batch:
-    """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'lzma2', 'lz4_block_compress',
-    'deflate_compress').
+    """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'lzma2', 'gzip', 'zlib', 'lz4_block_compress',
+    'deflate_compress', 'bzip2_compress').
+
+    'gzip' / 'zlib' decode one archive per unit (GzipArchive.unarchive, GzipArchive.swift:38-47, 79-100 / ZlibArchive.unarchive,
+    ZlibArchive.swift:25-42): the first member only, whose status, size and consumed bytes results() returns.  With
+    `headers=True` a 'gzip' batch also fills a device array of swc_gzip_header, which gzip_headers() reads back.
 
     'lz4_block_compress' compresses each unit into a raw LZ4 block (LZ4+Compress.swift:156-277); `aux` is then an optional
     (dict_off, dict_len) pair of u64 arrays placing each unit's dictionary window inside `in_buf`.
@@ -67,7 +71,8 @@ class Batch:
     to COMPRESS_SCRATCH_LIMIT; `scratch_bytes` caps it lower (the library then runs the batch in slices; a scratch that
     cannot hold the largest unit fails the run with SWC_ERR_INVALID_ARG)."""
 
-    def __init__(self, codec, in_buf, in_off, in_len, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=1):
+    def __init__(self, codec, in_buf, in_off, in_len, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=1,
+                 headers=False):
         self.codec = codec
         self.device = torch.device(device)
         self.n = len(in_off)
@@ -105,11 +110,18 @@ class Batch:
         if codec == "deflate":
             nbytes = _lib.lib().swc_deflate_batch_scratch_bytes(self.n, self.out_total)
             self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        if codec in ("gzip", "zlib"):
+            nbytes = _lib.lib().swc_unarchive_batch_scratch_bytes(self.n, self.out_total)
+            self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        self.d_headers = None
+        if headers and codec == "gzip":
+            from .api import _CGzipHeader
+            self.d_headers = torch.zeros(max(self.n, 1) * C.sizeof(_CGzipHeader), dtype=torch.uint8, device=self.device)
 
     @classmethod
-    def from_units(cls, codec, units, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=1):
+    def from_units(cls, codec, units, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=1, headers=False):
         buf, offs, lens = pack_units(units)
-        return cls(codec, buf, offs, lens, out_cap, device, aux, scratch_bytes, block_size)
+        return cls(codec, buf, offs, lens, out_cap, device, aux, scratch_bytes, block_size, headers)
 
     def run(self):
         L = _lib.lib()
@@ -120,6 +132,15 @@ class Batch:
                                                 p(self.d_out_off), p(self.d_out_cap), self.out_total, p(self.d_out_len),
                                                 p(self.d_consumed), p(self.d_status), self.n, p(self.d_scratch),
                                                 self.d_scratch.numel(), stream)
+        elif self.codec == "gzip":
+            st = L.swc_gzip_unarchive_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out), p(self.d_out_off),
+                                            p(self.d_out_cap), self.out_total, p(self.d_out_len), p(self.d_consumed),
+                                            p(self.d_status), None if self.d_headers is None else p(self.d_headers), self.n,
+                                            p(self.d_scratch), self.d_scratch.numel(), stream)
+        elif self.codec == "zlib":
+            st = L.swc_zlib_unarchive_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out), p(self.d_out_off),
+                                            p(self.d_out_cap), self.out_total, p(self.d_out_len), p(self.d_consumed),
+                                            p(self.d_status), self.n, p(self.d_scratch), self.d_scratch.numel(), stream)
         elif self.codec == "lz4_block":
             st = L.swc_lz4_block_decompress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), None, 0, p(self.d_out),
                                                   p(self.d_out_off), p(self.d_out_cap), p(self.d_out_len), p(self.d_status),
@@ -150,9 +171,19 @@ class Batch:
             raise RuntimeError(f"{self.codec} batch launch failed: {_lib.status_name(st)} {_lib.last_error()}")
 
     def results(self):
-        """-> (status int32[n], out_len int64[n], consumed int64[n]) on the host (synchronises)."""
+        """-> (status int32[n], out_len int64[n], consumed int64[n]) on the host (synchronises).  consumed is in bits for
+        'deflate' and 'bzip2', in bytes for 'lzma2', 'gzip' and 'zlib'."""
         torch.cuda.synchronize(self.device)
         return self.d_status.cpu().numpy(), self.d_out_len.cpu().numpy(), self.d_consumed.cpu().numpy()
+
+    def gzip_headers(self):
+        """-> the swc_gzip_header of every unit of a 'gzip' batch made with headers=True (synchronises); offsets are
+        relative to the batch's input buffer"""
+        from .api import _CGzipHeader
+        torch.cuda.synchronize(self.device)
+        raw = self.d_headers.cpu().numpy().tobytes()
+        size = C.sizeof(_CGzipHeader)
+        return [_CGzipHeader.from_buffer_copy(raw, i * size) for i in range(self.n)]
 
     def output(self, i):
         st, ln, _ = self.results()

@@ -1,7 +1,7 @@
 // api_wrappers.cu — GzipArchive / ZlibArchive framing around the device Deflate decoder, and the checksum C ABI.
 // Reference: Sources/GZip/GzipArchive.swift:38-100, GzipHeader.swift:68-199, Sources/Zlib/ZlibArchive.swift:25-42,
-// ZlibHeader.swift:47-93.  Headers/trailers (tens of bytes) are parsed on the host; Deflate and CRC-32 / Adler-32 over
-// the payload run on the device.
+// ZlibHeader.swift:47-93.  Headers/trailers (tens of bytes) are parsed on the host with the grammar of archive_header.cuh;
+// Deflate and CRC-32 / Adler-32 over the payload run on the device.  The batched form is unarchive_batch.cu.
 #include <algorithm>
 #include <chrono>
 #include <cstdio>
@@ -10,108 +10,18 @@
 #include <vector>
 #include "../../include/swcgpu.h"
 #include "host_util.h"
+#include "archive_header.cuh"
 #include "checks.cuh"
 
 using namespace swc;
 
 namespace {
 
-// GzipHeader.init(_: LsbBitReader), GzipHeader.swift:68-199 — one pass over the member's header that both validates it and
-// records where its fields are.  Written against the Swift source (guards in source order, one `Cursor` read per
-// `reader.byte()`); `left()` is `reader.bytesLeft`.  Reads the reference performs WITHOUT a guard trap there (BitByteData
-// precondition): they report SWC_ERR_REFERENCE_TRAP here.
-struct Cursor {
-    const uint8_t *base; size_t n, at;
-    size_t left() const { return n - at; }
-    bool finished() const { return at >= n; }
-};
-
-int gzip_parse(const uint8_t *in, size_t n, size_t member_off, swc_gzip_header *h) {
-    if (member_off > n) return SWC_GZIP_WRONG_MAGIC;
-    Cursor c{in, n, member_off};
-    swc_gzip_header out;
-    memset(&out, 0, sizeof(out));
-    if (c.left() < 10) return SWC_GZIP_WRONG_MAGIC;                                  // :70-71
-    if (in[c.at] != 0x1f || in[c.at + 1] != 0x8b) return SWC_GZIP_WRONG_MAGIC;       // :74-76 (uint16 == 0x8b1f)
-    if (in[c.at + 2] != 8) return SWC_GZIP_WRONG_COMPRESSION_METHOD;                 // :80-82
-    out.compression_method = 8;
-    const unsigned flg = in[c.at + 3];
-    if ((flg & 0xE0) != 0) return SWC_GZIP_WRONG_FLAGS;                              // :86-88
-    out.modification_time = (uint32_t)in[c.at + 4] | (uint32_t)in[c.at + 5] << 8 | (uint32_t)in[c.at + 6] << 16 | (uint32_t)in[c.at + 7] << 24;
-    out.os_type = in[c.at + 9];                                                      // :103-105 (XFL at +8 is only hashed)
-    out.is_text_file = (flg & 0x01) != 0;                                            // :107
-    c.at += 10;
-    if (flg & 0x04) {                                                                // FEXTRA :111-155
-        if (c.left() < 2) return SWC_GZIP_WRONG_MAGIC;                               // :112-113
-        size_t xlen = (size_t)in[c.at] | (size_t)in[c.at + 1] << 8;
-        c.at += 2;
-        if (!(c.left() >= xlen && xlen >= 4)) return SWC_GZIP_WRONG_MAGIC;           // :123-124
-        out.extra_off = c.at; out.extra_len = xlen;
-        long remaining = (long)xlen;                                                 // the reference's signed `xlen` countdown
-        while (remaining > 0) {                                                      // :125
-            // si1, si2, two length bytes: four unguarded reader.byte() calls (:126-140)
-            if (c.left() < 2) return SWC_ERR_REFERENCE_TRAP;
-            if (in[c.at + 1] == 0) return SWC_GZIP_WRONG_FLAGS;                      // :131-132 (checked before the length is read)
-            if (c.left() < 4) return SWC_ERR_REFERENCE_TRAP;
-            const long len = (long)in[c.at + 2] | (long)in[c.at + 3] << 8;
-            c.at += 4;
-            remaining -= 4;                                                          // :141
-            if (remaining < len) return SWC_GZIP_WRONG_MAGIC;                        // :145-146
-            if ((long)c.left() < len) return SWC_ERR_REFERENCE_TRAP;                 // :148-152 unguarded payload reads
-            c.at += (size_t)len;
-            remaining -= len;                                                        // :154
-        }
-    }
-    if (flg & 0x08) {                                                                // FNAME :159-172
-        out.has_file_name = 1; out.file_name_off = c.at;
-        for (;;) {
-            if (c.finished()) return SWC_GZIP_WRONG_MAGIC;                           // :162-163
-            if (in[c.at++] == 0) break;
-        }
-        out.file_name_len = c.at - 1 - out.file_name_off;
-    }
-    if (flg & 0x10) {                                                                // FCOMMENT :177-190
-        out.has_comment = 1; out.comment_off = c.at;
-        for (;;) {
-            if (c.finished()) return SWC_GZIP_WRONG_MAGIC;                           // :180-181
-            if (in[c.at++] == 0) break;
-        }
-        out.comment_len = c.at - 1 - out.comment_off;
-    }
-    if (flg & 0x02) {                                                                // FHCRC :194-200
-        if (c.left() < 2) return SWC_GZIP_WRONG_MAGIC;
-        const unsigned stored = (unsigned)in[c.at] | (unsigned)in[c.at + 1] << 8;
-        if ((crc32_framing(in + member_off, c.at - member_off) & 0xFFFFu) != stored) return SWC_GZIP_WRONG_HEADER_CRC;
-        c.at += 2;
-    }
-    out.header_len = c.at - member_off;
-    if (h) *h = out;
-    return SWC_OK;
-}
-
 int gzip_header(const uint8_t *in, size_t n, size_t *off) {
     swc_gzip_header h;
     const int st = gzip_parse(in, n, *off, &h);
     if (st == SWC_OK) *off += h.header_len;
     return st;
-}
-
-// ZlibHeader.init(_: LsbBitReader), ZlibHeader.swift:47-93
-int zlib_parse(const uint8_t *in, size_t n, swc_zlib_header *h) {
-    if (n < 2) return SWC_ZLIB_WRONG_COMPRESSION_METHOD;                             // :49-50
-    const unsigned cmf = in[0], flg = in[1];
-    if ((cmf & 0xF) != 8) return SWC_ZLIB_WRONG_COMPRESSION_METHOD;                  // :56-58
-    const unsigned cinfo = (cmf & 0xF0) >> 4;
-    if (cinfo > 7) return SWC_ZLIB_WRONG_COMPRESSION_INFO;                           // :62-64
-    // CompressionLevel(rawValue: (flags & 0xC0) >> 6) covers 0...3: it cannot fail (:80-82)
-    if ((((unsigned)cmf << 8) + flg) % 31 != 0) return SWC_ZLIB_WRONG_FCHECK;        // :84-85 (Swift precedence: (cmf << 8) + flags)
-    size_t len = 2;
-    if ((flg & 0x20) != 0) {                                                         // FDICT: four bytes are skipped (:88-92)
-        if (n - 2 < 4) return SWC_ZLIB_WRONG_FCHECK;
-        len = 6;
-    }
-    if (h) { h->compression_method = 8; h->compression_level = (int32_t)((flg & 0xC0) >> 6); h->window_size = 1 << (cinfo + 8); h->header_len = len; }
-    return SWC_OK;
 }
 
 // processMember GzipArchive.swift:79-100; d_in holds the whole archive on the device
@@ -381,6 +291,13 @@ int32_t swc_crc32_batch(const uint8_t *in_base, const uint64_t *off, const uint6
     if (!in_base || !off || !len || !result) return SWC_ERR_INVALID_ARG;
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     return checks::crc32_units(in_base, off, len, status, result, n, (cudaStream_t)cuda_stream);
+}
+int32_t swc_adler32_batch(const uint8_t *in_base, const uint64_t *off, const uint64_t *len, const int32_t *status,
+                          uint32_t *result, uint64_t n, void *cuda_stream) {
+    if (n == 0) return SWC_OK;
+    if (!in_base || !off || !len || !result) return SWC_ERR_INVALID_ARG;
+    if (ensure_device()) return SWC_ERR_NO_DEVICE;
+    return checks::adler32_units(in_base, off, len, status, result, n, (cudaStream_t)cuda_stream);
 }
 int32_t swc_xxh32_batch(const uint8_t *in_base, const uint64_t *off, const uint64_t *len,
                         uint32_t *result, uint64_t n, void *cuda_stream) {

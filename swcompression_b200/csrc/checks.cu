@@ -201,6 +201,54 @@ int crc32_units(const u8 *base, const u64 *off, const u64 *len, const int32_t *s
     return SWC_OK;
 }
 
+// ---------------------------------------------------------------- Adler-32 of many buffers: one warp per buffer
+// The same 32 segments as crc32_units_kernel.  A lane sums its segment from a = b = 0 (s1 = sum of bytes, s2 = sum of
+// (bytes left including this one) x byte), 16 bytes per step with byte dot products, in 64-bit sums reduced mod 65 521
+// every 4 KiB; the lanes are then chained with the concatenation rule a' = a + s1, b' = b + len x a + s2 (CheckSums.swift:
+// 48-57 over the whole buffer gives the same value).  64-bit sums cannot overflow for any byte values between reductions.
+constexpr u32 ADLER_MOD = 65521;
+__global__ void __launch_bounds__(256) adler32_units_kernel(const u8 *base, const u64 *off, const u64 *len, const int32_t *status, u32 *result, u64 n) {
+    const u64 unit = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (unit >= n) return;
+    const u32 lane = threadIdx.x & 31;
+    const bool skip = status && status[unit] != SWC_OK;
+    const u8 *p = base + off[unit];
+    const u64 L = skip ? 0 : len[unit];
+    const u64 seg = (((L + 31) / 32) + 15) & ~(u64)15;
+    const u64 sb = lane * seg < L ? lane * seg : L, se = sb + seg < L ? sb + seg : L;
+    u64 s1 = 0, s2 = 0;
+    u64 i = sb;
+    for (; i < se && ((uintptr_t)(p + i) & 15); i++) { s1 += p[i]; s2 += s1; }
+    u32 steps = 0;
+    for (; i + 16 <= se; i += 16) {
+        const uint4 v = __ldg((const uint4 *)(p + i));
+        // byte j of the 16 weighs 16 - j in s2
+        const u32 sum = __dp4a(v.x, 0x01010101u, __dp4a(v.y, 0x01010101u, __dp4a(v.z, 0x01010101u, __dp4a(v.w, 0x01010101u, 0u))));
+        const u32 wsum = __dp4a(v.x, 0x0D0E0F10u, __dp4a(v.y, 0x090A0B0Cu, __dp4a(v.z, 0x05060708u, __dp4a(v.w, 0x01020304u, 0u))));
+        s2 += 16 * s1 + wsum;
+        s1 += sum;
+        if (++steps == 256) { s1 %= ADLER_MOD; s2 %= ADLER_MOD; steps = 0; }
+    }
+    for (; i < se; i++) { s1 += p[i]; s2 += s1; }
+    s1 %= ADLER_MOD; s2 %= ADLER_MOD;
+    u64 a = 1, b = 0;
+    for (int l = 0; l < 32; l++) {
+        const u64 p1 = __shfl_sync(SWC_FULL, s1, l), p2 = __shfl_sync(SWC_FULL, s2, l);
+        const u64 lb = (u64)l * seg < L ? (u64)l * seg : L, le = lb + seg < L ? lb + seg : L;
+        b = (b + ((le - lb) % ADLER_MOD) * a + p2) % ADLER_MOD;
+        a = (a + p1) % ADLER_MOD;
+    }
+    if (lane == 0) result[unit] = skip ? 0u : (u32)((b << 16) | a);
+}
+
+int adler32_units(const u8 *base, const u64 *off, const u64 *len, const int32_t *status, u32 *result, u64 n, cudaStream_t s) {
+    if (!n) return SWC_OK;
+    adler32_units_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, s>>>(base, off, len, status, result, n);
+    count_launch();
+    SWC_CUDA_TRY(cudaGetLastError());
+    return SWC_OK;
+}
+
 // gzip member signature scan (GzipHeader.swift:70-81: magic 1f 8b, method 8, reserved flag bits clear); positions are
 // appended in any order and sorted by the host wrapper
 __global__ void __launch_bounds__(256) gzip_scan_kernel(const u8 *d, u64 n, u64 *list, unsigned long long *count, u64 cap) {

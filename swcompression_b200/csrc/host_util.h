@@ -6,6 +6,7 @@
 #include <stdlib.h>
 #include <vector>
 #include "common.cuh"
+#include "archive_header.cuh"   // crc32_framing
 
 #include <mutex>
 
@@ -243,14 +244,5 @@ int copy_back_regions(uint8_t *out_base, const u8 *d_out, const uint64_t *out_of
 // ---- container framing (a few bytes per header / block mark) read on the host ----
 inline uint32_t le32(const uint8_t *p) { return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24; }
 inline void put_le32(uint8_t *p, uint32_t v) { for (int k = 0; k < 4; k++) p[k] = (uint8_t)(v >> (8 * k)); }
-// bitwise CRC-32 of header / index / footer fields; payload CRCs run on the device
-inline uint32_t crc32_framing(const uint8_t *p, size_t n) {
-    uint32_t c = 0xFFFFFFFFu;
-    for (size_t i = 0; i < n; i++) {
-        c ^= p[i];
-        for (int k = 0; k < 8; k++) c = (c & 1) ? 0xEDB88320u ^ (c >> 1) : c >> 1;
-    }
-    return ~c;
-}
 
 }  // namespace swc
