@@ -309,6 +309,29 @@ int32_t swc_zlib_unarchive_batch(const uint8_t *in_base, const uint64_t *in_off,
                                  uint64_t *out_len, uint64_t *consumed_bytes, int32_t *status,
                                  uint64_t n, void *scratch, size_t scratch_bytes, void *cuda_stream);
 int32_t swc_xz_unarchive(const uint8_t *in, size_t in_len, uint8_t **out, size_t *out_len);
+/* XZArchive.unarchive(archive:) over n whole .xz files, device memory, asynchronous on `cuda_stream`: one launch, no host
+ * read, no allocation, no synchronisation and no scratch, so the call can be captured in a CUDA graph.  Unit i is the file
+ * in_base[in_off[i] ..+ in_len[i]) in the layout above; every stream (with its stream padding) and every block is decoded and
+ * the outputs are concatenated in out_base[out_off[i] ..+ out_cap[i]).  Nothing is written outside the output range, and no
+ * byte outside the input range affects a result: the container walk reads byte by byte inside it, while the LZMA2 decoder,
+ * like swc_lzma2_decompress_batch, loads the 4-byte words of the 128-byte-aligned lines that hold the unit's bytes and
+ * discards the bytes of those words that lie outside it.  status[i] is what swc_xz_unarchive returns for the same bytes, in the reference's order of checks (a read past
+ * in_len[i] is SWC_ERR_REFERENCE_TRAP where the single call reports it).  out_len[i] is:
+ *   SWC_OK                   the decoded size;
+ *   SWC_XZ_WRONG_CHECK       the data up to and including the failing block, which is in the unit's output region;
+ *   SWC_ERR_OUTPUT_OVERFLOW  (the unit would write past out_cap[i] before any other status arises) the size the archive
+ *                            declares: the sum of its indexes' uncompressed sizes, read backwards from the end of the unit
+ *                            through footers, indexes and stream padding, when that walk reaches byte 0; else 0;
+ *   any other status         0.
+ * Two deviations (DESIGN §6), each reported where the reference would start running the block's filter chain, so every
+ * earlier error still wins: a chain other than zero to three Delta filters followed by one LZMA2 filter, and an LZMA chunk
+ * with lc + lp > 4, report SWC_ERR_UNSUPPORTED.  swc_xz_unarchive decodes both. */
+int32_t swc_xz_unarchive_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                               uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                               uint64_t *out_len, int32_t *status, uint64_t n, void *cuda_stream);
+/* resident warps per SM of the LZMA / LZMA2 batch kernel and of the XZ batch kernel on the current device (either pointer
+ * may be NULL) */
+int32_t swc_xz_occupancy(int32_t *lzma_warps_per_sm, int32_t *xz_warps_per_sm);
 int32_t swc_xz_split_unarchive(const uint8_t *in, size_t in_len,
                                uint8_t **out, size_t *out_len, size_t **stream_ends, size_t *n_streams);
 
@@ -353,6 +376,8 @@ int32_t swc_xxh32_batch(const uint8_t *in_base, const uint64_t *off, const uint6
                         uint32_t *result, uint64_t n, void *cuda_stream);
 int32_t swc_adler32_batch(const uint8_t *in_base, const uint64_t *off, const uint64_t *len, const int32_t *status,
                           uint32_t *result, uint64_t n, void *cuda_stream);
+int32_t swc_crc64_batch(const uint8_t *in_base, const uint64_t *off, const uint64_t *len, const int32_t *status,
+                        uint64_t *result, uint64_t n, void *cuda_stream);
 
 #ifdef __cplusplus
 }

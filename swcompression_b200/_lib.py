@@ -101,6 +101,9 @@ def lib():
         L.swc_zlib_unarchive_batch.argtypes = [vp, vp, vp, vp, vp, vp, u64, vp, vp, vp, u64, vp, sz, vp]
         L.swc_zlib_unarchive.argtypes = [vp, sz, C.POINTER(vp), szp]
         L.swc_xz_unarchive.argtypes = [vp, sz, C.POINTER(vp), szp]
+        L.swc_xz_unarchive_batch.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, u64, vp]
+        L.swc_xz_occupancy.argtypes = [vp, vp]
+        L.swc_crc64_batch.argtypes = [vp, vp, vp, vp, vp, u64, vp]
         L.swc_xz_split_unarchive.argtypes = [vp, sz, C.POINTER(vp), szp, C.POINTER(vp), szp]
         for name in ("swc_crc32", "swc_bzip2_crc32", "swc_adler32", "swc_xxh32", "swc_crc64", "swc_sha256"):
             getattr(L, name).argtypes = [vp, sz, vp]

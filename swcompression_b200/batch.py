@@ -53,12 +53,14 @@ def pack_units(units, align=16):
 
 
 class Batch:
-    """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'lzma2', 'gzip', 'zlib', 'lz4_block_compress',
-    'deflate_compress', 'bzip2_compress').
+    """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'lzma2', 'gzip', 'zlib', 'xz',
+    'lz4_block_compress', 'deflate_compress', 'bzip2_compress').
 
     'gzip' / 'zlib' decode one archive per unit (GzipArchive.unarchive, GzipArchive.swift:38-47, 79-100 / ZlibArchive.unarchive,
     ZlibArchive.swift:25-42): the first member only, whose status, size and consumed bytes results() returns.  With
     `headers=True` a 'gzip' batch also fills a device array of swc_gzip_header, which gzip_headers() reads back.
+    'xz' decodes one whole .xz file per unit (XZArchive.unarchive, XZArchive.swift:27-50): every stream and block, the outputs
+    concatenated.  It takes no scratch and no aux, and reports no consumed bytes (results() gives zeros in that column).
 
     'lz4_block_compress' compresses each unit into a raw LZ4 block (LZ4+Compress.swift:156-277); `aux` is then an optional
     (dict_off, dict_len) pair of u64 arrays placing each unit's dictionary window inside `in_buf`.
@@ -141,6 +143,9 @@ class Batch:
             st = L.swc_zlib_unarchive_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out), p(self.d_out_off),
                                             p(self.d_out_cap), self.out_total, p(self.d_out_len), p(self.d_consumed),
                                             p(self.d_status), self.n, p(self.d_scratch), self.d_scratch.numel(), stream)
+        elif self.codec == "xz":
+            st = L.swc_xz_unarchive_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out), p(self.d_out_off),
+                                          p(self.d_out_cap), p(self.d_out_len), p(self.d_status), self.n, stream)
         elif self.codec == "lz4_block":
             st = L.swc_lz4_block_decompress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), None, 0, p(self.d_out),
                                                   p(self.d_out_off), p(self.d_out_cap), p(self.d_out_len), p(self.d_status),
@@ -172,7 +177,7 @@ class Batch:
 
     def results(self):
         """-> (status int32[n], out_len int64[n], consumed int64[n]) on the host (synchronises).  consumed is in bits for
-        'deflate' and 'bzip2', in bytes for 'lzma2', 'gzip' and 'zlib'."""
+        'deflate' and 'bzip2', in bytes for 'lzma2', 'gzip' and 'zlib', and 0 for 'xz'."""
         torch.cuda.synchronize(self.device)
         return self.d_status.cpu().numpy(), self.d_out_len.cpu().numpy(), self.d_consumed.cpu().numpy()
 

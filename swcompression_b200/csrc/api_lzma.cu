@@ -11,6 +11,7 @@
 #include "host_util.h"
 #include "lzma.cuh"
 #include "checks.cuh"
+#include "xz_framing.cuh"
 
 using namespace swc;
 
@@ -49,29 +50,8 @@ __global__ void delta_kernel(const u8 *in, u8 *out, u64 n, u32 distance) {
     for (u64 i = j; i < n; i += distance) { acc = (u8)(acc + in[i]); out[i] = acc; }
 }
 
-// ---- XZ framing ----
-struct Rd {
-    const uint8_t *p; size_t n, off;
-    bool need(size_t k) const { return n - off >= k; }
-};
-int multibyte(Rd &r, int64_t *val) {                          // LittleEndianByteReader+XZ.swift:10-30
-    if (!r.need(1)) return SWC_ERR_REFERENCE_TRAP;
-    int i = 1;
-    int64_t result = r.p[r.off++];
-    if (result <= 127) { *val = result; return SWC_OK; }
-    result &= 0x7F;
-    for (;;) {
-        if (!r.need(1)) return SWC_ERR_REFERENCE_TRAP;
-        unsigned b = r.p[r.off++];
-        if (i >= 9 || b == 0) return SWC_XZ_MULTI_BYTE_INTEGER_ERROR;
-        result += (int64_t)(b & 0x7F) << (7 * i);
-        i++;
-        if ((b & 0x80) == 0) break;
-    }
-    *val = result;
-    return SWC_OK;
-}
-int check_size(int t) { return t == 0 ? 0 : t == 1 ? 4 : t == 4 ? 8 : 32; }
+// ---- XZ framing: xz_framing.cuh ----
+using xz::Rd;
 
 // ---- speculative batch decode of every LZMA2 block of a (multi-stream / multi-block) .xz file ------------------------
 // XZArchive walks streams and blocks strictly in order, but the stream footers + indexes at the END of each stream
@@ -88,43 +68,12 @@ thread_local Prefetch *g_prefetch = nullptr;
 
 // XZBlock.init XZBlock.swift:18-97. Block data ends up in `blk` (device) with length blk_len.
 int xz_block(Rd &r, const u8 *d_in, unsigned hsize_byte, int csize, DevBuf &blk, size_t &blk_len, int64_t *unpadded) {
-    const size_t hstart = r.off - 1;
-    const size_t real = ((size_t)hsize_byte + 1) * 4;
-    if (!r.need(1)) return SWC_ERR_REFERENCE_TRAP;
-    const unsigned flags = r.p[r.off++];
-    const int nfilters = (flags & 0x03) + 1;
-    if (flags & 0x3C) return SWC_XZ_WRONG_FIELD;
-    int64_t comp_size = -1, uncomp_size = -1;
-    int st;
-    if (flags & 0x40) { if ((st = multibyte(r, &comp_size))) return st; }
-    if (flags & 0x80) { if ((st = multibyte(r, &uncomp_size))) return st; }
-    int kinds[4], params[4];
-    for (int f = 0; f < nfilters; f++) {
-        int64_t id, psz;
-        if ((st = multibyte(r, &id))) return st;
-        if ((uint64_t)id >= 0x4000000000000000ull) return SWC_XZ_WRONG_FILTER_ID;
-        if (id == 0x21) {
-            if ((st = multibyte(r, &psz))) return st;
-            if (psz != 1) return SWC_LZMA2_WRONG_DICTIONARY_SIZE;
-            if (!r.need(1)) return SWC_ERR_REFERENCE_TRAP;
-            kinds[f] = 0x21; params[f] = r.p[r.off++];
-        } else if (id == 0x03) {
-            if ((st = multibyte(r, &psz))) return st;
-            if (psz != 1) return SWC_XZ_WRONG_FIELD;
-            if (!r.need(1)) return SWC_ERR_REFERENCE_TRAP;
-            kinds[f] = 0x03; params[f] = (r.p[r.off++] + 1) & 0xFF;
-        } else return SWC_XZ_WRONG_FILTER_ID;
-    }
-    while ((int64_t)(r.off - hstart) < (int64_t)real - 4) {
-        if (!r.need(1)) return SWC_ERR_REFERENCE_TRAP;
-        if (r.p[r.off++] != 0) return SWC_XZ_WRONG_PADDING;
-    }
-    if (!r.need(4)) return SWC_ERR_REFERENCE_TRAP;
-    const uint32_t hcrc = le32(r.p + r.off);
-    if (r.n - hstart < real - 4) return SWC_ERR_REFERENCE_TRAP;
-    if (crc32_framing(r.p + hstart, real - 4) != hcrc) return SWC_XZ_WRONG_INFO_CRC;
-    r.off = hstart + real;
-
+    xz::BlockHeader h;
+    int st = xz::block_header(r, hsize_byte, h);
+    if (st) return st;
+    const int nfilters = h.nfilters;
+    const int64_t uncomp_size = h.uncomp_size;
+    const int *kinds = h.kind, *params = h.param;
     const size_t data_start = r.off;
     // filters.reversed().reduce(byteReader): the LAST filter reads the archive, earlier ones read its output
     DevBuf cur; size_t cur_len = 0; bool have_cur = false;
@@ -155,7 +104,7 @@ int xz_block(Rd &r, const u8 *d_in, unsigned hsize_byte, int csize, DevBuf &blk,
         } else {
             const size_t n = src_n - src_start;
             if ((st = next.alloc(n + 16))) return st;
-            if (n) { delta_kernel<<<1, 256, 0, 0>>>(src + src_start, next.as<u8>(), n, (u32)(params[f] == 0 ? 256 : params[f])); count_launch(); }
+            if (n) { delta_kernel<<<1, 256, 0, 0>>>(src + src_start, next.as<u8>(), n, (u32)params[f]); count_launch(); }
             SWC_CUDA_TRY(cudaGetLastError());
             if (!have_cur) r.off += n;
             next_len = n;
@@ -163,16 +112,7 @@ int xz_block(Rd &r, const u8 *d_in, unsigned hsize_byte, int csize, DevBuf &blk,
         cur.take(next);
         cur_len = next_len; have_cur = true;
     }
-    if (!((comp_size < 0 || comp_size == (int64_t)(r.off - data_start)) && (uncomp_size < 0 || uncomp_size == (int64_t)cur_len)))
-        return SWC_XZ_WRONG_DATA_SIZE;
-    const int64_t unp = (int64_t)(r.off - hstart);
-    if (unp % 4 != 0) {
-        for (int i = 0, pad = 4 - (int)(unp % 4); i < pad; i++) {
-            if (!r.need(1)) return SWC_ERR_REFERENCE_TRAP;
-            if (r.p[r.off++] != 0) return SWC_XZ_WRONG_PADDING;
-        }
-    }
-    *unpadded = unp + csize;
+    if ((st = xz::block_tail(r, h, data_start, (int64_t)cur_len, csize, unpadded))) return st;
     blk.take(cur);
     blk_len = cur_len;
     return SWC_OK;
@@ -180,15 +120,9 @@ int xz_block(Rd &r, const u8 *d_in, unsigned hsize_byte, int csize, DevBuf &blk,
 
 // processStream XZArchive.swift:90-130 (+ processIndex, processFooter); stream data is appended to `out` (host)
 int xz_stream(Rd &r, const u8 *d_in, HostOut &out, bool *check_error) {
-    static const uint8_t magic[6] = {0xFD, 0x37, 0x7A, 0x58, 0x5A, 0x00};
-    if (!r.need(12)) return SWC_ERR_REFERENCE_TRAP;
-    if (memcmp(r.p + r.off, magic, 6) != 0) return SWC_XZ_WRONG_MAGIC;
-    const uint8_t *fl = r.p + r.off + 6;
-    if (crc32_framing(fl, 2) != le32(r.p + r.off + 8)) return SWC_XZ_WRONG_INFO_CRC;
-    if (!(fl[0] == 0 && (fl[1] & 0xF0) == 0)) return SWC_XZ_WRONG_FIELD;
-    const int ctype = fl[1] & 0xF;
-    if (!(ctype == 0 || ctype == 1 || ctype == 4 || ctype == 0x0A)) return SWC_XZ_WRONG_FIELD;
-    r.off += 12;
+    int ctype = 0;
+    int st = xz::stream_header(r, &ctype);
+    if (st) return st;
     std::vector<std::pair<int64_t, int64_t>> infos;
     int64_t index_size = -1;
     *check_error = false;
@@ -196,118 +130,56 @@ int xz_stream(Rd &r, const u8 *d_in, HostOut &out, bool *check_error) {
         if (!r.need(1)) return SWC_ERR_REFERENCE_TRAP;
         const unsigned hs = r.p[r.off++];
         if (hs == 0) {                                               // processIndex
-            const size_t istart = r.off - 1;
-            int64_t v; int st;
-            if ((st = multibyte(r, &v))) return st;
-            if (v != (int64_t)infos.size()) return SWC_XZ_WRONG_FIELD;
-            for (auto &bi : infos) {
-                if ((st = multibyte(r, &v))) return st;
-                if (v != bi.first) return SWC_XZ_WRONG_FIELD;
-                if ((st = multibyte(r, &v))) return st;
-                if (v != bi.second) return SWC_XZ_WRONG_DATA_SIZE;
-            }
-            int64_t isz = (int64_t)(r.off - istart);
-            if (isz % 4 != 0) {
-                for (int i = 0, pad = 4 - (int)(isz % 4); i < pad; i++) {
-                    if (!r.need(1)) return SWC_ERR_REFERENCE_TRAP;
-                    if (r.p[r.off++] != 0) return SWC_XZ_WRONG_PADDING;
-                    isz++;
-                }
-            }
-            if (!r.need(4)) return SWC_ERR_REFERENCE_TRAP;
-            if (crc32_framing(r.p + istart, (size_t)isz) != le32(r.p + r.off)) return SWC_XZ_WRONG_INFO_CRC;
-            r.off = istart + (size_t)isz + 4;
-            index_size = isz + 4;
+            st = xz::index(r, (int64_t)infos.size(), [&](int64_t k, int64_t *unp, int64_t *unc) {
+                *unp = infos[(size_t)k].first; *unc = infos[(size_t)k].second;
+            }, &index_size);
+            if (st) return st;
             break;
         }
         DevBuf blk; size_t blk_len = 0; int64_t unp = 0;
-        int st = xz_block(r, d_in, hs, check_size(ctype), blk, blk_len, &unp);
-        if (st) return st;
+        if ((st = xz_block(r, d_in, hs, xz::check_size(ctype), blk, blk_len, &unp))) return st;
         uint8_t *dst = out.grow(blk_len);
         if (!dst) return SWC_ERR_OUTPUT_OVERFLOW;
         if (blk_len) SWC_CUDA_TRY(cudaMemcpy(dst, blk.p, blk_len, cudaMemcpyDeviceToHost));
+        const uint8_t *stored = nullptr;
+        if ((st = xz::check_field(r, ctype, &stored))) return st;
         if (ctype == 1) {
-            if (!r.need(4)) return SWC_ERR_REFERENCE_TRAP;
-            const uint32_t c = le32(r.p + r.off); r.off += 4;
             u64 got = 0;
             if ((st = checks::check_device(checks::CRC32, blk.as<u8>(), blk_len, &got))) return st;
-            if ((uint32_t)got != c) { *check_error = true; return SWC_OK; }
+            if ((uint32_t)got != le32(stored)) { *check_error = true; return SWC_OK; }
         } else if (ctype == 4) {
-            if (!r.need(8)) return SWC_ERR_REFERENCE_TRAP;
-            const uint64_t c = (uint64_t)le32(r.p + r.off) | (uint64_t)le32(r.p + r.off + 4) << 32; r.off += 8;
             u64 got = 0;
             if ((st = checks::check_device(checks::CRC64, blk.as<u8>(), blk_len, &got))) return st;
-            if (got != c) { *check_error = true; return SWC_OK; }
+            if (got != ((uint64_t)le32(stored) | (uint64_t)le32(stored + 4) << 32)) { *check_error = true; return SWC_OK; }
         } else if (ctype == 0x0A) {
-            if (!r.need(32)) return SWC_ERR_REFERENCE_TRAP;
             DevBuf dg; uint8_t h[32];
             if ((st = dg.alloc(32))) return st;
             if ((st = checks::sha256(blk.as<u8>(), blk_len, dg.as<u8>(), 0))) return st;
             SWC_CUDA_TRY(cudaMemcpy(h, dg.p, 32, cudaMemcpyDeviceToHost));
-            const bool bad = memcmp(h, r.p + r.off, 32) != 0; r.off += 32;
-            if (bad) { *check_error = true; return SWC_OK; }
+            if (memcmp(h, stored, 32) != 0) { *check_error = true; return SWC_OK; }
         }
         infos.emplace_back(unp, (int64_t)blk_len);
     }
-    if (!r.need(12)) return SWC_ERR_REFERENCE_TRAP;                  // processFooter
-    const uint32_t fcrc = le32(r.p + r.off);
-    const int64_t backward = ((int64_t)le32(r.p + r.off + 4) + 1) * 4;
-    const unsigned fflags = r.p[r.off + 8] | r.p[r.off + 9] << 8;
-    if (crc32_framing(r.p + r.off + 4, 6) != fcrc) return SWC_XZ_WRONG_INFO_CRC;
-    if (backward != index_size) return SWC_XZ_WRONG_FIELD;
-    if (!((fflags & 0xFF) == 0 && ((fflags & 0xF00) >> 8) == (unsigned)ctype && (fflags & 0xF000) == 0)) return SWC_XZ_WRONG_FIELD;
-    if (!(r.p[r.off + 10] == 0x59 && r.p[r.off + 11] == 0x5A)) return SWC_XZ_WRONG_MAGIC;
-    r.off += 12;
-    return SWC_OK;
+    return xz::footer(r, ctype, index_size);
 }
 
-int xz_padding(Rd &r) {                                               // processPadding XZArchive.swift:194-218
-    if (r.off >= r.n) return SWC_OK;
-    int padding = 0;
-    for (;;) {
-        const unsigned b = r.p[r.off++];
-        if (b != 0) { if (padding % 4 != 0) return SWC_XZ_WRONG_PADDING; break; }
-        if (r.off >= r.n) { if (padding % 4 != 3) return SWC_XZ_WRONG_PADDING; return SWC_OK; }
-        padding++;
-    }
-    r.off -= 1;
-    return SWC_OK;
-}
-
-// Walk the stream footers / indexes backwards and batch-decode every single-filter LZMA2 block. Any inconsistency simply
-// ends the discovery (the in-order parser will then report it in the reference's order); only a CUDA error is returned.
+// Walk the stream footers / indexes backwards (xz::back_stream) and batch-decode every single-filter LZMA2 block. Any
+// inconsistency simply ends the discovery (the in-order parser will then report it in the reference's order); only a CUDA
+// error is returned.
 int xz_prefetch(const uint8_t *in, size_t n, const u8 *d_in, Prefetch &pf) {
     struct Blk { size_t data_off, comp_len, uncomp; u8 dict_byte; };
     std::vector<Blk> blks;
     size_t pos = n;
     while (pos >= 32) {
-        while (pos >= 4 && in[pos - 1] == 0 && in[pos - 2] == 0 && in[pos - 3] == 0 && in[pos - 4] == 0) pos -= 4;   // stream padding
-        if (pos < 32 || in[pos - 2] != 0x59 || in[pos - 1] != 0x5A) break;
-        const size_t foot = pos - 12;
-        const int ctype = in[foot + 9] & 0xF;
-        const size_t csize = (size_t)check_size(ctype);
-        const size_t index_size = ((size_t)le32(in + foot + 4) + 1) * 4;
-        if (index_size + 12 > foot) break;
-        const size_t istart = foot - index_size;
-        if (in[istart] != 0) break;
-        Rd ir{in, foot, istart + 1};
-        int64_t count = 0;
-        if (multibyte(ir, &count) || count < 0 || count > 1000000) break;
-        std::vector<std::pair<int64_t, int64_t>> recs((size_t)count);
-        bool bad = false; uint64_t blocks_total = 0;
-        for (auto &rc : recs) {                                   // untrusted sizes: every sum is checked against the bytes before the index
-            if (multibyte(ir, &rc.first) || multibyte(ir, &rc.second) || rc.first <= 0 || rc.second < 0) { bad = true; break; }
-            if ((uint64_t)rc.first > (uint64_t)istart) { bad = true; break; }
-            const uint64_t padded = ((uint64_t)rc.first + 3) & ~3ull;
-            if (padded > (uint64_t)istart - blocks_total) { bad = true; break; }
-            blocks_total += padded;
-        }
-        if (bad || blocks_total + 12 > istart) break;
-        const size_t sstart = istart - (size_t)blocks_total - 12;
-        static const uint8_t magic[6] = {0xFD, 0x37, 0x7A, 0x58, 0x5A, 0x00};
-        if (memcmp(in + sstart, magic, 6) != 0) break;
-        size_t boff = sstart + 12;
-        for (auto &rc : recs) {
+        xz::BackStream s;
+        if (!xz::back_stream(in, pos, s)) break;
+        const size_t csize = (size_t)xz::check_size(s.ctype), istart = s.istart;
+        Rd ir{in, s.foot, s.rec_off};                                   // the records back_stream checked
+        size_t boff = s.start + 12;
+        bool bad = false;
+        for (int64_t k = 0; k < s.count; k++) {
+            int64_t unp = 0, unc = 0;
+            xz::multibyte(ir, &unp); xz::multibyte(ir, &unc);          // read and checked by back_stream
             if (boff + 2 > istart) { bad = true; break; }
             const size_t hsz = ((size_t)in[boff] + 1) * 4;
             if (hsz > istart - boff) { bad = true; break; }
@@ -315,15 +187,15 @@ int xz_prefetch(const uint8_t *in, size_t n, const u8 *d_in, Prefetch &pf) {
             Rd hr{in, boff + hsz, boff + 1};
             const unsigned flags = in[boff + 1]; hr.off = boff + 2;
             int64_t tmp; bool ok = (flags & 0x3F) == 0;
-            if (ok && (flags & 0x40)) ok = multibyte(hr, &tmp) == 0;
-            if (ok && (flags & 0x80)) ok = multibyte(hr, &tmp) == 0;
-            if (ok && hr.off + 3 <= boff + hsz && in[hr.off] == 0x21 && in[hr.off + 1] == 1 && (size_t)rc.first > hsz + csize) {
-                blks.push_back({boff + hsz, (size_t)rc.first - hsz - csize, (size_t)rc.second, in[hr.off + 2]});
+            if (ok && (flags & 0x40)) ok = xz::multibyte(hr, &tmp) == 0;
+            if (ok && (flags & 0x80)) ok = xz::multibyte(hr, &tmp) == 0;
+            if (ok && hr.off + 3 <= boff + hsz && in[hr.off] == 0x21 && in[hr.off + 1] == 1 && (size_t)unp > hsz + csize) {
+                blks.push_back({boff + hsz, (size_t)unp - hsz - csize, (size_t)unc, in[hr.off + 2]});
             }
-            boff += ((size_t)rc.first + 3) & ~(size_t)3;
+            boff += ((size_t)unp + 3) & ~(size_t)3;
         }
         if (bad) break;
-        pos = sstart;
+        pos = s.start;
     }
     if (blks.size() < 2) return SWC_OK;                   // nothing to gain
     uint64_t total = 0;
@@ -369,7 +241,7 @@ int xz_all(const uint8_t *in, size_t n, HostOut &out, std::vector<size_t> &ends)
         if ((st = xz_stream(r, d_in.as<u8>(), out, &check_error))) return st;
         ends.push_back(out.len);
         if (check_error) return SWC_XZ_WRONG_CHECK;
-        if ((st = xz_padding(r))) return st;
+        if ((st = xz::padding(r))) return st;
     }
     return SWC_OK;
 }

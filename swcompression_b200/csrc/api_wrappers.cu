@@ -299,6 +299,13 @@ int32_t swc_adler32_batch(const uint8_t *in_base, const uint64_t *off, const uin
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     return checks::adler32_units(in_base, off, len, status, result, n, (cudaStream_t)cuda_stream);
 }
+int32_t swc_crc64_batch(const uint8_t *in_base, const uint64_t *off, const uint64_t *len, const int32_t *status,
+                        uint64_t *result, uint64_t n, void *cuda_stream) {
+    if (n == 0) return SWC_OK;
+    if (!in_base || !off || !len || !result) return SWC_ERR_INVALID_ARG;
+    if (ensure_device()) return SWC_ERR_NO_DEVICE;
+    return checks::crc64_units(in_base, off, len, status, result, n, (cudaStream_t)cuda_stream);
+}
 int32_t swc_xxh32_batch(const uint8_t *in_base, const uint64_t *off, const uint64_t *len,
                         uint32_t *result, uint64_t n, void *cuda_stream) {
     if (n == 0) return SWC_OK;

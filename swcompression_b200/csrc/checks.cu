@@ -9,6 +9,7 @@
 #include <algorithm>
 #include <vector>
 #include "checks.cuh"
+#include "checks_device.cuh"
 #include "host_util.h"
 
 namespace swc {
@@ -16,52 +17,7 @@ namespace checks {
 
 constexpr u32 CHUNK = 4096;
 
-// ---------------------------------------------------------------- GF(2) helpers (device)
-// reflected 32-bit: bit 31 = x^0
-__device__ u32 mulmod32r(u32 a, u32 b) {
-    u32 m = 1u << 31, p = 0;
-    for (;;) {
-        if (a & m) { p ^= b; if ((a & (m - 1)) == 0) break; }
-        m >>= 1;
-        b = (b & 1) ? (b >> 1) ^ 0xEDB88320u : b >> 1;
-    }
-    return p;
-}
-__device__ u64 mulmod64r(u64 a, u64 b) {
-    u64 m = 1ull << 63, p = 0;
-    for (;;) {
-        if (a & m) { p ^= b; if ((a & (m - 1)) == 0) break; }
-        m >>= 1;
-        b = (b & 1) ? (b >> 1) ^ 0xC96C5795D7870F42ull : b >> 1;
-    }
-    return p;
-}
-// normal (MSB-first) 32-bit: bit 0 = x^0, poly 0x04C11DB7
-__device__ u32 mulmod32n(u32 a, u32 b) {
-    u32 p = 0;
-    while (a) {
-        if (a & 1) p ^= b;
-        a >>= 1;
-        b = (b & 0x80000000u) ? (b << 1) ^ 0x04C11DB7u : b << 1;
-    }
-    return p;
-}
-// x^(8*nbytes) mod P in each representation
-__device__ u32 xpow32r(u64 nbytes) {
-    u32 p = 1u << 31, sq = 1u << 23;           // x^0, x^8
-    while (nbytes) { if (nbytes & 1) p = mulmod32r(sq, p); sq = mulmod32r(sq, sq); nbytes >>= 1; }
-    return p;
-}
-__device__ u64 xpow64r(u64 nbytes) {
-    u64 p = 1ull << 63, sq = 1ull << 55;
-    while (nbytes) { if (nbytes & 1) p = mulmod64r(sq, p); sq = mulmod64r(sq, sq); nbytes >>= 1; }
-    return p;
-}
-__device__ u32 xpow32n(u64 nbytes) {
-    u32 p = 1, sq = 1u << 8;
-    while (nbytes) { if (nbytes & 1) p = mulmod32n(sq, p); sq = mulmod32n(sq, sq); nbytes >>= 1; }
-    return p;
-}
+// GF(2) helpers, the warp CRC and SHA-256: checks_device.cuh
 
 // ---------------------------------------------------------------- chunk kernels
 template <int KIND>   // 0 crc32, 1 bzip2 crc32, 2 crc64, 3 adler32
@@ -146,56 +102,45 @@ int crc64(const u8 *d, u64 n, u64 *d_result, u64 *d_partial, cudaStream_t s) { r
 int adler32(const u8 *d, u64 n, u64 *d_result, u64 *d_partial, cudaStream_t s) { return run<3>(d, n, d_result, d_partial, s); }
 
 // ---------------------------------------------------------------- CRC-32 of many buffers: one warp per buffer
-// Each lane folds one of 32 contiguous segments (a multiple of 16 bytes, read with 16-byte loads) four bytes per step with
-// four byte tables in shared memory ("slicing by 4": 2.8 instead of 6 instructions per byte), then the 32 conditioned values
-// are chained with x^(8*len) multiplications — the same identity as above, inside one warp.
-__device__ __forceinline__ u32 crc_word(const u32 (*tab)[256], u32 c, u32 w) {
-    c ^= w;
-    return tab[3][c & 0xFF] ^ tab[2][(c >> 8) & 0xFF] ^ tab[1][(c >> 16) & 0xFF] ^ tab[0][c >> 24];
-}
+// warp_crc (checks_device.cuh): each lane folds one of 32 contiguous segments (a multiple of 16 bytes, read with 16-byte
+// loads) four bytes per step with four byte tables in shared memory ("slicing by 4": 2.8 instead of 6 instructions per byte),
+// then the 32 conditioned values are chained with x^(8*len) multiplications — the same identity as above, inside one warp.
 __global__ void __launch_bounds__(256) crc32_units_kernel(const u8 *base, const u64 *off, const u64 *len, const int32_t *status, u32 *result, u64 n) {
     __shared__ u32 tab[4][256];
-    for (u32 i = threadIdx.x; i < 256; i += blockDim.x) {
-        u32 c = i;
-        for (int k = 0; k < 8; k++) c = (c & 1) ? 0xEDB88320u ^ (c >> 1) : c >> 1;
-        tab[0][i] = c;
-    }
+    crc_tables<Crc32R>(tab, threadIdx.x, blockDim.x);
     __syncthreads();
-    for (int t = 1; t < 4; t++) {
-        for (u32 i = threadIdx.x; i < 256; i += blockDim.x) { const u32 c = tab[t - 1][i]; tab[t][i] = (c >> 8) ^ tab[0][c & 0xFF]; }
-        __syncthreads();
-    }
     const u64 unit = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (unit >= n) return;
-    const u32 lane = threadIdx.x & 31;
-    const u8 *p = base + off[unit];
     // a unit that did not decode cleanly has no defined extent (Deflate reports the size it WOULD need on overflow): skip it
     const u64 L = (status && status[unit] != SWC_OK) ? 0 : len[unit];
-    const u64 seg = (((L + 31) / 32) + 15) & ~(u64)15;
-    const u64 sb = lane * seg < L ? lane * seg : L, se = sb + seg < L ? sb + seg : L;
-    u32 c = 0xFFFFFFFFu;
-    u64 i = sb;
-    for (; i < se && ((uintptr_t)(p + i) & 15); i++) c = tab[0][(c ^ p[i]) & 0xFF] ^ (c >> 8);
-    for (; i + 16 <= se; i += 16) {
-        const uint4 v = __ldg((const uint4 *)(p + i));
-        c = crc_word(tab, c, v.x); c = crc_word(tab, c, v.y); c = crc_word(tab, c, v.z); c = crc_word(tab, c, v.w);
-    }
-    for (; i < se; i++) c = tab[0][(c ^ p[i]) & 0xFF] ^ (c >> 8);
-    c = ~c;
-    const u32 pw = xpow32r(seg);
-    u32 acc = __shfl_sync(0xFFFFFFFFu, c, 0);
-    for (int l = 1; l < 32; l++) {
-        const u32 pl = __shfl_sync(0xFFFFFFFFu, c, l);
-        const u64 lb = (u64)l * seg < L ? (u64)l * seg : L, le = lb + seg < L ? lb + seg : L;
-        if (le == lb) continue;
-        acc = mulmod32r(le - lb == seg ? pw : xpow32r(le - lb), acc) ^ pl;
-    }
-    if (lane == 0) result[unit] = acc;
+    const u32 c = warp_crc<Crc32R, true>(tab, base + off[unit], L);
+    if (lane_id() == 0) result[unit] = c;
 }
 
 int crc32_units(const u8 *base, const u64 *off, const u64 *len, const int32_t *status, u32 *result, u64 n, cudaStream_t s) {
     if (!n) return SWC_OK;
     crc32_units_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, s>>>(base, off, len, status, result, n);
+    count_launch();
+    SWC_CUDA_TRY(cudaGetLastError());
+    return SWC_OK;
+}
+
+// ---------------------------------------------------------------- CRC-64 of many buffers: one warp per buffer
+// warp_crc (checks_device.cuh), the segment scheme of crc32_units_kernel in 64 bits; 8 KiB of slicing tables per CTA
+__global__ void __launch_bounds__(256) crc64_units_kernel(const u8 *base, const u64 *off, const u64 *len, const int32_t *status, u64 *result, u64 n) {
+    __shared__ u64 tab[4][256];
+    crc_tables<Crc64R>(tab, threadIdx.x, blockDim.x);
+    __syncthreads();
+    const u64 unit = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (unit >= n) return;
+    const u64 L = (status && status[unit] != SWC_OK) ? 0 : len[unit];
+    const u64 c = warp_crc<Crc64R, true>(tab, base + off[unit], L);
+    if (lane_id() == 0) result[unit] = c;
+}
+
+int crc64_units(const u8 *base, const u64 *off, const u64 *len, const int32_t *status, u64 *result, u64 n, cudaStream_t s) {
+    if (!n) return SWC_OK;
+    crc64_units_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, s>>>(base, off, len, status, result, n);
     count_launch();
     SWC_CUDA_TRY(cudaGetLastError());
     return SWC_OK;
@@ -415,52 +360,7 @@ int xxh32_batch(const u8 *base, const u64 *off, const u64 *len, u32 *result, u64
 }
 
 // ---------------------------------------------------------------- SHA-256, one thread
-__constant__ u32 c_k256[64] = {
-    0x428a2f98, 0x71374491, 0xb5c0fbcf, 0xe9b5dba5, 0x3956c25b, 0x59f111f1, 0x923f82a4, 0xab1c5ed5, 0xd807aa98, 0x12835b01,
-    0x243185be, 0x550c7dc3, 0x72be5d74, 0x80deb1fe, 0x9bdc06a7, 0xc19bf174, 0xe49b69c1, 0xefbe4786, 0x0fc19dc6, 0x240ca1cc,
-    0x2de92c6f, 0x4a7484aa, 0x5cb0a9dc, 0x76f988da, 0x983e5152, 0xa831c66d, 0xb00327c8, 0xbf597fc7, 0xc6e00bf3, 0xd5a79147,
-    0x06ca6351, 0x14292967, 0x27b70a85, 0x2e1b2138, 0x4d2c6dfc, 0x53380d13, 0x650a7354, 0x766a0abb, 0x81c2c92e, 0x92722c85,
-    0xa2bfe8a1, 0xa81a664b, 0xc24b8b70, 0xc76c51a3, 0xd192e819, 0xd6990624, 0xf40e3585, 0x106aa070, 0x19a4c116, 0x1e376c08,
-    0x2748774c, 0x34b0bcb5, 0x391c0cb3, 0x4ed8aa4a, 0x5b9cca4f, 0x682e6ff3, 0x748f82ee, 0x78a5636f, 0x84c87814, 0x8cc70208,
-    0x90befffa, 0xa4506ceb, 0xbef9a3f7, 0xc67178f2};
-__device__ __forceinline__ u32 rotr32(u32 v, int s) { return __funnelshift_r(v, v, s); }
-
-__device__ void sha256_block(u32 h[8], const u8 *b) {
-    u32 w[64];
-#pragma unroll
-    for (int i = 0; i < 16; i++) w[i] = (u32)b[4 * i] << 24 | (u32)b[4 * i + 1] << 16 | (u32)b[4 * i + 2] << 8 | b[4 * i + 3];
-#pragma unroll
-    for (int i = 16; i < 64; i++) {
-        u32 s0 = rotr32(w[i - 15], 7) ^ rotr32(w[i - 15], 18) ^ (w[i - 15] >> 3);
-        u32 s1 = rotr32(w[i - 2], 17) ^ rotr32(w[i - 2], 19) ^ (w[i - 2] >> 10);
-        w[i] = w[i - 16] + s0 + w[i - 7] + s1;
-    }
-    u32 a = h[0], bb = h[1], c = h[2], d = h[3], e = h[4], f = h[5], g = h[6], hh = h[7];
-#pragma unroll
-    for (int i = 0; i < 64; i++) {
-        u32 t1 = hh + (rotr32(e, 6) ^ rotr32(e, 11) ^ rotr32(e, 25)) + ((e & f) ^ (~e & g)) + c_k256[i] + w[i];
-        u32 t2 = (rotr32(a, 2) ^ rotr32(a, 13) ^ rotr32(a, 22)) + ((a & bb) ^ (a & c) ^ (bb & c));
-        hh = g; g = f; f = e; e = d + t1; d = c; c = bb; bb = a; a = t1 + t2;
-    }
-    h[0] += a; h[1] += bb; h[2] += c; h[3] += d; h[4] += e; h[5] += f; h[6] += g; h[7] += hh;
-}
-
-__global__ void sha256_kernel(const u8 *p, u64 n, u8 *digest) {
-    u32 h[8] = {0x6a09e667, 0xbb67ae85, 0x3c6ef372, 0xa54ff53a, 0x510e527f, 0x9b05688c, 0x1f83d9ab, 0x5be0cd19};
-    u64 i = 0;
-    for (; i + 64 <= n; i += 64) sha256_block(h, p + i);
-    u8 tail[128];
-    for (int k = 0; k < 128; k++) tail[k] = 0;
-    u64 rem = n - i;
-    for (u64 k = 0; k < rem; k++) tail[k] = p[i + k];
-    tail[rem] = 0x80;
-    int tl = rem + 9 <= 64 ? 64 : 128;
-    u64 bits = n * 8;
-    for (int k = 0; k < 8; k++) tail[tl - 1 - k] = (u8)(bits >> (8 * k));
-    sha256_block(h, tail);
-    if (tl == 128) sha256_block(h, tail + 64);
-    for (int k = 0; k < 8; k++) { digest[4 * k] = (u8)(h[k] >> 24); digest[4 * k + 1] = (u8)(h[k] >> 16); digest[4 * k + 2] = (u8)(h[k] >> 8); digest[4 * k + 3] = (u8)h[k]; }
-}
+__global__ void sha256_kernel(const u8 *p, u64 n, u8 *digest) { sha256_buffer(p, n, digest); }
 
 int sha256(const u8 *d, u64 n, u8 *d_digest, cudaStream_t s) {
     sha256_kernel<<<1, 1, 0, s>>>(d, n, d_digest);

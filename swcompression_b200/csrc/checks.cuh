@@ -14,6 +14,7 @@ int adler32(const u8 *d, u64 n, u64 *d_result, u64 *d_partial, cudaStream_t s);
 int xxh32_batch(const u8 *base, const u64 *off /* may be null */, const u64 *len, u32 *result, u64 n, cudaStream_t s);
 int sha256(const u8 *d, u64 n, u8 *d_digest, cudaStream_t s);
 int crc32_units(const u8 *base, const u64 *off, const u64 *len, const int32_t *status, u32 *result, u64 n, cudaStream_t s);   // warp per buffer; units with status != 0 are skipped (status may be null)
+int crc64_units(const u8 *base, const u64 *off, const u64 *len, const int32_t *status, u64 *result, u64 n, cudaStream_t s);   // the same for CRC-64
 int adler32_units(const u8 *base, const u64 *off, const u64 *len, const int32_t *status, u32 *result, u64 n, cudaStream_t s);  // the same for Adler-32 (skipped units: 0)
 int find_gzip_members(const u8 *d_in, u64 n, std::vector<size_t> &pos);   // sorted candidate member starts (device scan)
 int find_bzip2_magics(const u8 *d_in, u64 begin, u64 n, std::vector<u64> &entries);   // sorted (bit position << 1 | is_end_magic), device scan

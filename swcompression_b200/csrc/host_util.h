@@ -34,7 +34,7 @@ struct ApiLock {
     std::unique_lock<std::recursive_mutex> lk;
     ApiLock() : lk(device_ctx().api_mu) {}
 };
-enum { CFG_INFLATE_K1W = 0, CFG_INFLATE_K1L = 1, CFG_LZMA = 2, CFG_BZIP2_CRC = 3, CFG_LZ4 = 4 };
+enum { CFG_INFLATE_K1W = 0, CFG_INFLATE_K1L = 1, CFG_LZMA = 2, CFG_BZIP2_CRC = 3, CFG_LZ4 = 4, CFG_XZ = 5 };
 // runs `f` (returning an swc status) once per device, thread-safe; a failing `f` is retried by the next caller
 template <typename F> int configure_once(int slot, F f) {
     DeviceCtx &c = device_ctx();

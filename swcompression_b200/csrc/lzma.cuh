@@ -18,6 +18,7 @@ struct Args : DecodeIO {
 
 inline size_t lit_scratch_bytes(u64 n) { return (size_t)n * 4096 * 0x300 * 2; }
 int launch(const Args &a, cudaStream_t stream);
+int occupancy_blocks(int *blocks);   // resident lzma_kernel CTAs per SM (cudaOccupancyMaxActiveBlocksPerMultiprocessor)
 
 }  // namespace lzma
 }  // namespace swc
