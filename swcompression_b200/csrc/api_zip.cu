@@ -32,6 +32,8 @@ struct Seq {                       // sequential reads on top of a View: `at` ma
 };
 
 // String(data:encoding:.utf8) != nil
+constexpr uint64_t kDeflateUnitMax = ((uint64_t)1 << 28) - 1;     // longest Deflate unit every batch kernel takes
+
 bool utf8_ok(const uint8_t *s, size_t n) {
     for (size_t i = 0; i < n;) {
         const unsigned b = s[i];
@@ -280,6 +282,7 @@ int32_t swc_zip_open(const uint8_t *in, size_t in_len, uint8_t **out, size_t *ou
     struct Unit { size_t item; uint64_t in_off, in_len, out_off, cap; };
     std::vector<Unit> grp[4];                                           // 0 stored, 1 deflate, 2 bzip2, 3 lzma
     std::vector<int> early(n, SWC_OK);                                  // errors known before any decoding (reported in entry order)
+    std::vector<char> clipped(n, 0);                                    // Deflate units given less than the rest of the container
     uint64_t out_total = 0;
     for (size_t i = 0; i < n; i++) {
         Item &it = items[i];
@@ -299,7 +302,12 @@ int32_t swc_zip_open(const uint8_t *in, size_t in_len, uint8_t **out, size_t *ou
         const uint64_t reach = g == 1 ? avail * 1032 + 64 : g == 2 ? avail * 65536 + 4096 : g == 3 ? avail * 8192 + 4096 : avail;
         if (cap > reach + 16) cap = reach + 16;
         if (cap > ((uint64_t)8 << 30)) cap = (uint64_t)8 << 30;
-        Unit u{i, (uint64_t)it.data_off + (g == 3 ? 9 : 0), avail - (g == 3 ? 9 : 0), out_total, cap};
+        // A Deflate stream has no length of its own: the reference reads it from the rest of the container.  The batch's
+        // table-lookup kernel keeps 32-bit bit positions and refuses units of 2^28 bytes or more, so in a container past
+        // 256 MiB a unit gets at most 2^28 - 1 bytes; a clipped unit that fails is decoded again on its own with everything.
+        uint64_t in_len = avail - (g == 3 ? 9 : 0);
+        if (g == 1 && in_len > kDeflateUnitMax) { in_len = kDeflateUnitMax; clipped[i] = 1; }
+        Unit u{i, (uint64_t)it.data_off + (g == 3 ? 9 : 0), in_len, out_total, cap};
         out_total += round16((size_t)cap) + 16;
         grp[g].push_back(u);
     }
@@ -371,9 +379,10 @@ int32_t swc_zip_open(const uint8_t *in, size_t in_len, uint8_t **out, size_t *ou
         int ust = r_st[j];
         uint64_t got = r_len[j], used = r_used[j];
         uint32_t crc_got = r_crc[j];
-        if (ust == SWC_ERR_OUTPUT_OVERFLOW || ust == SWC_ERR_UNSUPPORTED) {
-            // more output than declared (-> wrongSize, unless the stream fails further on), or an LZMA stream the batch kernel
-            // does not take (lc + lp > 4): decode this entry alone through the single-unit path, which sizes itself
+        if (ust == SWC_ERR_OUTPUT_OVERFLOW || ust == SWC_ERR_UNSUPPORTED || (ust != SWC_OK && clipped[i])) {
+            // more output than declared (-> wrongSize, unless the stream fails further on), an LZMA stream the batch kernel
+            // does not take (lc + lp > 4), or a clipped Deflate unit that may have run out of input: decode this entry alone
+            // through the single-unit path, which sizes itself and reads the whole rest of the container
             const uint8_t *p = in + it.data_off;
             const size_t avail = in_len - (size_t)it.data_off;
             uint8_t *o = nullptr; size_t ol = 0, c = 0;
