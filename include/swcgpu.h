@@ -101,6 +101,52 @@ int32_t swc_lz4_block_decompress_batch_host(const uint8_t *in_base, const uint64
                                             uint64_t out_capacity_total,
                                             uint64_t *out_len, int32_t *status, uint64_t n);
 
+/* Whole frames, device memory, one asynchronous enqueue on `cuda_stream`.  Unit i is in_base[in_off[i] ..+ in_len[i]), any
+ * alignment ("Batch layout"), decoded as LZ4.decompress(data:dictionary:dictionaryID:) decodes it: leading skippable frames
+ * are skipped, then the first frame or legacy frame is decoded and the bytes behind it are ignored; consumed_bytes[i] is
+ * where it ended.  One dictionary (device pointer, NULL = nil; an empty dictionary is a non-NULL pointer with dict_len 0)
+ * serves the whole batch.  A unit that starts with a skippable frame is decoded without the dictionary and the dictionary
+ * ID, as the reference's recursion into decompress(data:) does.
+ * status[i] is what swc_lz4_decompress returns for the same bytes: the first failure the reference's sequential loop
+ * meets (descriptor checks, then per block: mark, size, room, block checksum, decode; then content size, content checksum).
+ * SWC_DATA_CHECKSUM_MISMATCH carries its data: the unit's output region holds the decoded bytes.
+ * Capacity: a unit that would be SWC_OK or SWC_DATA_CHECKSUM_MISMATCH but decodes to more than out_cap[i] reports
+ * SWC_ERR_OUTPUT_OVERFLOW with out_len[i] = the exact decoded size, so one rerun with that capacity gives the final
+ * answer; every other failure is reported as with unlimited capacity.  out_len[i] is the decoded size on OK /
+ * checksumMismatch, the required size on overflow and 0 otherwise; consumed_bytes[i] is set on OK / checksumMismatch and 0
+ * otherwise.  Nothing is written outside [out_off[i], out_off[i] + out_cap[i]); no byte outside a unit affects its result.
+ * max_blocks > 0 is the capacity of the batch's block table (at most 2^32 - 1): grids are sized from it and, with a
+ * caller scratch of swc_lz4_frame_batch_scratch_bytes(n, sum of in_len, max_blocks) bytes, the call reads nothing back and
+ * allocates nothing, so it can be captured in a CUDA graph.  Units are placed in order; a unit whose blocks do not fit in
+ * what is left of the table (or of the scratch) reports SWC_ERR_UNSUPPORTED and writes nothing; units without blocks
+ * always fit.  max_blocks == 0 lets the library count first (one walk, one synchronisation); a caller scratch too small for
+ * the count is SWC_ERR_INVALID_ARG.  scratch == NULL takes the library pool (and, with max_blocks > 0, reads in_len back).
+ * swc_lz4_frame_info_batch is the walk on its own, for sizing max_blocks and, when the frame declares it, out_cap. */
+#define SWC_LZ4F_DICTIONARY_DROPPED 0x100u   /* flags: a skippable frame came first, the unit decodes without dictionary */
+#define SWC_LZ4F_CHECKSUM_CUT       0x200u   /* flags: the EndMark was reached but the content checksum is cut short */
+typedef struct swc_lz4_frame_info {
+    int32_t  status;          /* the first framing failure (descriptor, block marks, end), or SWC_OK */
+    uint32_t kind;            /* 0 no frame (status says why), 1 independent blocks, 2 dependent blocks, 3 legacy */
+    uint64_t n_blocks;        /* blocks in front of the EndMark or of the framing failure */
+    uint32_t flags;           /* the FLG byte (0 for a legacy frame) | SWC_LZ4F_* */
+    uint32_t max_block_size;  /* from the BD byte; 0 for a legacy frame */
+    uint64_t content_size;    /* UINT64_MAX when the frame does not declare it */
+    uint64_t frame_start;     /* offset of the frame's magic in the unit (behind the skippable frames) */
+    uint64_t frame_end;       /* offset behind the frame when the walk reached it (= consumed_bytes), else 0 */
+} swc_lz4_frame_info;
+size_t  swc_lz4_frame_batch_scratch_bytes(uint64_t n, uint64_t in_bytes_total, uint64_t max_blocks);
+int32_t swc_lz4_frame_decompress_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                                       const uint8_t *dict /* device, NULL = nil */, uint64_t dict_len,
+                                       int32_t has_dict_id, uint32_t dict_id,
+                                       uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                       uint64_t *out_len, uint64_t *consumed_bytes, int32_t *status,
+                                       uint64_t n, uint64_t max_blocks,
+                                       void *scratch, size_t scratch_bytes, void *cuda_stream);
+int32_t swc_lz4_frame_info_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                                 int32_t has_dict, int32_t has_dict_id, uint32_t dict_id,
+                                 swc_lz4_frame_info *info /* device, n entries */,
+                                 uint64_t n, void *cuda_stream);
+
 /* ---- LZ4 compression ----------------------------------------------------------------------------------------
  * LZ4.compress(data:)                                                     Sources/LZ4/LZ4+Compress.swift:16-19
  * LZ4.compress(data:independentBlocks:blockChecksums:contentChecksum:contentSize:blockSize:dictionary:dictionaryID:)

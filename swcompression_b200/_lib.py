@@ -35,6 +35,13 @@ def declared_symbols():
     return sorted(set(re.findall(r"\b(swc_[a-z0-9_]+)\s*\(", txt)))
 
 
+class Lz4FrameInfo(C.Structure):
+    """swc_lz4_frame_info (include/swcgpu.h)"""
+    _fields_ = [("status", C.c_int32), ("kind", C.c_uint32), ("n_blocks", C.c_uint64), ("flags", C.c_uint32),
+                ("max_block_size", C.c_uint32), ("content_size", C.c_uint64), ("frame_start", C.c_uint64),
+                ("frame_end", C.c_uint64)]
+
+
 def lib():
     global _LIB
     if _LIB is None:
@@ -61,6 +68,10 @@ def lib():
         L.swc_lz4_multi_decompress.argtypes = [vp, sz, vp, sz, i32, u32, C.POINTER(vp), szp, C.POINTER(vp), szp]
         L.swc_lz4_block_decompress_batch.argtypes = [vp, vp, vp, vp, u64, vp, vp, vp, vp, vp, u64, vp]
         L.swc_lz4_block_decompress_batch_host.argtypes = [vp, vp, vp, u64, vp, vp, vp, u64, vp, vp, u64]
+        L.swc_lz4_frame_batch_scratch_bytes.restype = C.c_size_t
+        L.swc_lz4_frame_batch_scratch_bytes.argtypes = [u64, u64, u64]
+        L.swc_lz4_frame_decompress_batch.argtypes = [vp, vp, vp, vp, u64, i32, u32, vp, vp, vp, vp, vp, vp, u64, u64, vp, sz, vp]
+        L.swc_lz4_frame_info_batch.argtypes = [vp, vp, vp, i32, i32, u32, vp, u64, vp]
         L.swc_lz4_compress.argtypes = [vp, sz, i32, i32, i32, i32, C.c_int64, vp, sz, i32, u32, C.POINTER(vp), szp]
         L.swc_lz4_compress_batch_scratch_bytes.restype = C.c_size_t
         L.swc_lz4_compress_batch_scratch_bytes.argtypes = [C.c_uint64, C.c_uint64]

@@ -54,13 +54,19 @@ def pack_units(units, align=16):
 
 class Batch:
     """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'lzma2', 'gzip', 'zlib', 'xz',
-    'lz4_block_compress', 'deflate_compress', 'bzip2_compress').
+    'lz4_frame', 'lz4_block_compress', 'deflate_compress', 'bzip2_compress').
 
     'gzip' / 'zlib' decode one archive per unit (GzipArchive.unarchive, GzipArchive.swift:38-47, 79-100 / ZlibArchive.unarchive,
     ZlibArchive.swift:25-42): the first member only, whose status, size and consumed bytes results() returns.  With
     `headers=True` a 'gzip' batch also fills a device array of swc_gzip_header, which gzip_headers() reads back.
     'xz' decodes one whole .xz file per unit (XZArchive.unarchive, XZArchive.swift:27-50): every stream and block, the outputs
     concatenated.  It takes no scratch and no aux, and reports no consumed bytes (results() gives zeros in that column).
+
+    'lz4_frame' decodes the first LZ4 frame of each unit (LZ4.decompress(data:dictionary:dictionaryID:), LZ4.swift:73-91):
+    `aux` is the dictionary's bytes (None: nil), `dict_id` the dictionary ID (None: nil), and results() gives the consumed
+    bytes.  `max_blocks` is the capacity of the batch's block table; with it the batch owns a scratch sized for it and run()
+    reads nothing back (it can be captured in a CUDA graph).  None lets the library count the blocks first (one
+    synchronisation) and use its pool.
 
     'lz4_block_compress' compresses each unit into a raw LZ4 block (LZ4+Compress.swift:156-277); `aux` is then an optional
     (dict_off, dict_len) pair of u64 arrays placing each unit's dictionary window inside `in_buf`.
@@ -74,7 +80,7 @@ class Batch:
     cannot hold the largest unit fails the run with SWC_ERR_INVALID_ARG)."""
 
     def __init__(self, codec, in_buf, in_off, in_len, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=1,
-                 headers=False):
+                 headers=False, dict_id=None, max_blocks=None):
         self.codec = codec
         self.device = torch.device(device)
         self.n = len(in_off)
@@ -98,7 +104,16 @@ class Batch:
         self.d_scratch = None
         self.d_dict_off = self.d_dict_len = None
         self.block_size = int(block_size)
-        if codec == "lz4_block_compress":
+        self.dict_id, self.max_blocks = dict_id, 0 if max_blocks is None else int(max_blocks)
+        if codec == "lz4_frame":
+            # an empty dictionary is still a dictionary: one spare byte keeps its pointer non-null
+            self.dict_len = 0 if aux is None else len(aux)
+            self.d_aux = None if aux is None else t(np.frombuffer(bytes(aux) + b"\0", dtype=np.uint8).copy())
+            if self.max_blocks:
+                nbytes = _lib.lib().swc_lz4_frame_batch_scratch_bytes(self.n, int(np.asarray(in_len, dtype=np.uint64).sum()),
+                                                                     self.max_blocks)
+                self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        elif codec == "lz4_block_compress":
             self.d_aux = None
             if aux is not None:
                 self.d_dict_off, self.d_dict_len = t(np.asarray(aux[0], dtype=np.uint64)), t(np.asarray(aux[1], dtype=np.uint64))
@@ -121,9 +136,10 @@ class Batch:
             self.d_headers = torch.zeros(max(self.n, 1) * C.sizeof(_CGzipHeader), dtype=torch.uint8, device=self.device)
 
     @classmethod
-    def from_units(cls, codec, units, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=1, headers=False):
+    def from_units(cls, codec, units, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=1, headers=False,
+                   dict_id=None, max_blocks=None):
         buf, offs, lens = pack_units(units)
-        return cls(codec, buf, offs, lens, out_cap, device, aux, scratch_bytes, block_size, headers)
+        return cls(codec, buf, offs, lens, out_cap, device, aux, scratch_bytes, block_size, headers, dict_id, max_blocks)
 
     def run(self):
         L = _lib.lib()
@@ -150,6 +166,13 @@ class Batch:
             st = L.swc_lz4_block_decompress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), None, 0, p(self.d_out),
                                                   p(self.d_out_off), p(self.d_out_cap), p(self.d_out_len), p(self.d_status),
                                                   self.n, stream)
+        elif self.codec == "lz4_frame":
+            opt = lambda t: None if t is None else p(t)
+            st = L.swc_lz4_frame_decompress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), opt(self.d_aux), self.dict_len,
+                                                  self.dict_id is not None, self.dict_id or 0, p(self.d_out), p(self.d_out_off),
+                                                  p(self.d_out_cap), p(self.d_out_len), p(self.d_consumed), p(self.d_status),
+                                                  self.n, self.max_blocks, opt(self.d_scratch),
+                                                  0 if self.d_scratch is None else self.d_scratch.numel(), stream)
         elif self.codec == "lz4_block_compress":
             opt = lambda t: None if t is None else p(t)
             st = L.swc_lz4_block_compress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), opt(self.d_dict_off),
@@ -177,7 +200,7 @@ class Batch:
 
     def results(self):
         """-> (status int32[n], out_len int64[n], consumed int64[n]) on the host (synchronises).  consumed is in bits for
-        'deflate' and 'bzip2', in bytes for 'lzma2', 'gzip' and 'zlib', and 0 for 'xz'."""
+        'deflate' and 'bzip2', in bytes for 'lzma2', 'gzip', 'zlib' and 'lz4_frame', and 0 for 'xz'."""
         torch.cuda.synchronize(self.device)
         return self.d_status.cpu().numpy(), self.d_out_len.cpu().numpy(), self.d_consumed.cpu().numpy()
 

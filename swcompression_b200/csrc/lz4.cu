@@ -76,7 +76,7 @@ __device__ __forceinline__ void lz4_block_body(const Args &a) {
     const u64 cap = a.out_cap[unit];
     const u64 b0 = a.first_blk ? a.first_blk[unit] : unit;
     const u64 nb = a.n_blk ? a.n_blk[unit] : 1;
-    const i64 dict_len = (i64)a.dict_len;
+    const i64 dict_len = (a.no_dict && a.no_dict[unit]) ? 0 : (i64)a.dict_len;
     const u8 *dict_end = a.dict + a.dict_len;       // dict bytes sit at virtual positions [-dict_len, 0)
     u64 op = 0, fail_blk = 0;
     int status = SWC_OK;
@@ -161,7 +161,6 @@ __device__ __forceinline__ void lz4_block_body(const Args &a) {
 //      (>= 64 bytes: incompressible or zero-filled blocks) are done by the whole warp.
 // Units whose lengths do not fit 24 bits, and units that read or write 4 GiB or more, are flagged for the one-kernel
 // decoder above.
-constexpr int LZ4_INTERNAL_FALLBACK = 9002;
 
 __device__ __forceinline__ u32 ext_bytes(u32 len_field_value /* length minus its base */) {
     return len_field_value < 15 ? 0u : 1u + (len_field_value - 15u) / 255u;
@@ -178,9 +177,12 @@ __global__ void __launch_bounds__(128) lz4_parse_kernel(Args a, const u64 *rec_b
     u32 nrec = 0;
     int status = SWC_OK;
     u64 ip = 0, op = 0, seq = 0;
-    const u64 prefix = a.dict ? a.dict_len : 0;
+    const u64 prefix = a.dict && !(a.no_dict && a.no_dict[unit]) ? a.dict_len : 0;
     i64 last_match_start = -1;
-    if (stored) { status = LZ4_INTERNAL_FALLBACK; }
+    // a stored block, or a field that does not fit a record: the walk goes on without records, so that the size and the
+    // status are final here, and the one-kernel decoder does the copying
+    bool no_records = stored;
+    if (stored) { op = n; }
     else for (;;) {
         seq++;
         if (ip >= n) { status = SWC_DATA_TRUNCATED; break; }                                     // LZ4.swift:343
@@ -196,8 +198,8 @@ __global__ void __launch_bounds__(128) lz4_parse_kernel(Args a, const u64 *rec_b
         if (ip == n) {                                                                           // :369-377
             if (!(lit >= 5 || seq == 1)) status = SWC_DATA_CORRUPTED;
             else if (last_match_start >= 0 && (i64)op - last_match_start < 12) status = SWC_DATA_CORRUPTED;
-            else if (lit >= (1u << 24)) status = LZ4_INTERNAL_FALLBACK;
-            else rec[nrec++] = lit;
+            else if (lit >= (1u << 24)) no_records = true;
+            else if (!no_records) rec[nrec++] = lit;
             break;
         }
         if (n - ip < 2) { status = SWC_DATA_TRUNCATED; break; }                                  // :379
@@ -211,14 +213,14 @@ __global__ void __launch_bounds__(128) lz4_parse_kernel(Args a, const u64 *rec_b
             if (!ok) { status = SWC_DATA_TRUNCATED; break; }
         }
         last_match_start = (i64)op;
-        if (lit >= (1u << 24) || mlen >= (1u << 24)) { status = LZ4_INTERNAL_FALLBACK; break; }
-        rec[nrec++] = lit | (mlen << 24) | ((u64)offset << 48);
+        if (lit >= (1u << 24) || mlen >= (1u << 24)) no_records = true;
+        if (!no_records) rec[nrec++] = lit | (mlen << 24) | ((u64)offset << 48);
         op += mlen;
     }
     if (status == SWC_OK && op > cap) status = SWC_ERR_OUTPUT_OVERFLOW;
     // the exec kernel keeps input and output positions in 32 bits: a block that reads or writes 4 GiB or more goes to the
     // fallback (after the capacity check, so that an overflowing unit still reports its exact size)
-    if (status == SWC_OK && ((op >> 32) != 0 || (n >> 32) != 0)) status = LZ4_INTERNAL_FALLBACK;
+    if (status == SWC_OK && (no_records || (op >> 32) != 0 || (n >> 32) != 0)) status = LZ4_INTERNAL_FALLBACK;
     a.out_len[unit] = op;
     a.status[unit] = status;
     rec_count[unit] = nrec;
@@ -359,6 +361,22 @@ size_t two_phase_scratch_bytes(u64 n, u64 in_total) {
 __global__ void __launch_bounds__(256) lz4_block_kernel(Args a) { lz4_block_body<false>(a); }
 __global__ void __launch_bounds__(256) lz4_fallback_kernel(Args a) { lz4_block_body<true>(a); }
 
+int launch_parse(const Args &a, const u64 *rec_base, u64 *recs, u32 *rec_count, cudaStream_t stream) {
+    lz4_parse_kernel<<<(unsigned)((a.n + 127) / 128), 128, 0, stream>>>(a, rec_base, recs, rec_count);
+    count_launch();
+    SWC_CUDA_TRY(cudaGetLastError());
+    return SWC_OK;
+}
+
+int launch_exec(const Args &a, const u64 *rec_base, const u64 *recs, const u32 *rec_count, cudaStream_t stream) {
+    lz4_exec_kernel<<<(unsigned)((a.n * 32 + 255) / 256), 256, 0, stream>>>(a, rec_base, recs, rec_count);
+    timing_mark(stream);
+    lz4_fallback_kernel<<<(unsigned)((a.n * 32 + 255) / 256), 256, 0, stream>>>(a);
+    count_launch(2);
+    SWC_CUDA_TRY(cudaGetLastError());
+    return SWC_OK;
+}
+
 int launch(const Args &a, cudaStream_t stream) {
     if (a.n == 0) return SWC_OK;
     if (a.first_blk == nullptr && a.scratch != nullptr) {
@@ -367,14 +385,10 @@ int launch(const Args &a, cudaStream_t stream) {
         u64 *recs = (u64 *)(((uintptr_t)(cnt + a.n) + 255) & ~(uintptr_t)255);
         timing_mark(stream);
         lz4_rec_scan_kernel<<<1, 1024, 0, stream>>>(a.in_len, a.n, base);
-        lz4_parse_kernel<<<(unsigned)((a.n + 127) / 128), 128, 0, stream>>>(a, base, recs, cnt);
+        count_launch();
+        if (int st = launch_parse(a, base, recs, cnt, stream)) return st;
         timing_mark(stream);
-        lz4_exec_kernel<<<(unsigned)((a.n * 32 + 255) / 256), 256, 0, stream>>>(a, base, recs, cnt);
-        timing_mark(stream);
-        lz4_fallback_kernel<<<(unsigned)((a.n * 32 + 255) / 256), 256, 0, stream>>>(a);
-        count_launch(4);
-        SWC_CUDA_TRY(cudaGetLastError());
-        return SWC_OK;
+        return launch_exec(a, base, recs, cnt, stream);
     }
     const u64 g = (a.n * 32 + 255) / 256;
     lz4_block_kernel<<<(unsigned)g, 256, 0, stream>>>(a);
