@@ -155,7 +155,8 @@ int32_t swc_lz4_frame_info_batch(const uint8_t *in_base, const uint64_t *in_off,
  * The output bytes equal the reference's for every option combination (its greedy parse, not liblz4's).  The reference
  * cannot fail; where it traps (block_size outside 1 ... 4 MiB, a 1-3 byte dictionary, a dependent frame of blocks of
  * 1-3 bytes) these calls return SWC_ERR_REFERENCE_TRAP.
- * swc_lz4_compress: one frame from host memory; dict == NULL is `dictionary: nil`, has_dict_id == 0 `dictionaryID: nil`. */
+ * swc_lz4_compress: one frame from host memory; dict == NULL is `dictionary: nil`, has_dict_id == 0 `dictionaryID: nil`.
+ * It runs as the one-unit swc_lz4_frame_compress_batch below. */
 int32_t swc_lz4_compress(const uint8_t *in, size_t in_len, int32_t independent_blocks, int32_t block_checksums,
                          int32_t content_checksum, int32_t content_size, int64_t block_size,
                          const uint8_t *dict, size_t dict_len, int32_t has_dict_id, uint32_t dict_id,
@@ -175,6 +176,41 @@ int32_t swc_lz4_block_compress_batch(const uint8_t *in_base, const uint64_t *in_
                                      const uint64_t *dict_off /* NULL = none */, const uint64_t *dict_len,
                                      uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
                                      uint64_t *out_len, int32_t *status, uint64_t n,
+                                     void *scratch, size_t scratch_bytes, void *cuda_stream);
+/* Whole frames, device memory, one asynchronous enqueue on `cuda_stream`.  Unit i is in_base[in_off[i] ..+ in_len[i]) and
+ * its frame goes to out_base[out_off[i] ..+ out_cap[i]), both at any alignment; the frame equals LZ4.compress(data:...)'s
+ * (swc_lz4_compress's) for the unit.  The options, the dictionary (device pointer, NULL = nil; an empty dictionary is a
+ * non-NULL pointer with dict_len 0; only its last 64 KiB is used) and the dictionary ID apply to the whole batch.
+ * block_size outside 1 ... 4 MiB returns SWC_ERR_REFERENCE_TRAP (:51) and enqueues nothing.  status[i]:
+ *   SWC_OK;
+ *   SWC_ERR_REFERENCE_TRAP from the unit's first failing block, as the reference traps in compress(block:_:): a non-empty
+ *     unit with a 1-3 byte dictionary, or a dependent frame of 1-3 byte blocks with more than one block (an empty unit is
+ *     header + EndMark (+ the content checksum of no bytes) and never traps);
+ *   SWC_ERR_OUTPUT_OVERFLOW when the frame is longer than out_cap[i]: out_len[i] is then the exact frame size, so one rerun
+ *     with that capacity gives the frame.  Bytes inside the region are unspecified (a unit's first blocks may be written
+ *     before its total is known); nothing outside it is written;
+ *   SWC_ERR_UNSUPPORTED when the unit's blocks do not fit in what is left of the block table; nothing is written.
+ * out_len[i] is the frame size on OK, the required size on overflow and 0 otherwise.
+ * swc_lz4_frame_compress_max_bytes is exact: 7 + 8 content_size + 4 has_dict_id + in_len + nb (4 + 4 block_checksums) + 4 +
+ * 4 content_checksum with nb = ceil(in_len / block_size), the size of a frame whose blocks are all stored; a capacity of
+ * that size never overflows (0 for an invalid block_size).
+ * max_blocks > 0 is the capacity of the block table (at most 2^32 - 1), filled with the units' ceil(in_len / block_size)
+ * blocks in unit order; with a caller scratch the call reads nothing back and allocates nothing, and its launches depend
+ * only on (n, max_blocks, scratch_bytes), so it can be captured in a CUDA graph.  max_blocks == 0 reads in_len back (one
+ * synchronisation) and counts the blocks.  scratch == NULL takes the library pool.  A scratch of
+ * swc_lz4_frame_compress_batch_scratch_bytes(n, max_blocks, ...) runs the batch in one slice; a smaller one runs it in
+ * slices of whole blocks with the same results; one that cannot hold the columns and one block is SWC_ERR_INVALID_ARG. */
+size_t  swc_lz4_frame_compress_max_bytes(uint64_t in_len, int64_t block_size, int32_t block_checksums,
+                                         int32_t content_checksum, int32_t content_size, int32_t has_dict_id);
+size_t  swc_lz4_frame_compress_batch_scratch_bytes(uint64_t n, uint64_t max_blocks, int64_t block_size,
+                                                   int32_t independent_blocks, uint64_t dict_len);
+int32_t swc_lz4_frame_compress_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                                     int32_t independent_blocks, int32_t block_checksums, int32_t content_checksum,
+                                     int32_t content_size, int64_t block_size,
+                                     const uint8_t *dict /* device, NULL = nil */, uint64_t dict_len,
+                                     int32_t has_dict_id, uint32_t dict_id,
+                                     uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                     uint64_t *out_len, int32_t *status, uint64_t n, uint64_t max_blocks,
                                      void *scratch, size_t scratch_bytes, void *cuda_stream);
 
 /* ---- Deflate compression ------------------------------------------------------------------------------------

@@ -76,6 +76,12 @@ def lib():
         L.swc_lz4_compress_batch_scratch_bytes.restype = C.c_size_t
         L.swc_lz4_compress_batch_scratch_bytes.argtypes = [C.c_uint64, C.c_uint64]
         L.swc_lz4_block_compress_batch.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, u64, vp, sz, vp]
+        L.swc_lz4_frame_compress_max_bytes.restype = C.c_size_t
+        L.swc_lz4_frame_compress_max_bytes.argtypes = [u64, C.c_int64, i32, i32, i32, i32]
+        L.swc_lz4_frame_compress_batch_scratch_bytes.restype = C.c_size_t
+        L.swc_lz4_frame_compress_batch_scratch_bytes.argtypes = [u64, u64, C.c_int64, i32, u64]
+        L.swc_lz4_frame_compress_batch.argtypes = [vp, vp, vp, i32, i32, i32, i32, C.c_int64, vp, u64, i32, u32, vp, vp, vp,
+                                                   vp, vp, u64, u64, vp, sz, vp]
         L.swc_deflate_compress.argtypes = [vp, sz, C.POINTER(vp), szp]
         L.swc_zlib_archive.argtypes = [vp, sz, C.POINTER(vp), szp]
         L.swc_gzip_archive.argtypes = [vp, sz, vp, C.POINTER(vp), szp]

@@ -188,6 +188,15 @@ class LZ4:
         return payload
 
     @staticmethod
+    def max_compressed_size(n, blockChecksums=False, contentChecksum=True, contentSize=False, blockSize=4 * 1024 * 1024,
+                            dictionaryID=None):
+        """the largest frame compress(...) writes for n bytes with these options: every block stored (0 for a blockSize
+        outside 1 ... 4 MiB)"""
+        return int(_lib.lib().swc_lz4_frame_compress_max_bytes(n, int(blockSize), int(bool(blockChecksums)),
+                                                                int(bool(contentChecksum)), int(bool(contentSize)),
+                                                                0 if dictionaryID is None else 1))
+
+    @staticmethod
     def decompress(data, dictionary=None, dictionaryID=None):
         args, _keep = _dict_args(dictionary, dictionaryID)
         return _single("swc_lz4_decompress", data, *args)[0]

@@ -18,6 +18,10 @@ def _align(v, a=16):
 # the most scratch a compress Batch allocates: past it the library runs the batch in slices that fit
 COMPRESS_SCRATCH_LIMIT = 16 << 30
 
+# the frame options of LZ4.compress(data:) (LZ4+Compress.swift:16-19), the defaults of an 'lz4_frame_compress' Batch
+LZ4_FRAME_DEFAULTS = dict(independentBlocks=True, blockChecksums=False, contentChecksum=True, contentSize=False)
+LZ4_FRAME_BLOCK_SIZE = 4 << 20
+
 
 def compress_scratch_bytes(codec, in_len, dict_len=None, block_size=1):
     """The scratch that runs a compress batch of units of `in_len` bytes in one slice, capped at COMPRESS_SCRATCH_LIMIT.
@@ -54,7 +58,7 @@ def pack_units(units, align=16):
 
 class Batch:
     """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'lzma2', 'gzip', 'zlib', 'xz',
-    'lz4_frame', 'lz4_block_compress', 'deflate_compress', 'bzip2_compress').
+    'lz4_frame', 'lz4_block_compress', 'lz4_frame_compress', 'deflate_compress', 'bzip2_compress').
 
     'gzip' / 'zlib' decode one archive per unit (GzipArchive.unarchive, GzipArchive.swift:38-47, 79-100 / ZlibArchive.unarchive,
     ZlibArchive.swift:25-42): the first member only, whose status, size and consumed bytes results() returns.  With
@@ -70,17 +74,23 @@ class Batch:
 
     'lz4_block_compress' compresses each unit into a raw LZ4 block (LZ4+Compress.swift:156-277); `aux` is then an optional
     (dict_off, dict_len) pair of u64 arrays placing each unit's dictionary window inside `in_buf`.
+    'lz4_frame_compress' compresses each unit into a whole LZ4 frame, as LZ4.compress(data:independentBlocks:blockChecksums:
+    contentChecksum:contentSize:blockSize:dictionary:dictionaryID:) (LZ4+Compress.swift:47-154) does: `frame_flags` takes
+    any of LZ4_FRAME_DEFAULTS' keys, `block_size` is the block size (default 4 MiB), `aux` the dictionary's bytes (None: nil)
+    and `dict_id` the dictionary ID (None: nil); every option applies to the whole batch.  api.LZ4.max_compressed_size
+    gives the output a unit may need.  `max_blocks` works as for 'lz4_frame' (None: the library counts the blocks first,
+    one synchronisation); results() gives 0 consumed bytes.
     'deflate_compress' compresses each unit into a raw Deflate stream (Deflate.compress, Deflate+Compress.swift:22-42); a
     unit of n bytes needs at most (9 n + 17) // 8 bytes of output.
     'bzip2_compress' compresses each unit into a complete .bz2 stream (BZip2.compress(data:blockSize:),
     BZip2+Compress.swift:44-74) with raw blocks of 80 000 x `block_size` bytes; api.BZip2.max_compressed_size gives the
     output a unit may need.
-    The three compress codecs pass a caller scratch of compress_scratch_bytes(...), which runs the batch in one slice up
-    to COMPRESS_SCRATCH_LIMIT; `scratch_bytes` caps it lower (the library then runs the batch in slices; a scratch that
+    The compress codecs pass a caller scratch that runs the batch in one slice (compress_scratch_bytes(...) for the raw
+    codecs) up to COMPRESS_SCRATCH_LIMIT; `scratch_bytes` caps it lower (the library then runs the batch in slices; a scratch that
     cannot hold the largest unit fails the run with SWC_ERR_INVALID_ARG)."""
 
-    def __init__(self, codec, in_buf, in_off, in_len, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=1,
-                 headers=False, dict_id=None, max_blocks=None):
+    def __init__(self, codec, in_buf, in_off, in_len, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=None,
+                 headers=False, dict_id=None, max_blocks=None, frame_flags=None):
         self.codec = codec
         self.device = torch.device(device)
         self.n = len(in_off)
@@ -103,7 +113,7 @@ class Batch:
         self.d_status = torch.full((self.n,), -1, dtype=torch.int32, device=self.device)
         self.d_scratch = None
         self.d_dict_off = self.d_dict_len = None
-        self.block_size = int(block_size)
+        self.block_size = int(block_size) if block_size is not None else LZ4_FRAME_BLOCK_SIZE if codec == "lz4_frame_compress" else 1
         self.dict_id, self.max_blocks = dict_id, 0 if max_blocks is None else int(max_blocks)
         if codec == "lz4_frame":
             # an empty dictionary is still a dictionary: one spare byte keeps its pointer non-null
@@ -113,6 +123,21 @@ class Batch:
                 nbytes = _lib.lib().swc_lz4_frame_batch_scratch_bytes(self.n, int(np.asarray(in_len, dtype=np.uint64).sum()),
                                                                      self.max_blocks)
                 self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        elif codec == "lz4_frame_compress":
+            unknown = set(frame_flags or {}) - set(LZ4_FRAME_DEFAULTS)
+            if unknown:
+                raise ValueError(f"unknown frame flags {sorted(unknown)}")
+            self.frame_flags = dict(LZ4_FRAME_DEFAULTS, **(frame_flags or {}))
+            self.dict_len = 0 if aux is None else len(aux)
+            self.d_aux = None if aux is None else t(np.frombuffer(bytes(aux) + b"\0", dtype=np.uint8).copy())
+            bs = self.block_size
+            lens = np.asarray(in_len, dtype=np.uint64)
+            blocks = self.max_blocks or (max(1, int(((lens + np.uint64(bs - 1)) // np.uint64(bs)).sum())) if bs >= 1 else 1)
+            nbytes = min(_lib.lib().swc_lz4_frame_compress_batch_scratch_bytes(
+                self.n, blocks, bs, int(bool(self.frame_flags["independentBlocks"])), self.dict_len), COMPRESS_SCRATCH_LIMIT)
+            if scratch_bytes is not None:
+                nbytes = min(nbytes, int(scratch_bytes))
+            self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         elif codec == "lz4_block_compress":
             self.d_aux = None
             if aux is not None:
@@ -136,10 +161,11 @@ class Batch:
             self.d_headers = torch.zeros(max(self.n, 1) * C.sizeof(_CGzipHeader), dtype=torch.uint8, device=self.device)
 
     @classmethod
-    def from_units(cls, codec, units, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=1, headers=False,
-                   dict_id=None, max_blocks=None):
+    def from_units(cls, codec, units, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=None, headers=False,
+                   dict_id=None, max_blocks=None, frame_flags=None):
         buf, offs, lens = pack_units(units)
-        return cls(codec, buf, offs, lens, out_cap, device, aux, scratch_bytes, block_size, headers, dict_id, max_blocks)
+        return cls(codec, buf, offs, lens, out_cap, device, aux, scratch_bytes, block_size, headers, dict_id, max_blocks,
+                   frame_flags)
 
     def run(self):
         L = _lib.lib()
@@ -179,6 +205,15 @@ class Batch:
                                                 opt(self.d_dict_len), p(self.d_out), p(self.d_out_off), p(self.d_out_cap),
                                                 p(self.d_out_len), p(self.d_status), self.n, p(self.d_scratch),
                                                 self.d_scratch.numel(), stream)
+        elif self.codec == "lz4_frame_compress":
+            fl = self.frame_flags
+            st = L.swc_lz4_frame_compress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), int(bool(fl["independentBlocks"])),
+                                                int(bool(fl["blockChecksums"])), int(bool(fl["contentChecksum"])),
+                                                int(bool(fl["contentSize"])), self.block_size,
+                                                None if self.d_aux is None else p(self.d_aux), self.dict_len,
+                                                self.dict_id is not None, self.dict_id or 0, p(self.d_out), p(self.d_out_off),
+                                                p(self.d_out_cap), p(self.d_out_len), p(self.d_status), self.n, self.max_blocks,
+                                                p(self.d_scratch), self.d_scratch.numel(), stream)
         elif self.codec == "deflate_compress":
             st = L.swc_deflate_compress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out), p(self.d_out_off),
                                               p(self.d_out_cap), p(self.d_out_len), p(self.d_status), self.n, p(self.d_scratch),
@@ -200,7 +235,7 @@ class Batch:
 
     def results(self):
         """-> (status int32[n], out_len int64[n], consumed int64[n]) on the host (synchronises).  consumed is in bits for
-        'deflate' and 'bzip2', in bytes for 'lzma2', 'gzip', 'zlib' and 'lz4_frame', and 0 for 'xz'."""
+        'deflate' and 'bzip2', in bytes for 'lzma2', 'gzip', 'zlib' and 'lz4_frame', and 0 for 'xz' and the compress codecs."""
         torch.cuda.synchronize(self.device)
         return self.d_status.cpu().numpy(), self.d_out_len.cpu().numpy(), self.d_consumed.cpu().numpy()
 

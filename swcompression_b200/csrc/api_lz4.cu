@@ -2,15 +2,15 @@
 // LZ4.decompress / LZ4.multiDecompress (reference Sources/LZ4/LZ4.swift:73-330).  Frame descriptors and block marks
 // are walked on the host (a few bytes per block); block decode, block checksums and the content checksum run on the
 // device.  Errors are reported in the order the reference's sequential loop would meet them.
-// The compress half (LZ4.compress, LZ4+Compress.swift:16-154) writes its frame the other way round: every block is
-// compressed on the device, the host lays out the frame from the compressed sizes, the device writes the payloads and
-// checksums in place, and the host adds the header, block marks and EndMark.
+// The compress half here is the raw block batch; frames (LZ4.compress, LZ4+Compress.swift:16-154) are laid out on the
+// device by lz4_frame_compress.cu.
 #include <cstring>
 #include <vector>
 #include "../../include/swcgpu.h"
 #include "compress_host.h"
 #include "lz4.cuh"
 #include "lz4_compress.cuh"
+#include "lz4_frame.cuh"
 
 using namespace swc;
 
@@ -18,17 +18,6 @@ namespace {
 
 inline uint64_t rd64(const uint8_t *p) { return (uint64_t)le32(p) | (uint64_t)le32(p + 4) << 32; }
 inline bool is_magic(uint32_t v) { return v == 0x184D2204u || v == 0x184C2102u || (v >= 0x184D2A50u && v <= 0x184D2A5Fu); }
-
-// xxHash32 of the <= 14-byte frame descriptor (framing, not payload) — XxHash32.swift:24-83 with n < 16
-uint32_t xxh32_descriptor(const uint8_t *p, size_t n) {
-    auto rotl = [](uint32_t v, int s) { return (v << s) | (v >> (32 - s)); };
-    uint32_t acc = 0x165667B1u + (uint32_t)n;
-    size_t i = 0;
-    for (; n - i >= 4; i += 4) acc = rotl(acc + le32(p + i) * 0xC2B2AE3Du, 17) * 0x27D4EB2Fu;
-    for (; n - i >= 1; i += 1) acc = rotl(acc + (uint32_t)p[i] * 0x165667B1u, 11) * 0x9E3779B1u;
-    acc ^= acc >> 15; acc *= 0x85EBCA77u; acc ^= acc >> 13; acc *= 0xC2B2AE3Du; acc ^= acc >> 16;
-    return acc;
-}
 
 struct Block { uint64_t off, len; bool stored; uint32_t stored_ck; bool has_ck; };
 
@@ -173,7 +162,7 @@ int frame(DeviceInput &dev, const uint8_t *p, size_t n_total, size_t pos, bool h
         uint32_t id = le32(in + off); off += 4;
         if (has_ext_id && ext_id != id) return SWC_DATA_CORRUPTED;
     }
-    const uint8_t hc = (uint8_t)((xxh32_descriptor(in, off) >> 8) & 0xFF);
+    const uint8_t hc = (uint8_t)((lz4f::xxh32_descriptor(in, (u32)off) >> 8) & 0xFF);
     if (hc != in[off]) return SWC_DATA_CORRUPTED;
     off++;
 
@@ -441,123 +430,6 @@ int32_t swc_lz4_block_compress_batch(const uint8_t *in_base, const uint64_t *in_
         int st = lz4c::parse(a, first, count, scr, (const u64 *)scr, s);
         return st ? st : lz4c::emit(a, first, count, scr, (const u64 *)scr, s);
     });
-}
-
-// LZ4.compress(data:independentBlocks:blockChecksums:contentChecksum:contentSize:blockSize:dictionary:dictionaryID:)
-// LZ4+Compress.swift:47-154
-int32_t swc_lz4_compress(const uint8_t *in, size_t in_len, int32_t independent_blocks, int32_t block_checksums,
-                         int32_t content_checksum, int32_t content_size, int64_t block_size,
-                         const uint8_t *dict, size_t dict_len, int32_t has_dict_id, uint32_t dict_id,
-                         uint8_t **out, size_t *out_len) {
-    if (!out || !out_len || (!in && in_len)) return SWC_ERR_INVALID_ARG;
-    *out = nullptr; *out_len = 0;
-    if (!(block_size <= (int64_t)lz4c::MAX_BLOCK && block_size > 0)) return SWC_ERR_REFERENCE_TRAP;     // :51
-    const u64 bs = (u64)block_size;
-    const u64 nb = (in_len + bs - 1) / bs;
-    const u64 D = dict ? (dict_len > lz4c::MAX_DICT ? lz4c::MAX_DICT : dict_len) : 0;                    // :95-101
-    // compress(block:_:) traps on a 1-3 byte dictionary (:283): the user's, or a short previous block (:106-110)
-    if (nb > 0 && D >= 1 && D <= 3) return SWC_ERR_REFERENCE_TRAP;
-    if (nb > 1 && !independent_blocks && bs <= 3) return SWC_ERR_REFERENCE_TRAP;
-    if (ensure_device()) return SWC_ERR_NO_DEVICE;
-    ApiLock api_lock;
-
-    uint8_t hdr[19];                                                                                     // :54-93
-    size_t h = 0;
-    hdr[h++] = 0x04; hdr[h++] = 0x22; hdr[h++] = 0x4D; hdr[h++] = 0x18;
-    hdr[h++] = (uint8_t)(0x40 | (independent_blocks ? 0x20 : 0) | (block_checksums ? 0x10 : 0) | (content_size ? 0x8 : 0) |
-                         (content_checksum ? 0x4 : 0) | (has_dict_id ? 0x1 : 0));
-    hdr[h++] = bs <= (64u << 10) ? 0x40 : bs <= (256u << 10) ? 0x50 : bs <= (1u << 20) ? 0x60 : 0x70;
-    if (content_size) for (int k = 0; k < 8; k++) hdr[h++] = (uint8_t)((uint64_t)in_len >> (8 * k));
-    if (has_dict_id) for (int k = 0; k < 4; k++) hdr[h++] = (uint8_t)(dict_id >> (8 * k));
-    hdr[h] = (uint8_t)((xxh32_descriptor(hdr + 4, h - 4) >> 8) & 0xFF);
-    h++;
-
-    int st;
-    // device input: the dictionary window, then the data
-    DevBuf d_in;
-    if ((st = d_in.alloc(D + in_len + 16))) return st;
-    if (D) SWC_CUDA_TRY(cudaMemcpy(d_in.p, dict + (dict_len - D), D, cudaMemcpyHostToDevice));
-    if (in_len) { int cst = copy_pageable(d_in.as<u8>() + D, in, in_len, true); if (cst) return cst; }
-
-    // per block: where it is read from and which window precedes it; after the parse, where its payload goes in the frame
-    UnitTable t;
-    const Col<u64> in_off = t.in<u64>(nb), in_len_c = t.in<u64>(nb), dict_off = t.in<u64>(nb), dict_len_c = t.in<u64>(nb);
-    const Col<u64> out_off = t.in<u64>(nb), out_cap = t.in<u64>(nb), scr_off = t.in<u64>(nb), pay_len_c = t.in<u64>(nb);
-    const Col<u8> stored_c = t.in<u8>(nb);
-    const Col<u64> res_len_c = t.out<u64>(nb);
-    const Col<int32_t> status_c = t.out<int32_t>(nb);
-    const Col<uint32_t> ck_c = t.out<uint32_t>(nb);
-    u64 *h_in_len = t.host(in_len_c), *h_dlen = t.host(dict_len_c), *pay_off = t.host(out_off), *pay_len = t.host(pay_len_c);
-    u8 *stored = t.host(stored_c);
-    u64 scr_total = 0;
-    for (u64 k = 0; k < nb; k++) {
-        const u64 o = k * bs, l = in_len - o < bs ? in_len - o : bs;
-        t.host(in_off)[k] = D + o; h_in_len[k] = l;
-        if (independent_blocks || k == 0) { t.host(dict_off)[k] = 0; h_dlen[k] = D; }                     // :105
-        else { const u64 pl = bs < lz4c::MAX_DICT ? bs : lz4c::MAX_DICT; t.host(dict_off)[k] = D + o - pl; h_dlen[k] = pl; }   // :106-110
-        pay_off[k] = 0; t.host(out_cap)[k] = ~0ull;
-        t.host(scr_off)[k] = scr_total;
-        scr_total += need_of(l, h_dlen[k]);
-    }
-    DevBuf d_scr;
-    if ((st = t.alloc())) return st;
-    if ((st = d_scr.alloc(scr_total + 256))) return st;
-    std::vector<uint64_t> res_len;
-    std::vector<int32_t> res_st;
-    std::vector<uint32_t> cks;
-    u64 frame_len = h;
-    lz4c::Args a;
-    if (nb) {
-        if ((st = t.upload())) return st;
-        a.in_base = d_in.as<u8>(); a.in_off = t.dev(in_off); a.in_len = t.dev(in_len_c);
-        a.dict_off = t.dev(dict_off); a.dict_len = t.dev(dict_len_c);
-        a.out_base = nullptr; a.out_off = t.dev(out_off); a.out_cap = t.dev(out_cap);
-        a.out_len = t.dev(res_len_c); a.status = t.dev(status_c); a.stored = nullptr; a.n = nb;
-        if ((st = lz4c::parse(a, 0, nb, d_scr.as<u8>(), t.dev(scr_off), 0))) return st;
-        if ((st = t.fetch(res_len_c, res_len)) || (st = t.fetch(status_c, res_st))) return st;
-        for (u64 k = 0; k < nb; k++) {
-            if (res_st[k] != SWC_OK) return res_st[k];
-            stored[k] = res_len[k] > h_in_len[k];                                                        // :112
-            pay_len[k] = stored[k] ? h_in_len[k] : res_len[k];
-            pay_off[k] = frame_len + 4;
-            frame_len += 4 + pay_len[k] + (block_checksums ? 4 : 0);
-        }
-    }
-    const u64 payload_end = frame_len;
-    frame_len += 4 + (content_checksum ? 4 : 0);                                                         // :143-151
-    DevBuf d_frame;
-    if ((st = d_frame.alloc(frame_len + 16))) return st;
-    if (nb) {
-        // the payloads go straight to their frame offsets; out_cap keeps the parse's "unbounded" fence
-        if ((st = t.upload())) return st;
-        a.out_base = d_frame.as<u8>(); a.stored = t.dev(stored_c);
-        if ((st = lz4c::emit(a, 0, nb, d_scr.as<u8>(), t.dev(scr_off), 0))) return st;
-        if (block_checksums) {                                                                           // :120-125, :133-138
-            if ((st = checks::xxh32_batch(d_frame.as<u8>(), a.out_off, t.dev(pay_len_c), t.dev(ck_c), nb, 0))) return st;
-            if ((st = t.fetch(ck_c, cks))) return st;
-        }
-    }
-    uint32_t content_ck = xxh32_descriptor(nullptr, 0);
-    if (content_checksum && in_len) {                                                                    // :146-151
-        u64 v = 0;
-        if ((st = checks::check_device(checks::XXH32, d_in.as<u8>() + D, in_len, &v))) return st;
-        content_ck = (uint32_t)v;
-    }
-    uint8_t *host = (uint8_t *)swc_alloc(frame_len);
-    if (!host) return SWC_ERR_OUTPUT_OVERFLOW;
-    if (payload_end > h) {
-        int cst = copy_pageable(host + h, d_frame.as<u8>() + h, payload_end - h, false);
-        if (cst) { swc_free(host); return cst; }
-    }
-    memcpy(host, hdr, h);
-    for (u64 k = 0; k < nb; k++) {                                                                       // :113-139
-        put_le32(host + pay_off[k] - 4, (stored[k] ? 0x80000000u : 0u) | (uint32_t)pay_len[k]);
-        if (block_checksums) put_le32(host + pay_off[k] + pay_len[k], cks[k]);
-    }
-    put_le32(host + payload_end, 0);
-    if (content_checksum) put_le32(host + payload_end + 4, content_ck);
-    *out = host; *out_len = frame_len;
-    return SWC_OK;
 }
 
 }  // extern "C"

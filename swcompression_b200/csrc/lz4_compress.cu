@@ -45,7 +45,8 @@ __device__ __forceinline__ Geo geo(const Args &a, u64 u) {
     const u64 l = a.in_len[u];
     u64 d = a.dict_off ? a.dict_len[u] : 0;
     g.blk = a.in_base + a.in_off[u];
-    g.dict = a.dict_off ? a.in_base + a.dict_off[u] + (d > MAX_DICT ? d - MAX_DICT : 0) : nullptr;
+    const u64 o = a.dict_off ? a.dict_off[u] : 0;
+    g.dict = a.dict_off ? (o & USER_DICT ? a.user_dict + (o - USER_DICT) : a.in_base + o) + (d > MAX_DICT ? d - MAX_DICT : 0) : nullptr;
     g.st = l > MAX_BLOCK ? SWC_ERR_UNSUPPORTED : (d >= 1 && d <= 3) ? SWC_ERR_REFERENCE_TRAP : SWC_OK;   // :283 traps
     if (d > MAX_DICT) d = MAX_DICT;
     g.d = (u32)d; g.l = g.st ? 0u : (u32)l; g.w = g.d + g.l;

@@ -19,28 +19,19 @@
 #include "checks.cuh"
 #include "host_util.h"
 #include "lz4.cuh"
+#include "lz4_frame.cuh"
 
 namespace swc {
 namespace {
 
 typedef swc_lz4_frame_info Info;
 enum : u32 { KIND_NONE = 0, KIND_INDEPENDENT = 1, KIND_DEPENDENT = 2, KIND_LEGACY = 3 };
-constexpr u32 FLG_DICT_ID = 0x01, FLG_CONTENT_CK = 0x04, FLG_CONTENT_SIZE = 0x08, FLG_BLOCK_CK = 0x10, FLG_INDEPENDENT = 0x20;
+using namespace lz4f;
 constexpr u32 UNPLACED = 0x10000;          // internal: the unit's blocks do not fit the block table or the record area
 constexpr u64 STORED = 1ull << 63;
 
 __device__ __forceinline__ u32 rd32(const u8 *p) { return (u32)p[0] | (u32)p[1] << 8 | (u32)p[2] << 16 | (u32)p[3] << 24; }
-__device__ __forceinline__ u32 rotl(u32 v, int s) { return __funnelshift_l(v, v, s); }
 __device__ __forceinline__ bool is_magic(u32 v) { return v == 0x184D2204u || v == 0x184C2102u || (v >= 0x184D2A50u && v <= 0x184D2A5Fu); }
-
-// xxHash32 of the <= 14-byte frame descriptor (XxHash32.swift:24-83 with n < 16)
-__device__ u32 xxh32_descriptor(const u8 *p, u32 n) {
-    u32 acc = 0x165667B1u + n, i = 0;
-    for (; n - i >= 4; i += 4) acc = rotl(acc + rd32(p + i) * 0xC2B2AE3Du, 17) * 0x27D4EB2Fu;
-    for (; i < n; i++) acc = rotl(acc + (u32)p[i] * 0x165667B1u, 11) * 0x9E3779B1u;
-    acc ^= acc >> 15; acc *= 0x85EBCA77u; acc ^= acc >> 13; acc *= 0xC2B2AE3Du; acc ^= acc >> 16;
-    return acc;
-}
 
 // the block columns of the batch, indexed by block; walk<FILL> writes them
 struct BlockCols {
