@@ -80,11 +80,11 @@ def run_batch(codec, k, in_buf, in_off, in_len, out_off, out_cap, out_total, scr
     return rc, d_st.cpu().numpy(), d_len.cpu().numpy(), d_out.cpu().numpy(), launches
 
 
-def fenced(codec, k, units, scratch=None):
-    """runs `units` packed hostile into fenced output regions and checks every result and the fence
-    -> (status, out_len, output buffer, kernel launches)"""
+def fenced(codec, k, units, scratch=None, exp=None):
+    """runs `units` packed hostile into fenced output regions and checks every result and the fence; `exp` are the
+    expected streams when the caller has them already -> (status, out_len, output buffer, kernel launches)"""
     from swcompression_b200.batch import compress_scratch_bytes
-    exp = expected(codec, k, units)
+    exp = expected(codec, k, units) if exp is None else exp
     in_buf, in_off, in_len = H.pack_hostile(units, random.Random(5))
     out_off, out_cap, total = H.fenced_layout([len(e) for e in exp], align=ALIGN[codec])
     if scratch is None:
