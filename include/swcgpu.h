@@ -72,6 +72,8 @@ int32_t swc_deflate_decompress_batch(const uint8_t *in_base, const uint64_t *in_
                                      uint64_t *out_len, uint64_t *consumed_bits, int32_t *status,
                                      uint64_t n, void *scratch, size_t scratch_bytes /* NULL,0 = library pool */,
                                      void *cuda_stream);
+/* Every Deflate decode (batched, single-stream, gzip / zlib / ZIP entries) produces at most 0xFFFFFFF0 bytes (4 GiB - 16)
+ * per unit: a stream that decodes to more reports SWC_ERR_UNSUPPORTED whatever its capacity (0 included). */
 int32_t swc_deflate_decompress_batch_host(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
                                           uint64_t in_total,
                                           uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,

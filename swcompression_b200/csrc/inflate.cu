@@ -93,22 +93,27 @@ lz_resolve_kernel(BatchArgs a) {
     const u32 *rec = a.rec_base + rec_start(off + a.out_cap[unit]);      // record k at rec - 1 - k
     const u8 *lits = (const u8 *)(a.rec_base + rec_start(off));
     const u32 ph = (u32)((uintptr_t)out & 15);
+    u8 *const outa = out - ph;       // 16-byte aligned: output chunk c starts at outa + 16 c
     const u32 M = RING - 1;
     u32 done = 0;          // output bytes placed by earlier batches
     u32 flushed = 0;       // output bytes written to global memory
     u32 lit = 0;           // literals consumed
     u32 g = 0;             // next record
     u32 part = 0;          // bytes of record g already placed (an escape longer than SPAN)
-    // writes output bytes [flushed, to) from the ring: whole aligned chunks as 16-byte stores, the rest byte by byte
+    // writes output bytes [flushed, to) from the ring: whole aligned chunks as 16-byte stores, the rest byte by byte.
+    // Positions are taken relative to the aligned base out - ph (output byte p is byte p + ph of it), where every value up
+    // to len + ph <= OUT_MAX + 15 fits a u32; only the first chunk starts before out[0], and its flushed + ph - cb >= ph
+    // keeps those bytes out of the copy.  The chunk end cb + 16 is never formed: it wraps for the output's last chunk.
     auto flush = [&](u32 to) {
-        const u32 c0 = (flushed + ph) >> 4, c1 = (to + ph + 15) >> 4;
+        const u32 q0 = flushed + ph, q1 = to + ph;
+        const u32 c0 = q0 >> 4, c1 = (q1 >> 4) + ((q1 & 15) != 0);
         for (u32 c = c0 + lane; c < c1; c += 32) {
-            const int cs = (int)(c * 16) - (int)ph;                     // chunk start as an output position
-            const u32 lo = cs < (int)flushed ? flushed : (u32)cs, hi = (u32)(cs + 16) < to ? (u32)(cs + 16) : to;
-            if ((int)lo == cs && hi == (u32)(cs + 16)) {
-                *(uint4 *)(out + cs) = *(const uint4 *)(S.ring + ((c * 16) & M));
+            const u32 cb = c * 16;                                      // chunk start relative to outa
+            const u32 lo = q0 > cb ? q0 - cb : 0u, hi = q1 - cb < 16 ? q1 - cb : 16u;   // bytes [lo, hi) of the chunk
+            if (lo == 0 && hi == 16) {
+                *(uint4 *)(outa + cb) = *(const uint4 *)(S.ring + (cb & M));
             } else {
-                for (u32 p = lo; p < hi; p++) out[p] = S.ring[(p + ph) & M];
+                for (u32 i = lo; i < hi; i++) outa[cb + i] = S.ring[(cb + i) & M];
             }
         }
         flushed = to;
@@ -171,8 +176,8 @@ lz_resolve_kernel(BatchArgs a) {
         for (u32 c = lane; c < nch; c += 32) cp_async16(S.buf + c * 16, lchunk + c * 16);
         const u32 msx = done + endx - mx.len, mqx = msx - mx.dist;      // the lane's matches: start, first source byte
         const u32 msy = done + end - my.len, mqy = msy - my.dist;
-        const bool farx = ix < k && mx.len != 0 && mqx + RING < bend;
-        const bool fary = iy < k && my.len != 0 && mqy + RING < bend;
+        const bool farx = ix < k && mx.len != 0 && bend - mqx > RING;  // mqx + RING would wrap near the 2^32 ceiling
+        const bool fary = iy < k && my.len != 0 && bend - mqy > RING;
         const u32 c0x = (mqx + ph) >> 4, c0y = (mqy + ph) >> 4;          // first source chunks (output chunk index)
         const u32 fchx = farx ? ((mqx + mx.len - 1 + ph) >> 4) - c0x + 1 : 0u;
         const u32 fchy = fary ? ((mqy + my.len - 1 + ph) >> 4) - c0y + 1 : 0u;
@@ -183,7 +188,6 @@ lz_resolve_kernel(BatchArgs a) {
             if (lane >= (u32)d) fend += v;
         }
         const u32 fbx = nch + fend - fchx - fchy, fby = fbx + fchx;      // first staging chunks of x and y
-        const u8 *outa = out - ph;                               // 16-byte aligned: output chunk c starts at outa + 16 c
         for (u32 c = 0; c < fchx + fchy; c++) {
             const u32 oc = c < fchx ? c0x + c : c0y + c - fchx;  // output chunk
             u8 *dst = S.buf + (fbx + c) * 16;

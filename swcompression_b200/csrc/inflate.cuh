@@ -46,6 +46,10 @@ void seat_scratch(BatchArgs &a, void *scratch, u64 n, u64 first, int tickets, in
 // bytes of the scratch region of a unit
 __device__ __forceinline__ u64 region_bytes(u64 out_off, u64 cap) { return (rec_start(out_off + cap) - rec_start(out_off)) * 4; }
 
+// The largest output a unit may decode to.  Positions in the Huffman stages and in K2 are 32-bit, and K2 works on them
+// plus the output's phase (< 16) without wrapping; a stream that would produce more fails with SWC_ERR_UNSUPPORTED.
+constexpr u32 OUT_MAX = 0xFFFFFFF0u;
+
 constexpr u32 REC_ESC = 0x8000u;       // also the padding record: an escape that skips nothing
 constexpr u32 REC_DIRECT = 0xFFFFFFFFu;  // rec_count of a unit whose output is already written
 

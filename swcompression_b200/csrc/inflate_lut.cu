@@ -344,6 +344,7 @@ __device__ __forceinline__ int begin_block(HeaderBits &hb, Emit &em, const LaneM
     if (const int st = hdr::block_start(hb, bc.is_last, btype)) return st;
     if (btype == 0) {
         if (const int st = hdr::stored_length(hb, length)) return st;
+        if ((u64)em.op + length > OUT_MAX) return SWC_ERR_UNSUPPORTED;
         const u8 *src = hb.sp.origin + (hb.pos >> 3);                                   // byte aligned here
         for (u32 i = 0; i < length; i++) em.stored_byte(__ldg(src + i));
         hb.skip(length * 8);
@@ -446,7 +447,7 @@ __device__ __forceinline__ int parked_step(Reader &br, Emit &em, const LaneMem &
     br.pos += db;
     if (br.pos > sp.end) return SWC_DEFLATE_SYMBOL_NOT_FOUND;
     if (dist > em.op) return SWC_ERR_REFERENCE_TRAP;                                     // :219 negative array index
-    if ((u64)em.op + length > 0xFFFFFFF0ull) return SWC_ERR_UNSUPPORTED;
+    if ((u64)em.op + length > OUT_MAX) return SWC_ERR_UNSUPPORTED;
     em.match(length, dist);
     state = ST_SYMBOLS;
     return SWC_OK;
@@ -491,6 +492,7 @@ inflate_lut_kernel(BatchArgs a) {
     for (;;) {
         if (state == ST_DONE && have_unit) {                                             // retire the finished unit
             const bool fits = em.finish(region_bytes(a.out_off[unit], cap64));
+            if (status == SWC_OK && em.op > OUT_MAX) status = SWC_ERR_UNSUPPORTED;
             if (status == SWC_OK && (u64)em.op > cap64) status = SWC_ERR_OUTPUT_OVERFLOW;
             if (status == SWC_OK && !fits) status = SWC_INTERNAL_NEEDS_SLOW;
             a.consumed[unit] = br.pos - sp.pos0;
@@ -530,7 +532,7 @@ inflate_lut_kernel(BatchArgs a) {
                         cap64 = a.out_cap[unit];
                         em.lits = (u8 *)(a.rec_base + rec_start(a.out_off[unit]));
                         em.rec = a.rec_base + rec_start(a.out_off[unit] + cap64);
-                        em.cap = cap64 > 0xFFFFFFF0ull ? 0xFFFFFFF0u : (u32)cap64;
+                        em.cap = cap64 > OUT_MAX ? OUT_MAX : (u32)cap64;
                         em.op = 0; em.nlit = 0; em.last_end = 0; em.nrec = 0; em.acc_lo = em.acc_hi = 0;
                         const u32 bitskip = a.start_bits ? a.start_bits[unit] : 0;
                         sp.ubeg = a.in_base + a.in_off[unit];
@@ -551,6 +553,9 @@ inflate_lut_kernel(BatchArgs a) {
         if (state == ST_SYMBOLS) {
             br.topup(ring, sp);
             if (br.pos > sp.end) { status = SWC_DEFLATE_SYMBOL_NOT_FOUND; state = ST_DONE; }
+            // literals are not bounded one by one: a round adds at most KLIT + 1 of them, so em.op <= OUT_MAX at the
+            // start of every round keeps the u32 from wrapping
+            else if (em.op > OUT_MAX) { status = SWC_ERR_UNSUPPORTED; state = ST_DONE; }
         }
         // ---- fast: table lookups; a lane leaves the loop at its first non-literal ----
         u32 f_lo = 0, f_hi = 0;

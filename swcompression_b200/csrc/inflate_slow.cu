@@ -138,6 +138,7 @@ __global__ void __launch_bounds__(64) inflate_slow_kernel(BatchArgs a) {
 done:
 #undef FAIL
 #undef TRY
+    if (status == SWC_OK && op > OUT_MAX) status = SWC_ERR_UNSUPPORTED;            // the Huffman stages' limit (inflate.cuh)
     if (status == SWC_OK && op > cap) status = SWC_ERR_OUTPUT_OVERFLOW;
     a.out_len[unit] = op;
     a.consumed[unit] = r.pos - skip;

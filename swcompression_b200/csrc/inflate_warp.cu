@@ -156,7 +156,7 @@ __device__ __forceinline__ int window_match(const Smem &S, const Tables &T, cons
     c.skip(db); p += (u32)db;
     if (EMIT) {
         if (dist > em->op) return SWC_ERR_REFERENCE_TRAP;                  // Deflate.swift:219 negative array index
-        if ((u64)em->op + length > 0xFFFFFFF0ull) return SWC_ERR_UNSUPPORTED;
+        if ((u64)em->op + length > OUT_MAX) return SWC_ERR_UNSUPPORTED;
         em->match(length, dist);
     }
     length_out = length;
@@ -261,7 +261,7 @@ inflate_warp_kernel(BatchArgs a) {
 
         const u64 in_len = a.in_len[unit];
         const u64 cap64 = a.out_cap[unit];
-        const u32 cap = cap64 > 0xFFFFFFF0ull ? 0xFFFFFFF0u : (u32)cap64;
+        const u32 cap = cap64 > OUT_MAX ? OUT_MAX : (u32)cap64;
         u8 *lits = (u8 *)(a.rec_base + rec_start(a.out_off[unit]));
         u32 *rec = a.rec_base + rec_start(a.out_off[unit] + cap64);
         const u32 bitskip = a.start_bits ? a.start_bits[unit] : 0;
@@ -293,7 +293,7 @@ inflate_warp_kernel(BatchArgs a) {
                 u32 length;
                 TRY(hdr::stored_length(st, length));
                 const u8 *src = (const u8 *)st.wbase + ((st.pos + st.bit0) >> 3);
-                if (op + length > 0xFFFFFFF0ull) FAIL(SWC_ERR_UNSUPPORTED);
+                if (op + length > OUT_MAX) FAIL(SWC_ERR_UNSUPPORTED);
                 if (op + length <= cap) for (u32 i = lane; i < length; i += 32) lits[nlit + i] = src[i];
                 op += length; nlit += length; run_carry += length;
                 st.pos += (u64)length * 8;
@@ -461,7 +461,7 @@ inflate_warp_kernel(BatchArgs a) {
                     if (lane >= (u32)d) { ib += vb; il += vl; ir += vr; }
                 }
                 const u32 tot_b = __shfl_sync(SWC_FULL, ib, 31), tot_l = __shfl_sync(SWC_FULL, il, 31), tot_r = __shfl_sync(SWC_FULL, ir, 31);
-                if (op + tot_b > 0xFFFFFFF0ull) FAIL(SWC_ERR_UNSUPPORTED);
+                if (op + tot_b > OUT_MAX) FAIL(SWC_ERR_UNSUPPORTED);
                 // pass B: emit
                 int my_err = 0;
                 {
