@@ -254,6 +254,39 @@ int32_t swc_deflate_compress_batch(const uint8_t *in_base, const uint64_t *in_of
                                    uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
                                    uint64_t *out_len, int32_t *status, uint64_t n,
                                    void *scratch, size_t scratch_bytes, void *cuda_stream);
+/* GzipArchive.archive's header for `options`: the bytes swc_gzip_archive writes before the Deflate stream (FHCRC
+ * included).  Host only, needs no device.  *len = the header's size; if cap < *len nothing is written and
+ * SWC_ERR_OUTPUT_OVERFLOW is returned (buf may be NULL with cap 0).  XLEN > 65 535 -> SWC_GZIP_CANNOT_ENCODE_ISO_LATIN1,
+ * as swc_gzip_archive. */
+int32_t swc_gzip_archive_header(const swc_gzip_options *options, uint8_t *buf, size_t cap, size_t *len);
+/* the largest archive of in_len bytes: header_len + (9 in_len + 17) / 8 + 8 (gzip), 2 + (9 in_len + 17) / 8 + 4 (zlib) */
+size_t  swc_gzip_archive_max_bytes(uint64_t in_len, uint64_t header_len);
+size_t  swc_zlib_archive_max_bytes(uint64_t in_len);
+/* Whole gzip members / zlib streams, device memory, asynchronous on `cuda_stream`.  Unit i compresses
+ * in_base[in_off[i] ..+ in_len[i]) into out_base[out_off[i] ..+ out_cap[i]); input and output at any alignment.
+ *   gzip: header i (hdr_base[hdr_off[i] ..+ hdr_len[i]), device memory, written as given), the Deflate.compress stream,
+ *         then CRC-32 and ISIZE little-endian.  A batch that shares one header passes all-zero offsets.
+ *   zlib: 78 DA, the stream, then the big-endian Adler-32 (1 for an empty unit).
+ * With a header from swc_gzip_archive_header the result equals swc_gzip_archive / swc_zlib_archive's, byte for byte.
+ * status[i] / out_len[i]: SWC_OK / the archive's size; SWC_ERR_OUTPUT_OVERFLOW / the exact archive size (nothing
+ * written; one rerun with that capacity succeeds); SWC_ERR_UNSUPPORTED / 0 (in_len[i] >= 4 GiB, or the unit does not fit
+ * in max_in_bytes; nothing written).  Nothing outside [out_off[i], out_off[i] + out_len[i]) is ever written.
+ * max_in_bytes > 0: units are taken in order while the exclusive prefix sum of in_len plus the unit's own length is at
+ * most max_in_bytes.  With a caller scratch of at least swc_archive_compress_batch_scratch_bytes(n, max_in_bytes) the
+ * call reads nothing back and allocates nothing, and its launches and grids depend only on (n, max_in_bytes,
+ * scratch_bytes): it can be captured in a CUDA graph.  A smaller caller scratch is SWC_ERR_INVALID_ARG.
+ * max_in_bytes == 0: in_len is read back (one synchronisation) and the batch runs in slices of the scratch, which may be
+ * NULL (library pool); a caller scratch must then hold the largest unit, else SWC_ERR_INVALID_ARG. */
+size_t  swc_archive_compress_batch_scratch_bytes(uint64_t n, uint64_t max_in_bytes);
+int32_t swc_gzip_archive_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                               const uint8_t *hdr_base, const uint64_t *hdr_off, const uint64_t *hdr_len,
+                               uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                               uint64_t *out_len, int32_t *status, uint64_t n, uint64_t max_in_bytes,
+                               void *scratch, size_t scratch_bytes, void *cuda_stream);
+int32_t swc_zlib_archive_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                               uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                               uint64_t *out_len, int32_t *status, uint64_t n, uint64_t max_in_bytes,
+                               void *scratch, size_t scratch_bytes, void *cuda_stream);
 
 /* ---- BZip2 compression ---------------------------------------------------------------------------------------
  * BZip2.compress(data:) / compress(data:blockSize:)   Sources/BZip2/BZip2+Compress.swift:19-74

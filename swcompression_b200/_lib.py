@@ -88,6 +88,15 @@ def lib():
         L.swc_deflate_compress_batch_scratch_bytes.restype = C.c_size_t
         L.swc_deflate_compress_batch_scratch_bytes.argtypes = [C.c_uint64, C.c_uint64]
         L.swc_deflate_compress_batch.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, u64, vp, sz, vp]
+        L.swc_gzip_archive_header.argtypes = [vp, vp, sz, szp]
+        L.swc_gzip_archive_max_bytes.restype = C.c_size_t
+        L.swc_gzip_archive_max_bytes.argtypes = [u64, u64]
+        L.swc_zlib_archive_max_bytes.restype = C.c_size_t
+        L.swc_zlib_archive_max_bytes.argtypes = [u64]
+        L.swc_archive_compress_batch_scratch_bytes.restype = C.c_size_t
+        L.swc_archive_compress_batch_scratch_bytes.argtypes = [u64, u64]
+        L.swc_gzip_archive_batch.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, u64, u64, vp, sz, vp]
+        L.swc_zlib_archive_batch.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, u64, u64, vp, sz, vp]
         L.swc_bzip2_compress.argtypes = [vp, sz, i32, C.POINTER(vp), szp]
         L.swc_bzip2_compress_max_bytes.restype = C.c_size_t
         L.swc_bzip2_compress_max_bytes.argtypes = [C.c_uint64, i32]

@@ -286,6 +286,37 @@ class ZlibHeader:
         self.windowSize = h.window_size
 
 
+def _gzip_options(comment=None, fileName=None, writeHeaderCRC=False, isTextFile=False, osType=None, modificationTime=None,
+                  extraFields=()):
+    """GzipArchive.archive's keyword options -> (swc_gzip_options, the buffers it points into)"""
+    # the reference encodes the comment first, then the file name (:130-157); both fail the same way
+    c = None if comment is None else _latin1(comment)
+    f = None if fileName is None else _latin1(fileName)
+    o = _CGzipOptions()
+    keep = []
+    for text, ptr, ln in ((f, "file_name", "file_name_len"), (c, "comment", "comment_len")):
+        if text is not None:
+            b = C.create_string_buffer(text, len(text))
+            keep.append(b)
+            setattr(o, ptr, C.cast(b, C.c_void_p))
+            setattr(o, ln, len(text))
+    o.write_header_crc, o.is_text_file = int(bool(writeHeaderCRC)), int(bool(isTextFile))
+    if modificationTime is not None:
+        t = modificationTime.timestamp() if isinstance(modificationTime, datetime.datetime) else modificationTime
+        o.has_mtime, o.mtime = 1, int(t)                 # Int(timeIntervalSince1970) truncates toward zero
+    o.os_type = 255 if osType is None else _OS_BYTES.get(osType, 255)
+    fields = list(extraFields)
+    if fields:
+        ids = (C.c_uint8 * (2 * len(fields)))(*[v for e in fields for v in (e.si1, e.si2)])
+        lens = (C.c_uint64 * len(fields))(*[len(e.bytes) for e in fields])
+        blob = b"".join(bytes(e.bytes) for e in fields)
+        bb = C.create_string_buffer(blob, max(len(blob), 1))
+        keep += [ids, lens, bb]
+        o.n_extra, o.extra_ids, o.extra_lens = len(fields), C.cast(ids, C.c_void_p), C.cast(lens, C.c_void_p)
+        o.extra_bytes = C.cast(bb, C.c_void_p)
+    return o, keep
+
+
 class GzipArchive:
     """Sources/GZip/GzipArchive.swift:10-241"""
 
@@ -296,32 +327,27 @@ class GzipArchive:
         osType is a FileSystemType name ("fat", "unix", "macintosh", "ntfs", "other") or None; modificationTime a
         datetime or seconds since 1970.  Text that is not ISO-Latin-1, and extra fields whose XLEN exceeds 65 535, raise
         GzipError.cannotEncodeISOLatin1 as the reference throws."""
-        # the reference encodes the comment first, then the file name (:130-157); both fail the same way
-        c = None if comment is None else _latin1(comment)
-        f = None if fileName is None else _latin1(fileName)
-        o = _CGzipOptions()
-        keep = []
-        for text, ptr, ln in ((f, "file_name", "file_name_len"), (c, "comment", "comment_len")):
-            if text is not None:
-                b = C.create_string_buffer(text, len(text))
-                keep.append(b)
-                setattr(o, ptr, C.cast(b, C.c_void_p))
-                setattr(o, ln, len(text))
-        o.write_header_crc, o.is_text_file = int(bool(writeHeaderCRC)), int(bool(isTextFile))
-        if modificationTime is not None:
-            t = modificationTime.timestamp() if isinstance(modificationTime, datetime.datetime) else modificationTime
-            o.has_mtime, o.mtime = 1, int(t)                 # Int(timeIntervalSince1970) truncates toward zero
-        o.os_type = 255 if osType is None else _OS_BYTES.get(osType, 255)
-        fields = list(extraFields)
-        if fields:
-            ids = (C.c_uint8 * (2 * len(fields)))(*[v for e in fields for v in (e.si1, e.si2)])
-            lens = (C.c_uint64 * len(fields))(*[len(e.bytes) for e in fields])
-            blob = b"".join(bytes(e.bytes) for e in fields)
-            bb = C.create_string_buffer(blob, max(len(blob), 1))
-            keep += [ids, lens, bb]
-            o.n_extra, o.extra_ids, o.extra_lens = len(fields), C.cast(ids, C.c_void_p), C.cast(lens, C.c_void_p)
-            o.extra_bytes = C.cast(bb, C.c_void_p)
+        o, _keep = _gzip_options(comment, fileName, writeHeaderCRC, isTextFile, osType, modificationTime, extraFields)
         return _compressed("swc_gzip_archive", data, C.byref(o))
+
+    @staticmethod
+    def archive_header(**options):
+        """the header archive(data, **options) writes before the Deflate stream (FHCRC included), as bytes: the
+        per-unit header of a 'gzip_archive' Batch"""
+        o, _keep = _gzip_options(**options)
+        L = _lib.lib()
+        n = C.c_size_t(0)
+        st = L.swc_gzip_archive_header(C.byref(o), None, 0, C.byref(n))
+        if st not in (0, 1):                                 # 1: SWC_ERR_OUTPUT_OVERFLOW, the size is in n
+            raise error_for(st, None)
+        buf = C.create_string_buffer(max(n.value, 1))
+        check(L.swc_gzip_archive_header(C.byref(o), buf, n.value, C.byref(n)))
+        return buf.raw[:n.value]
+
+    @staticmethod
+    def max_archive_size(n, **options):
+        """the largest archive archive(data, **options) writes for n bytes of data"""
+        return int(_lib.lib().swc_gzip_archive_max_bytes(n, len(GzipArchive.archive_header(**options))))
 
     @dataclass
     class Member:
@@ -360,6 +386,11 @@ class ZlibArchive:
     def archive(data):
         """ZlibArchive.archive(data:): 78 DA, the Deflate.compress stream, the big-endian Adler-32."""
         return _compressed("swc_zlib_archive", data)
+
+    @staticmethod
+    def max_archive_size(n):
+        """the largest archive archive(data) writes for n bytes of data"""
+        return int(_lib.lib().swc_zlib_archive_max_bytes(n))
 
     @staticmethod
     def unarchive(archive):

@@ -37,6 +37,8 @@ def compress_scratch_bytes(codec, in_len, dict_len=None, block_size=1):
         nbytes = L.swc_deflate_compress_batch_scratch_bytes(n, total)
     elif codec == "bzip2_compress":
         nbytes = L.swc_bzip2_compress_batch_scratch_bytes(n, total, max(1, min(9, int(block_size))))
+    elif codec in ("gzip_archive", "zlib_archive"):
+        nbytes = L.swc_archive_compress_batch_scratch_bytes(n, total)
     else:
         raise ValueError(codec)
     return min(nbytes, COMPRESS_SCRATCH_LIMIT)
@@ -58,7 +60,8 @@ def pack_units(units, align=16):
 
 class Batch:
     """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'lzma2', 'gzip', 'zlib', 'xz',
-    'lz4_frame', 'lz4_block_compress', 'lz4_frame_compress', 'deflate_compress', 'bzip2_compress').
+    'lz4_frame', 'lz4_block_compress', 'lz4_frame_compress', 'deflate_compress', 'gzip_archive', 'zlib_archive',
+    'bzip2_compress').
 
     'gzip' / 'zlib' decode one archive per unit (GzipArchive.unarchive, GzipArchive.swift:38-47, 79-100 / ZlibArchive.unarchive,
     ZlibArchive.swift:25-42): the first member only, whose status, size and consumed bytes results() returns.  With
@@ -82,6 +85,13 @@ class Batch:
     one synchronisation); results() gives 0 consumed bytes.
     'deflate_compress' compresses each unit into a raw Deflate stream (Deflate.compress, Deflate+Compress.swift:22-42); a
     unit of n bytes needs at most (9 n + 17) // 8 bytes of output.
+    'gzip_archive' / 'zlib_archive' compress each unit into a whole gzip member / zlib stream, as GzipArchive.archive
+    (GzipArchive.swift:126-241) / ZlibArchive.archive (ZlibArchive.swift:54-70) do.  `gzip_options` is one dict of
+    GzipArchive.archive's keywords for the whole batch, or a list of n of them (identical headers are uploaded once);
+    api.GzipArchive.max_archive_size / api.ZlibArchive.max_archive_size give the output a unit may need.
+    `max_in_bytes` bounds the batch's input: the batch owns a scratch sized for it and run() reads nothing back (it can be
+    captured in a CUDA graph); units past the bound report SWC_ERR_UNSUPPORTED.  None lets the library read the lengths
+    back first (one synchronisation) and run in slices of the scratch.
     'bzip2_compress' compresses each unit into a complete .bz2 stream (BZip2.compress(data:blockSize:),
     BZip2+Compress.swift:44-74) with raw blocks of 80 000 x `block_size` bytes; api.BZip2.max_compressed_size gives the
     output a unit may need.
@@ -90,7 +100,7 @@ class Batch:
     cannot hold the largest unit fails the run with SWC_ERR_INVALID_ARG)."""
 
     def __init__(self, codec, in_buf, in_off, in_len, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=None,
-                 headers=False, dict_id=None, max_blocks=None, frame_flags=None):
+                 headers=False, dict_id=None, max_blocks=None, frame_flags=None, gzip_options=None, max_in_bytes=None):
         self.codec = codec
         self.device = torch.device(device)
         self.n = len(in_off)
@@ -144,7 +154,29 @@ class Batch:
                 self.d_dict_off, self.d_dict_len = t(np.asarray(aux[0], dtype=np.uint64)), t(np.asarray(aux[1], dtype=np.uint64))
         else:
             self.d_aux = None if aux is None else torch.from_numpy(np.frombuffer(bytes(aux), dtype=np.uint8).copy()).to(self.device)
-        if codec in ("lz4_block_compress", "deflate_compress", "bzip2_compress"):
+        self.max_in_bytes = 0 if max_in_bytes is None else int(max_in_bytes)
+        if codec == "gzip_archive":
+            from .api import GzipArchive
+            opts = gzip_options if isinstance(gzip_options, (list, tuple)) else [gzip_options or {}] * self.n
+            if len(opts) != self.n:
+                raise ValueError(f"gzip_options has {len(opts)} entries for {self.n} units")
+            # each distinct header once, back to back
+            blob, at, hdr_off, hdr_len = bytearray(), {}, np.zeros(self.n, dtype=np.uint64), np.zeros(self.n, dtype=np.uint64)
+            for i, o in enumerate(opts):
+                h = GzipArchive.archive_header(**o)
+                if h not in at:
+                    at[h] = len(blob)
+                    blob += h
+                hdr_off[i], hdr_len[i] = at[h], len(h)
+            self.headers = [bytes(blob[int(o):int(o) + int(ln)]) for o, ln in zip(hdr_off, hdr_len)]
+            self.d_hdr = t(np.frombuffer(bytes(blob) + b"\0", dtype=np.uint8).copy())
+            self.d_hdr_off, self.d_hdr_len = t(hdr_off), t(hdr_len)
+        if codec in ("gzip_archive", "zlib_archive") and self.max_in_bytes:
+            nbytes = _lib.lib().swc_archive_compress_batch_scratch_bytes(self.n, self.max_in_bytes)
+            if scratch_bytes is not None:
+                nbytes = min(nbytes, int(scratch_bytes))
+            self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        elif codec in ("lz4_block_compress", "deflate_compress", "bzip2_compress", "gzip_archive", "zlib_archive"):
             nbytes = compress_scratch_bytes(codec, in_len, None if aux is None else aux[1], self.block_size)
             if scratch_bytes is not None:
                 nbytes = min(nbytes, int(scratch_bytes))
@@ -162,10 +194,10 @@ class Batch:
 
     @classmethod
     def from_units(cls, codec, units, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=None, headers=False,
-                   dict_id=None, max_blocks=None, frame_flags=None):
+                   dict_id=None, max_blocks=None, frame_flags=None, gzip_options=None, max_in_bytes=None):
         buf, offs, lens = pack_units(units)
         return cls(codec, buf, offs, lens, out_cap, device, aux, scratch_bytes, block_size, headers, dict_id, max_blocks,
-                   frame_flags)
+                   frame_flags, gzip_options, max_in_bytes)
 
     def run(self):
         L = _lib.lib()
@@ -218,6 +250,15 @@ class Batch:
             st = L.swc_deflate_compress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out), p(self.d_out_off),
                                               p(self.d_out_cap), p(self.d_out_len), p(self.d_status), self.n, p(self.d_scratch),
                                               self.d_scratch.numel(), stream)
+        elif self.codec == "gzip_archive":
+            st = L.swc_gzip_archive_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_hdr), p(self.d_hdr_off),
+                                          p(self.d_hdr_len), p(self.d_out), p(self.d_out_off), p(self.d_out_cap), p(self.d_out_len),
+                                          p(self.d_status), self.n, self.max_in_bytes, p(self.d_scratch), self.d_scratch.numel(),
+                                          stream)
+        elif self.codec == "zlib_archive":
+            st = L.swc_zlib_archive_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out), p(self.d_out_off),
+                                          p(self.d_out_cap), p(self.d_out_len), p(self.d_status), self.n, self.max_in_bytes,
+                                          p(self.d_scratch), self.d_scratch.numel(), stream)
         elif self.codec == "bzip2_compress":
             st = L.swc_bzip2_compress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), self.block_size, p(self.d_out),
                                             p(self.d_out_off), p(self.d_out_cap), p(self.d_out_len), p(self.d_status), self.n,

@@ -48,17 +48,12 @@ int run_in_slices(u64 n, Need need, Head head, void *scratch, size_t scratch_byt
     return SWC_OK;
 }
 
-struct NoTail { void operator()(uint8_t *, uint32_t) const {} };
-
 // The single call of a batched compressor: in[0, in_len) goes through batch() as a 1-unit batch on the library pool, into
-// an output of `cap` bytes (the largest stream the codec writes for in_len bytes).  `a` carries the codec's own fields;
-// the unit table is filled here.  The result is handed back as one swc_alloc'ed buffer: `head`, the stream, then
-// tail_len bytes written by tail(p, check), where `check` is the device checksum `kind` of the input (computed only when
-// there is a tail; for an empty input it is 1 for Adler-32 and 0 otherwise).
-template <typename Args, typename Tail = NoTail>
+// an output of `cap` bytes (the largest result the codec writes for in_len bytes).  `a` carries the codec's own fields;
+// the unit table is filled here.  The result is handed back as one swc_alloc'ed buffer.
+template <typename Args>
 int compress_one(Args a, int (*batch)(const Args &, const std::vector<u64> &, void *, size_t, cudaStream_t), u64 cap,
-                 const uint8_t *in, size_t in_len, uint8_t **out, size_t *out_len, const std::vector<uint8_t> &head = {},
-                 checks::Kind kind = checks::CRC32, size_t tail_len = 0, Tail tail = {}) {
+                 const uint8_t *in, size_t in_len, uint8_t **out, size_t *out_len) {
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
     DevBuf d_in, d_out;
@@ -80,15 +75,11 @@ int compress_one(Args a, int (*batch)(const Args &, const std::vector<u64> &, vo
     std::vector<int32_t> status;
     if ((st = t.fetch(r_len, len)) || (st = t.fetch(r_st, status))) return st;
     if (status[0] != SWC_OK) return status[0];
-    u64 check = kind == checks::ADLER32 ? 1 : 0;
-    if (tail_len && in_len && (st = checks::check_device(kind, d_in.as<u8>(), in_len, &check))) return st;
-    const size_t n = (size_t)len[0], total = head.size() + n + tail_len;
-    uint8_t *host = (uint8_t *)swc_alloc(total);
+    const size_t n = (size_t)len[0];
+    uint8_t *host = (uint8_t *)swc_alloc(n);
     if (!host) return SWC_ERR_OUTPUT_OVERFLOW;
-    if (!head.empty()) memcpy(host, head.data(), head.size());
-    if (n && (st = copy_pageable(host + head.size(), d_out.p, n, false))) { swc_free(host); return st; }
-    tail(host + head.size() + n, (uint32_t)check);
-    *out = host; *out_len = total;
+    if (n && (st = copy_pageable(host, d_out.p, n, false))) { swc_free(host); return st; }
+    *out = host; *out_len = n;
     return SWC_OK;
 }
 

@@ -29,12 +29,8 @@ namespace {
 constexpr u32 EMPTY = 0xFFFFFFFFu;
 constexpr int HBITS = 12;                       // 4096 buckets: 16 KiB of shared memory per warp, 2 warps per CTA
 
-__host__ __device__ __forceinline__ u64 a256(u64 v) { return (v + 255) & ~(u64)255; }
-__host__ __device__ __forceinline__ u64 keyed(u64 n) { return n >= 3 ? n - 2 : 0; }       // positions with a full key
-__host__ __device__ __forceinline__ u64 tiles_of(u64 n) { return n >= MAX_UNIT ? 0 : (keyed(n) + TILE - 1) / TILE; }
-__host__ __device__ __forceinline__ u64 chunks_of(u64 n) { return n >= MAX_UNIT ? 0 : n ? (n + CHUNK - 1) / CHUNK : 1; }
-
 struct Checkpoint { u32 rec, off, pos, pad; u64 bit; };   // first symbol at or after the chunk's first byte
+static_assert(sizeof(Checkpoint) == CHECKPOINT_BYTES, "unit_scratch counts checkpoints of this size");
 
 // ---- the link builder (a template over key width and reach, so other LZ77 parses can share it) ----
 
@@ -105,27 +101,20 @@ __device__ __forceinline__ void build_links(const u8 *src, u32 t0, u32 t1, u16 *
 }
 
 typedef Keying<3>::Entry Entry3;
+static_assert(sizeof(Entry3) == CHAIN_ENTRY_BYTES, "unit_scratch counts chain entries of this size");
 
 // scratch of one unit: header | link (u16 per keyed position) | visited bitmap | checkpoints | seam words |
 // link-builder chains, later reused for the records
 struct Scr {
     u64 *hdr;                 // [0] records, [1] stream bits including the end-of-block code, [2] stored
     u16 *link; u32 *vis; Checkpoint *cp; u32 *seam; u8 *big;
-    __host__ __device__ __forceinline__ static u64 chain_entries(u64 n) {
-        const u64 t = tiles_of(n);
-        return t ? keyed(n) + (t - 1) * REACH : 0;
-    }
-    __host__ __device__ __forceinline__ static u64 big_bytes(u64 n) {
-        const u64 c = sizeof(Entry3) * chain_entries(n), r = 8 * (n / 3 + 2);
-        return c > r ? c : r;
-    }
     __device__ __forceinline__ Scr(u8 *base, u64 n) {
         hdr = (u64 *)base;
         link = (u16 *)(base + 256);
         vis = (u32 *)((u8 *)link + a256(2 * keyed(n)));
         cp = (Checkpoint *)((u8 *)vis + a256(4 * ((keyed(n) + 31) / 32)));
-        seam = (u32 *)((u8 *)cp + a256(sizeof(Checkpoint) * (chunks_of(n) + 1)));
-        big = (u8 *)seam + a256(8 * chunks_of(n));
+        seam = (u32 *)((u8 *)cp + a256(sizeof(Checkpoint) * (unit_chunks(n) + 1)));
+        big = (u8 *)seam + a256(8 * unit_chunks(n));
     }
     __device__ __forceinline__ u64 *rec() const { return (u64 *)big; }
 };
@@ -200,7 +189,7 @@ __device__ __forceinline__ u64 chunk_end(const Scr &s, u32 c, u32 nch) { return 
 __global__ void __launch_bounds__(64) link_kernel(Args a, u64 first, u64 count, u8 *scr, Plan p) {
     __shared__ u32 heads[2][1u << HBITS];
     const u64 g = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (g >= p.tiles) return;
+    if (g >= p.tile_start[count]) return;
     const u64 j = locate(p.tile_start, count, g);
     const u32 t = (u32)(g - p.tile_start[j]);
     const Unit un(a, first + j);
@@ -221,7 +210,7 @@ __global__ void __launch_bounds__(128) parse_kernel(Args a, u64 first, u64 count
     if (un.n >= MAX_UNIT) { a.out_len[u] = 0; a.status[u] = SWC_ERR_UNSUPPORTED; return; }
     const Scr s(scr + p.scr_off[j], un.n);
     const u8 *d = un.src;
-    const u32 n = (u32)un.n, nch = (u32)chunks_of(n);
+    const u32 n = (u32)un.n, nch = (u32)unit_chunks(n);
     u64 *rec = s.rec();
     u64 bits = 3;                                                                 // BFINAL, BTYPE (:96-97)
     u32 i = 0, lit = 0, nrec = 0, next = 1;
@@ -264,14 +253,14 @@ __global__ void __launch_bounds__(128) parse_kernel(Args a, u64 first, u64 count
 __global__ void __launch_bounds__(128) emit_kernel(Args a, u64 first, u64 count, u8 *scr, Plan p) {
     __shared__ u32 stage[4][64];
     const u64 g = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (g >= p.chunks) return;
+    if (g >= p.chunk_start[count]) return;
     const u64 j = locate(p.chunk_start, count, g);
     const u64 u = first + j;
     if (a.status[u] != SWC_OK) return;
     const u32 c = (u32)(g - p.chunk_start[j]);
     const u32 lane = lane_id();
     const Unit un(a, u);
-    const u32 n = (u32)un.n, nch = (u32)chunks_of(n);
+    const u32 n = (u32)un.n, nch = (u32)unit_chunks(n);
     const Scr s(scr + p.scr_off[j], n);
     u8 *out = a.out_base + a.out_off[u];
     if (s.hdr[2]) {                                                               // createUncompressedBlock :74-83
@@ -373,13 +362,13 @@ __global__ void __launch_bounds__(128) emit_kernel(Args a, u64 first, u64 count,
 
 __global__ void __launch_bounds__(256) seam_kernel(Args a, u64 first, u64 count, u8 *scr, Plan p) {
     const u64 g = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (g >= p.chunks) return;
+    if (g >= p.chunk_start[count]) return;
     const u64 j = locate(p.chunk_start, count, g);
     const u64 u = first + j;
     if (a.status[u] != SWC_OK) return;
     const u32 c = (u32)(g - p.chunk_start[j]);
     const u64 n = a.in_len[u];
-    const u32 nch = (u32)chunks_of(n);
+    const u32 nch = (u32)unit_chunks(n);
     const Scr s(scr + p.scr_off[j], n);
     if (s.hdr[2]) return;
     const u64 sb = chunk_begin(s, c), eb = chunk_end(s, c, nch);
@@ -392,14 +381,6 @@ __global__ void __launch_bounds__(256) seam_kernel(Args a, u64 first, u64 count,
     const u64 len = a.out_len[u];
     if (4 * w + 4 <= len) { ((u32 *)out)[w] = v; return; }
     for (u64 b = 4 * w; b < len; b++) out[b] = (u8)(v >> (8 * (b - 4 * w)));
-}
-
-u64 unit_tiles(u64 n) { return tiles_of(n); }
-u64 unit_chunks(u64 n) { return chunks_of(n); }
-u64 unit_scratch(u64 n) {
-    if (n >= MAX_UNIT) return 0;
-    return 256 + a256(2 * keyed(n)) + a256(4 * ((keyed(n) + 31) / 32)) + a256(sizeof(Checkpoint) * (chunks_of(n) + 1)) +
-           a256(8 * chunks_of(n)) + a256(Scr::big_bytes(n));
 }
 
 int run(const Args &a, u64 first, u64 count, u8 *scr, const Plan &p, cudaStream_t s) {
