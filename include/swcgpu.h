@@ -84,7 +84,9 @@ int32_t swc_deflate_decompress_batch_host(const uint8_t *in_base, const uint64_t
  * LZ4.decompress(data:)                                   Sources/LZ4/LZ4.swift:49-51
  * LZ4.decompress(data:dictionary:dictionaryID:)           Sources/LZ4/LZ4.swift:73-91
  * LZ4.multiDecompress(data:dictionary:dictionaryID:)      Sources/LZ4/LZ4.swift:116-146
- * LZ4.process(block:_:) (private raw-block decoder)       Sources/LZ4/LZ4.swift:332-413  -> *_block_batch */
+ * LZ4.process(block:_:) (private raw-block decoder)       Sources/LZ4/LZ4.swift:332-413  -> *_block_batch
+ * swc_lz4_decompress: *consumed_bytes is where the frame ended on SWC_OK and SWC_DATA_CHECKSUM_MISMATCH, and 0 on every
+ * other status, as consumed_bytes[i] of swc_lz4_frame_decompress_batch below, whose one-unit case it is. */
 int32_t swc_lz4_decompress(const uint8_t *in, size_t in_len, const uint8_t *dict /* NULL = nil */, size_t dict_len,
                            int32_t has_dict_id, uint32_t dict_id,
                            uint8_t **out, size_t *out_len, size_t *consumed_bytes);
@@ -109,8 +111,8 @@ int32_t swc_lz4_block_decompress_batch_host(const uint8_t *in_base, const uint64
  * where it ended.  One dictionary (device pointer, NULL = nil; an empty dictionary is a non-NULL pointer with dict_len 0)
  * serves the whole batch.  A unit that starts with a skippable frame is decoded without the dictionary and the dictionary
  * ID, as the reference's recursion into decompress(data:) does.
- * status[i] is what swc_lz4_decompress returns for the same bytes: the first failure the reference's sequential loop
- * meets (descriptor checks, then per block: mark, size, room, block checksum, decode; then content size, content checksum).
+ * status[i] is the first failure the reference's sequential loop meets (descriptor checks, then per block: mark, size,
+ * room, block checksum, decode; then content size, content checksum); swc_lz4_decompress is this batch on one unit.
  * SWC_DATA_CHECKSUM_MISMATCH carries its data: the unit's output region holds the decoded bytes.
  * Capacity: a unit that would be SWC_OK or SWC_DATA_CHECKSUM_MISMATCH but decodes to more than out_cap[i] reports
  * SWC_ERR_OUTPUT_OVERFLOW with out_len[i] = the exact decoded size, so one rerun with that capacity gives the final

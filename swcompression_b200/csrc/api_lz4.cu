@@ -1,240 +1,57 @@
-// api_lz4.cu — C ABI for LZ4: raw block batches (device / host) and the frame layer of
-// LZ4.decompress / LZ4.multiDecompress (reference Sources/LZ4/LZ4.swift:73-330).  Frame descriptors and block marks
-// are walked on the host (a few bytes per block); block decode, block checksums and the content checksum run on the
-// device.  Errors are reported in the order the reference's sequential loop would meet them.
+// api_lz4.cu — C ABI for LZ4: raw block batches (device / host) and the single calls LZ4.decompress /
+// LZ4.multiDecompress (reference Sources/LZ4/LZ4.swift:73-146).  A frame is one unit of the frame batch
+// (lz4_frame_batch.cu), which walks descriptors and block marks on the device and reports the reference's statuses;
+// only multiDecompress's loop over frames (skippable frames, the next magic) stays on the host.
 // The compress half here is the raw block batch; frames (LZ4.compress, LZ4+Compress.swift:16-154) are laid out on the
 // device by lz4_frame_compress.cu.
-#include <cstring>
+#include <algorithm>
 #include <vector>
 #include "../../include/swcgpu.h"
 #include "compress_host.h"
 #include "lz4.cuh"
 #include "lz4_compress.cuh"
-#include "lz4_frame.cuh"
 
 using namespace swc;
 
 namespace {
 
-inline uint64_t rd64(const uint8_t *p) { return (uint64_t)le32(p) | (uint64_t)le32(p + 4) << 32; }
-inline bool is_magic(uint32_t v) { return v == 0x184D2204u || v == 0x184C2102u || (v >= 0x184D2A50u && v <= 0x184D2A5Fu); }
-
-struct Block { uint64_t off, len; bool stored; uint32_t stored_ck; bool has_ck; };
-
-struct DeviceInput {      // compressed input + optional dictionary, resident on the device for one API call
-    DevBuf in, dict;
-    size_t in_len = 0, dict_len = 0;
-    bool have_dict = false;
-};
-
-// Decode `blocks` (offsets into dev.in) as `units` on the device and append the result to `host_out`.
-// mode: 0 = every block is its own unit (independent / legacy), 1 = one chain (dependent blocks).
-// `pending_error` is the framing error the host scan stopped at (0 if it reached the EndMark).
-int run_blocks(DeviceInput &dev, const std::vector<Block> &blocks, int mode, bool use_dict, size_t max_block,
-               bool check_blocks, int pending_error, HostOut &host_out, DevBuf &d_out_keep, size_t &d_out_len) {
-    const size_t nb = blocks.size();
-    d_out_len = 0;
-    if (nb == 0) return pending_error;
-    const size_t nunits = mode == 0 ? nb : 1;
-    // block columns, then unit columns (a unit is one block, or the whole chain of a dependent frame)
+// LZ4.decompress(data:dictionary:dictionaryID:) of d_in[start, in_len) as a one-unit swc_lz4_frame_decompress_batch;
+// r.consumed counts from `start`.  d_dict is NULL for `dictionary: nil`.
+int frame_unit(const u8 *d_in, size_t in_len, size_t start, const u8 *d_dict, size_t dict_len, int32_t has_dict_id,
+               uint32_t dict_id, UnitResult &r) {
+    const u64 len = in_len - start;
     UnitTable t;
-    const Col<u64> blk_off = t.in<u64>(nb), blk_len = t.in<u64>(nb), unit_off = t.in<u64>(nunits), unit_cap = t.in<u64>(nunits);
-    const Col<uint32_t> first = t.in<uint32_t>(nunits), count = t.in<uint32_t>(nunits);
-    const Col<u64> unit_len = t.out<u64>(nunits);
-    const Col<int32_t> status = t.out<int32_t>(nunits);
-    const Col<uint32_t> ck = t.out<uint32_t>(nb);
-    u64 *u_off = t.host(unit_off), *u_cap = t.host(unit_cap);
-    uint32_t *h_first = t.host(first), *h_cnt = t.host(count);
-    for (size_t i = 0; i < nb; i++) { t.host(blk_off)[i] = blocks[i].off; t.host(blk_len)[i] = blocks[i].len | (blocks[i].stored ? 1ull << 63 : 0); }
-    // first-attempt capacity: the frame's block size, but never more than an LZ4 block of that many bytes can expand to
-    // (each input byte adds at most 255 output bytes) — frames made of many tiny flushed blocks would otherwise ask for
-    // nb x 4 MiB; a block that decodes to more than this reports the size it needs and is redone (overflow retry below)
-    auto cap_of = [&](size_t i) {
-        if (blocks[i].stored) return round16(blocks[i].len);
-        const size_t expand = blocks[i].len < (max_block / 255 + 1) ? blocks[i].len * 255 + 64 : max_block;
-        return round16(expand < max_block ? expand : max_block);
-    };
-    size_t total = 0;
-    if (mode == 0) {
-        for (size_t i = 0; i < nb; i++) { u_off[i] = total; u_cap[i] = cap_of(i); total += u_cap[i]; h_first[i] = (uint32_t)i; h_cnt[i] = 1; }
-    } else {
-        for (size_t i = 0; i < nb; i++) total += cap_of(i);
-        u_off[0] = 0; u_cap[0] = total; h_first[0] = 0; h_cnt[0] = (uint32_t)nb;
-    }
-    std::vector<uint64_t> r_len;
-    std::vector<int32_t> r_st;
-    std::vector<uint32_t> r_ck;
+    const UnitCols c(t, 1);
+    const Col<swc_lz4_frame_info> info = t.out<swc_lz4_frame_info>(1);
+    // the walk alone first: it sizes the block table and the first output attempt
+    std::vector<swc_lz4_frame_info> f;
     int st = t.alloc();
     if (st) return st;
-    for (int attempt = 0; attempt < 2; attempt++) {
-        if ((st = d_out_keep.alloc(total))) return st;
-        if ((st = t.upload())) return st;
-        lz4::Args a{{dev.in.as<u8>(), t.dev(blk_off), t.dev(blk_len), d_out_keep.as<u8>(), t.dev(unit_off), t.dev(unit_cap),
-                     t.dev(unit_len), t.dev(status), nunits},
-                    t.dev(first), t.dev(count), use_dict && dev.have_dict ? dev.dict.as<u8>() : nullptr,
-                    use_dict && dev.have_dict ? dev.dict_len : 0, nullptr};
-        if (mode == 1 && a.dict_len > 65536) { a.dict += a.dict_len - 65536; a.dict_len = 65536; }    // LZ4.swift:309
-        if (mode == 0) {               // one block per unit: take the two-phase (parse + 8-wide execute) path
-            uint64_t tot = 0;
-            for (size_t i = 0; i < nb; i++) tot += blocks[i].len;
-            void *scr = nullptr;
-            if ((st = scratch_get(lz4::two_phase_scratch_bytes(nb, tot), &scr, 0))) return st;
-            a.first_blk = nullptr; a.n_blk = nullptr; a.scratch = scr;
-        }
-        if ((st = lz4::launch(a, 0))) return st;
-        if (check_blocks && attempt == 0) {
-            if ((st = checks::xxh32_batch(dev.in.as<u8>(), t.dev(blk_off), t.dev(blk_len), t.dev(ck), nb, 0))) return st;
-            if ((st = t.fetch(ck, r_ck))) return st;
-        }
-        if ((st = t.fetch(unit_len, r_len)) || (st = t.fetch(status, r_st))) return st;
-        bool overflow = false;
-        for (size_t u = 0; u < nunits; u++) if (r_st[u] == SWC_ERR_OUTPUT_OVERFLOW) overflow = true;
-        if (!overflow) break;
-        // a block decoded to more than the frame's block size (the reference does not forbid it): redo with exact sizes
-        total = 0;
-        for (size_t u = 0; u < nunits; u++) {
-            if (r_st[u] == SWC_ERR_OUTPUT_OVERFLOW || r_st[u] == SWC_OK) u_cap[u] = round16((size_t)r_len[u]);
-            u_off[u] = total; total += u_cap[u];
-        }
-    }
-    // report in the reference's sequential order: block k checksum (LZ4.swift:300), then block k decode (:305-313)
-    if (mode == 0) {
-        for (size_t i = 0; i < nb; i++) {
-            if (check_blocks && blocks[i].has_ck && r_ck[i] != blocks[i].stored_ck) return SWC_DATA_CORRUPTED;
-            if (r_st[i] != SWC_OK) return r_st[i];
-        }
-    } else {
-        size_t fail_blk = r_st[0] != SWC_OK ? (size_t)r_len[0] : nb;
-        for (size_t i = 0; i < nb; i++) {
-            if (check_blocks && blocks[i].has_ck && r_ck[i] != blocks[i].stored_ck) return SWC_DATA_CORRUPTED;
-            if (i == fail_blk) return r_st[0];
-        }
-        if (r_st[0] != SWC_OK) return r_st[0];
-    }
-    if (pending_error) return pending_error;
-    // gather
-    size_t produced = 0;
-    for (size_t u = 0; u < nunits; u++) produced += (size_t)r_len[u];
-    uint8_t *dst = host_out.grow(produced);
-    if (!dst) return SWC_ERR_OUTPUT_OVERFLOW;
-    bool contiguous = true;
-    { size_t run = 0; for (size_t u = 0; u < nunits; u++) { if (u_off[u] != run) contiguous = false; run += (size_t)r_len[u]; } }
-    if (contiguous) {
-        if (produced) SWC_CUDA_TRY(cudaMemcpy(dst, d_out_keep.p, produced, cudaMemcpyDeviceToHost));
-    } else {
-        for (size_t u = 0; u < nunits; u++) {
-            if (r_len[u]) SWC_CUDA_TRY(cudaMemcpy(dst, d_out_keep.as<u8>() + u_off[u], (size_t)r_len[u], cudaMemcpyDeviceToHost));
-            dst += (size_t)r_len[u];
-        }
-    }
-    d_out_len = contiguous ? produced : 0;     // 0 = the device copy is not one contiguous run
-    return SWC_OK;
+    *t.host(c.in_off) = start;
+    *t.host(c.in_len) = len;
+    if ((st = t.upload()) || (st = swc_lz4_frame_info_batch(d_in, t.dev(c.in_off), t.dev(c.in_len), d_dict != nullptr, has_dict_id,
+                                                            dict_id, t.dev(info), 1, 0)) || (st = t.fetch(info, f)))
+        return st;
+    // every block could be full, but no input byte decodes to more than 255 bytes; a legacy frame's blocks are guessed at
+    // 8 MiB.  A unit that needs more reports its exact size, and the one rerun at that size is final.
+    const u64 nb = f[0].n_blocks, max_block = f[0].max_block_size ? f[0].max_block_size : 8u << 20;
+    u64 cap = std::min(nb * max_block, 255 * (len - f[0].frame_start) + 64 * nb);
+    if (f[0].content_size != UINT64_MAX) cap = std::min(cap, f[0].content_size);
+    const u64 max_blocks = nb ? nb : 1;
+    const size_t scratch_bytes = swc_lz4_frame_batch_scratch_bytes(1, len, max_blocks);
+    void *scratch = nullptr;
+    if ((st = scratch_get(scratch_bytes, &scratch, 0))) return st;
+    return decode_unit(t, c, d_in, start, in_len, cap, 2, [](size_t, size_t need) { return need; }, [&](const DecodeIO &io, size_t) {
+        return swc_lz4_frame_decompress_batch(io.in_base, io.in_off, io.in_len, d_dict, dict_len, has_dict_id, dict_id, io.out_base,
+                                              io.out_off, io.out_cap, io.out_len, io.consumed, io.status, 1, max_blocks, scratch,
+                                              scratch_bytes, 0);
+    }, r);
 }
 
-// process(frame:) LZ4.swift:188-330; `p` is the whole input, `pos` points right after the magic.
-int frame(DeviceInput &dev, const uint8_t *p, size_t n_total, size_t pos, bool have_dict, bool has_ext_id, uint32_t ext_id,
-          HostOut &out, size_t *next) {
-    const uint8_t *in = p + pos;
-    const size_t n = n_total - pos;
-    if (n < 7) return SWC_DATA_TRUNCATED;
-    size_t off = 0;
-    const unsigned flg = in[off++];
-    if (!(((flg & 0xC0) >> 6) == 1 && (flg & 0x2) == 0)) return SWC_DATA_CORRUPTED;
-    const bool independent = flg & 0x20, block_ck = flg & 0x10, csize_p = flg & 0x8, cck = flg & 0x4, dictid_p = flg & 1;
-    const unsigned bd = in[off++];
-    size_t max_block;
-    switch (bd) {
-    case 0x40: max_block = 64u << 10; break;
-    case 0x50: max_block = 256u << 10; break;
-    case 0x60: max_block = 1u << 20; break;
-    case 0x70: max_block = 4u << 20; break;
-    default: return SWC_DATA_CORRUPTED;
-    }
-    uint64_t content_size = 0;
-    if (csize_p) {
-        if (n - off < 13) return SWC_DATA_TRUNCATED;
-        content_size = rd64(in + off); off += 8;
-        if (content_size > (uint64_t)INT64_MAX) return SWC_DATA_UNSUPPORTED_FEATURE;
-    }
-    if (dictid_p) {
-        if (!have_dict) return SWC_DATA_CORRUPTED;
-        if (n - off < 9) return SWC_DATA_TRUNCATED;
-        uint32_t id = le32(in + off); off += 4;
-        if (has_ext_id && ext_id != id) return SWC_DATA_CORRUPTED;
-    }
-    const uint8_t hc = (uint8_t)((lz4f::xxh32_descriptor(in, (u32)off) >> 8) & 0xFF);
-    if (hc != in[off]) return SWC_DATA_CORRUPTED;
-    off++;
-
-    std::vector<Block> blocks;
-    int pending = SWC_OK;
-    for (;;) {                                                     // LZ4.swift:278-318 framing only
-        if (n - off < 4) { pending = SWC_DATA_TRUNCATED; break; }
-        uint32_t mark = le32(in + off); off += 4;
-        if (mark == 0) break;
-        size_t bs = mark & 0x7FFFFFFFu;
-        if (bs > max_block) { pending = SWC_DATA_CORRUPTED; break; }
-        if (n - off < bs + (block_ck ? 4 : 0) + 4) { pending = SWC_DATA_TRUNCATED; break; }
-        Block b; b.off = pos + off; b.len = bs; b.stored = (mark & 0x80000000u) != 0; b.has_ck = block_ck; b.stored_ck = 0;
-        off += bs;
-        if (block_ck) { b.stored_ck = le32(in + off); off += 4; }
-        blocks.push_back(b);
-    }
-    const size_t fstart = out.len;
-    DevBuf d_out; size_t d_out_len = 0;
-    int st = run_blocks(dev, blocks, independent ? 0 : 1, have_dict, max_block, block_ck, pending, out, d_out, d_out_len);
-    if (st) return st;
-    const size_t flen = out.len - fstart;
-    if (csize_p && (uint64_t)flen != content_size) return SWC_DATA_CORRUPTED;
-    if (cck) {                                                     // :323-328
-        if (n - off < 4) return SWC_DATA_TRUNCATED;
-        uint32_t stored = le32(in + off); off += 4;
-        // content checksum over the decoded frame, on the device
-        DevBuf d_tmp;
-        const u8 *d_data = d_out.as<u8>();
-        if (d_out_len != flen || d_out_len == 0) {  // output was gathered from non-contiguous regions (or is empty): re-upload
-            if ((st = d_tmp.alloc(flen + 16))) return st;
-            if (flen) SWC_CUDA_TRY(cudaMemcpy(d_tmp.p, out.p + fstart, flen, cudaMemcpyHostToDevice));
-            d_data = d_tmp.as<u8>();
-        }
-        u64 got = 0;
-        if ((st = checks::check_device(checks::XXH32, d_data, flen, &got))) return st;
-        *next = pos + off;
-        if ((uint32_t)got != stored) return SWC_DATA_CHECKSUM_MISMATCH;
-    }
-    *next = pos + off;
-    return SWC_OK;
-}
-
-// process(legacyFrame:) LZ4.swift:160-186
-int legacy_frame(DeviceInput &dev, const uint8_t *p, size_t n_total, size_t pos, HostOut &out, size_t *next) {
-    size_t off = pos;
-    std::vector<Block> blocks;
-    int pending = SWC_OK;
-    while (off < n_total) {
-        if (n_total - off < 4) { pending = SWC_DATA_TRUNCATED; break; }
-        uint32_t raw = le32(p + off); off += 4;
-        if (is_magic(raw)) { off -= 4; break; }
-        if (n_total - off < raw) { pending = SWC_DATA_TRUNCATED; break; }
-        Block b; b.off = off; b.len = raw; b.stored = false; b.has_ck = false; b.stored_ck = 0;
-        blocks.push_back(b);
-        off += raw;
-    }
-    DevBuf d_out; size_t d_out_len = 0;
-    int st = run_blocks(dev, blocks, 0, false, 8u << 20, false, pending, out, d_out, d_out_len);
-    if (st) return st;
-    *next = off;
-    return SWC_OK;
-}
-
-int upload(DeviceInput &dev, const uint8_t *in, size_t in_len, const uint8_t *dict, size_t dict_len) {
-    int st;
-    if ((st = upload_input(dev.in, in, in_len))) return st;
-    dev.in_len = in_len;
-    dev.have_dict = dict != nullptr;
-    dev.dict_len = dict ? dict_len : 0;
-    if (dict && dict_len && (st = upload_input(dev.dict, dict, dict_len))) return st;
-    return SWC_OK;
+// the input, and the dictionary unless it is nil (an empty one is still a device pointer)
+int upload(DevBuf &d_in, DevBuf &d_dict, const uint8_t *in, size_t in_len, const uint8_t *dict, size_t dict_len) {
+    const int st = upload_input(d_in, in, in_len);
+    return st || !dict ? st : upload_input(d_dict, dict, dict_len);
 }
 
 }  // namespace
@@ -311,35 +128,16 @@ int32_t swc_lz4_decompress(const uint8_t *in, size_t in_len, const uint8_t *dict
     if (consumed_bytes) *consumed_bytes = 0;
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
-    size_t base = 0;
-    bool have_dict = dict != nullptr;
-    for (;;) {
-        if (in_len - base < 4) return SWC_DATA_TRUNCATED;
-        const uint32_t magic = le32(in + base);
-        if (magic >= 0x184D2A50u && magic <= 0x184D2A5Fu) {           // :148-155, then recursion without dictionary (:85)
-            if (in_len - base - 4 < 4) return SWC_DATA_TRUNCATED;
-            size_t size = le32(in + base + 4);
-            if (in_len - base - 4 < size + 4) return SWC_DATA_TRUNCATED;
-            base += 4 + size + 4;
-            have_dict = false; has_dict_id = 0;
-            continue;
-        }
-        if (magic != 0x184D2204u && magic != 0x184C2102u) return SWC_DATA_CORRUPTED;
-        DeviceInput dev;
-        int st = upload(dev, in, in_len, have_dict ? dict : nullptr, dict_len);
-        if (st) return st;
-        HostOut o;
-        size_t next = base + 4;
-        if (magic == 0x184D2204u) st = frame(dev, in, in_len, base + 4, have_dict, has_dict_id != 0, dict_id, o, &next);
-        else st = legacy_frame(dev, in, in_len, base + 4, o, &next);
-        if (consumed_bytes) *consumed_bytes = next;
-        if (st != SWC_OK && st != SWC_DATA_CHECKSUM_MISMATCH) return st;
-        int g = o.release_to(out, out_len);
-        return g ? g : st;
-    }
+    DevBuf d_in, d_dict;
+    UnitResult r;
+    int st = upload(d_in, d_dict, in, in_len, dict, dict_len);
+    if (st || (st = frame_unit(d_in.as<u8>(), in_len, 0, d_dict.as<u8>(), dict_len, has_dict_id, dict_id, r))) return st;
+    if (consumed_bytes) *consumed_bytes = r.consumed;
+    if (r.status != SWC_OK && r.status != SWC_DATA_CHECKSUM_MISMATCH) return r.status;
+    return (st = to_host_alloc(r.out.p, r.out_len, out, out_len)) ? st : r.status;
 }
 
-// LZ4.multiDecompress LZ4.swift:116-146
+// LZ4.multiDecompress LZ4.swift:116-146: the frame loop on the host, each frame one unit of the frame batch
 int32_t swc_lz4_multi_decompress(const uint8_t *in, size_t in_len, const uint8_t *dict, size_t dict_len,
                                  int32_t has_dict_id, uint32_t dict_id,
                                  uint8_t **out, size_t *out_len, size_t **frame_ends, size_t *n_frames) {
@@ -347,31 +145,34 @@ int32_t swc_lz4_multi_decompress(const uint8_t *in, size_t in_len, const uint8_t
     *out = nullptr; *out_len = 0; *frame_ends = nullptr; *n_frames = 0;
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
-    DeviceInput dev;
-    bool uploaded = false;
+    DevBuf d_in, d_dict;
+    int st = upload(d_in, d_dict, in, in_len, dict, dict_len);
+    if (st) return st;
     HostOut o;
     std::vector<size_t> ends;
     size_t next = 0;
     int result = SWC_OK;
     do {
-        if (next + 4 > in_len) { result = SWC_DATA_TRUNCATED; break; }
-        const uint32_t magic = le32(in + next); next += 4;
-        int st = SWC_OK; bool produced = false;
-        if (magic == 0x184D2204u || magic == 0x184C2102u) {
-            if (!uploaded) { if ((st = upload(dev, in, in_len, dict, dict_len))) return st; uploaded = true; }
-            size_t nn = next;
-            if (magic == 0x184D2204u) st = frame(dev, in, in_len, next, dict != nullptr, has_dict_id != 0, dict_id, o, &nn);
-            else st = legacy_frame(dev, in, in_len, next, o, &nn);
-            next = nn; produced = true;
-        } else if (magic >= 0x184D2A50u && magic <= 0x184D2A5Fu) {
-            if (in_len - next < 4) { result = SWC_DATA_TRUNCATED; break; }
-            size_t size = le32(in + next);
-            if (in_len - next < size + 4) { result = SWC_DATA_TRUNCATED; break; }
-            next += size + 4;
-        } else { result = SWC_DATA_CORRUPTED; break; }
-        if (produced && (st == SWC_OK || st == SWC_DATA_CHECKSUM_MISMATCH)) ends.push_back(o.len);
-        if (st) { result = st; break; }
-    } while (next < in_len);
+        if (in_len - next < 4) { result = SWC_DATA_TRUNCATED; break; }
+        const uint32_t magic = le32(in + next);
+        if (magic >= 0x184D2A50u && magic <= 0x184D2A5Fu) {       // skipped here; unlike decompress(data:), the dictionary stays
+            if (in_len - next - 4 < 4) { result = SWC_DATA_TRUNCATED; break; }
+            const size_t size = le32(in + next + 4);
+            if (in_len - next - 8 < size) { result = SWC_DATA_TRUNCATED; break; }
+            next += 8 + size;
+            continue;
+        }
+        if (magic != 0x184D2204u && magic != 0x184C2102u) { result = SWC_DATA_CORRUPTED; break; }
+        UnitResult r;
+        if ((st = frame_unit(d_in.as<u8>(), in_len, next, d_dict.as<u8>(), dict_len, has_dict_id, dict_id, r))) return st;
+        result = r.status;
+        if (result != SWC_OK && result != SWC_DATA_CHECKSUM_MISMATCH) break;
+        uint8_t *dst = o.grow(r.out_len);
+        if (!dst) return SWC_ERR_OUTPUT_OVERFLOW;
+        if ((st = copy_pageable(dst, r.out.p, r.out_len, false))) return st;
+        ends.push_back(o.len);
+        next += r.consumed;
+    } while (result == SWC_OK && next < in_len);
     if (result != SWC_OK && result != SWC_DATA_CHECKSUM_MISMATCH) return result;
     int g;
     if ((g = o.release_to(out, out_len)) || (g = give_sizes(ends, frame_ends, out, out_len))) return g;

@@ -83,9 +83,10 @@ inline int read_lens(const u64 *d, u64 n, cudaStream_t s, std::vector<u64> &v) {
 }
 
 // ---- unit tables: the per-unit metadata of one batch, as typed columns in one device allocation ----
-// Declare every column first, then seat the table with alloc() (its own cudaMalloc) or place() (memory the caller owns);
-// host() pointers stay valid from the last declaration on.  in<T>() columns have a zero-filled host side that upload()
-// sends in one copy; out<T>() columns exist on the device only (kernel results, or filled by the caller's own copies).
+// Declare every column first, then seat the table with alloc() (its own cudaMalloc, kept when alloc() is called again) or
+// place() (memory the caller owns); host() pointers stay valid from the last declaration on.  in<T>() columns have a
+// zero-filled host side that upload() sends in one copy; out<T>() columns exist on the device only (kernel results, or
+// filled by the caller's own copies).
 // Every column starts on a 256-byte boundary, so a column never overlaps its neighbour whatever its type and length.
 template <typename T> struct Col { size_t off = 0, n = 0; bool dev_only = false; };
 class UnitTable {
@@ -95,7 +96,7 @@ class UnitTable {
     template <typename T> T *host(Col<T> c) { return (T *)(host_.data() + c.off); }
     template <typename T> T *dev(Col<T> c) const { return (T *)(dev_.as<u8>() + (c.dev_only ? host_.size() : 0) + c.off); }
     size_t bytes() const { return host_.size() + out_bytes_; }
-    int alloc() { return dev_.alloc(bytes()); }
+    int alloc() { return dev_.p && dev_.owned && dev_.bytes == bytes() ? SWC_OK : dev_.alloc(bytes()); }
     void place(void *p) { dev_.borrow(p, bytes()); }
     int upload(cudaStream_t s = 0) {
         if (!host_.empty()) SWC_CUDA_TRY(cudaMemcpyAsync(dev_.p, host_.data(), host_.size(), cudaMemcpyHostToDevice, s));
