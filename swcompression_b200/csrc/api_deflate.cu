@@ -24,15 +24,14 @@ int deflate_batch_impl(const DecodeIO &io, const uint8_t *start_bits, uint64_t o
 }
 
 // Decode one Deflate stream that already sits on the device; retries once more at the exact size the counting pass reports.
-int deflate_unit_device(const u8 *d_in, size_t in_len, size_t start_bit_abs, UnitResult &r, size_t hint) {
+static int deflate_unit_device(const u8 *d_in, size_t in_len, size_t start_bit_abs, UnitResult &r) {
     size_t start_byte = start_bit_abs >> 3;
     if (start_byte > in_len) start_byte = in_len;
     UnitTable t;
     UnitCols c(t, 1);
     const Col<u8> sb = t.in<u8>(1);
     *t.host(sb) = (u8)(start_bit_abs & 7);
-    const size_t first_cap = hint ? hint : (in_len - start_byte) * 4 + 65536;
-    int st = decode_unit(t, c, d_in, start_byte, in_len, first_cap, 3, [](size_t, size_t need) { return need; },
+    int st = decode_unit(t, c, d_in, start_byte, in_len, (in_len - start_byte) * 4 + 65536, 3, [](size_t, size_t need) { return need; },
                          [&](const DecodeIO &io, size_t cap) { return deflate_batch_impl(io, t.dev(sb), cap, nullptr, 0, 0); }, r);
     if (st) return st;
     if (r.status == SWC_INTERNAL_NEEDS_SLOW) r.status = SWC_ERR_UNSUPPORTED;

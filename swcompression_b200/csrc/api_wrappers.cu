@@ -1,7 +1,7 @@
-// api_wrappers.cu — GzipArchive / ZlibArchive framing around the device Deflate decoder, and the checksum C ABI.
-// Reference: Sources/GZip/GzipArchive.swift:38-100, GzipHeader.swift:68-199, Sources/Zlib/ZlibArchive.swift:25-42,
-// ZlibHeader.swift:47-93.  Headers/trailers (tens of bytes) are parsed on the host with the grammar of archive_header.cuh;
-// Deflate and CRC-32 / Adler-32 over the payload run on the device.  The batched form is unarchive_batch.cu.
+// api_wrappers.cu — GzipArchive / ZlibArchive single and multi-member calls, and the checksum C ABI.
+// Reference: Sources/GZip/GzipArchive.swift:38-100, Sources/Zlib/ZlibArchive.swift:25-42.  An archive or member is one unit
+// of the device unarchive batch (unarchive_batch.cu), which parses the header, decodes the Deflate stream, checks the
+// trailer and reports the reference's statuses; only multiUnarchive's walk over members stays on the host.
 #include <algorithm>
 #include <chrono>
 #include <cstdio>
@@ -17,47 +17,41 @@ using namespace swc;
 
 namespace {
 
-int gzip_header(const uint8_t *in, size_t n, size_t *off) {
-    swc_gzip_header h;
-    const int st = gzip_parse(in, n, *off, &h);
-    if (st == SWC_OK) *off += h.header_len;
-    return st;
+// GzipArchive.unarchive / ZlibArchive.unarchive of d_in[start, in_len) as a one-unit unarchive batch, r.consumed counted from
+// `start`: 4 x the input plus 64 KiB first; a unit that needs more reports its exact size, and the rerun at that size is final.
+int archive_unit(bool gzip, const u8 *d_in, size_t in_len, size_t start, UnitResult &r) {
+    UnitTable t;
+    const UnitCols c(t, 1);
+    return decode_unit(t, c, d_in, start, in_len, (in_len - start) * 4 + 65536, 3, [](size_t, size_t need) { return need; },
+                       [&](const DecodeIO &io, size_t cap) { return unarchive_batch_impl(gzip, io, nullptr, cap, nullptr, 0, 0); }, r);
 }
 
-// processMember GzipArchive.swift:79-100; d_in holds the whole archive on the device
-int gzip_member(const uint8_t *in, size_t n, const u8 *d_in, size_t *off, HostOut &out, bool *crc_error) {
-    if (n - *off < 20) return SWC_GZIP_WRONG_MAGIC;
-    int st = gzip_header(in, n, off);
-    if (st) return st;
+// processMember GzipArchive.swift:79-100 at *off, appended to `out` with its end and start; *off moves past the member.  A
+// member with a wrong CRC is still returned and sets *crc_error; any other failure is the result.
+int next_member(const u8 *d_in, size_t n, size_t *off, HostOut &out, std::vector<size_t> &ends, std::vector<size_t> &starts,
+                bool *crc_error) {
     UnitResult r;
-    if ((st = deflate_unit_device(d_in, n, (size_t)*off * 8, r))) return st;
-    if (r.status != SWC_OK) return r.status;
-    size_t p = *off + (r.consumed + 7) / 8;                          // align()
-    if (n - p < 8) return SWC_GZIP_WRONG_MAGIC;
-    const uint32_t crc = le32(in + p), isize = le32(in + p + 4);
-    p += 8;
-    if ((uint32_t)r.out_len != isize) return SWC_GZIP_WRONG_ISIZE;
-    u64 got = 0;
-    if ((st = checks::check_device(checks::CRC32, r.out.as<u8>(), r.out_len, &got))) return st;
-    *crc_error = (uint32_t)got != crc;
+    int st = archive_unit(true, d_in, n, *off, r);
+    if (st) return st;
+    if (r.status != SWC_OK && r.status != SWC_GZIP_WRONG_CRC) return r.status;
     uint8_t *dst = out.grow(r.out_len);
     if (!dst) return SWC_ERR_OUTPUT_OVERFLOW;
     if (r.out_len) SWC_CUDA_TRY(cudaMemcpy(dst, r.out.p, r.out_len, cudaMemcpyDeviceToHost));
-    *off = p;
+    ends.push_back(out.len); starts.push_back(*off);
+    *crc_error = r.status == SWC_GZIP_WRONG_CRC;
+    *off += r.consumed;
     return SWC_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Batch path for multi-member archives (BGZF and friends).  Members are independent Deflate streams, so candidate member
-// starts are found by signature, every candidate is decoded speculatively in ONE batched launch (its input ends 8 bytes
-// before the next candidate; its capacity is the ISIZE found there), and the in-order walk of GzipArchive.multiUnarchive
-// (GzipArchive.swift:52-77) then only *validates*: member k is accepted iff it decoded cleanly, stopped exactly at that
-// trailer and produced ISIZE bytes — exactly what the sequential decoder would have computed from the same start.  A
-// member that does not validate (a signature look-alike inside its payload, ISIZE wrap-around, damage) is decoded by the
-// sequential path, and the walk resynchronises on the candidate list afterwards.
-static size_t inflate_scratch_bytes(u64 n, u64 out_total) { return swc_deflate_batch_scratch_bytes(n, out_total); }
-
-struct Cand { size_t at, dstart, next; uint32_t crc, isize; long unit; };
+// starts are found by signature, and every candidate is one unit [at, next) of ONE unarchive batch, its capacity the ISIZE
+// found at next - 4.  The in-order walk of GzipArchive.multiUnarchive (GzipArchive.swift:52-77) then only *validates*:
+// member k is accepted iff its status is OK or a wrong CRC and it consumed exactly next - at bytes — its trailer then sits
+// at next - 8, so it is what the sequential decoder would have computed from the same start.  A member that does not
+// validate (a signature look-alike inside its payload, ISIZE wrap-around, damage) is decoded by the sequential path, and
+// the walk resynchronises on the candidate list afterwards.
+struct Cand { size_t at, next; uint32_t isize; long unit; };
 
 int gzip_multi_batch(const uint8_t *in, size_t n, const u8 *d_in, HostOut &o, std::vector<size_t> &ends, std::vector<size_t> &starts, size_t *off, int *result, bool *stop) {
     const bool trace = getenv("SWC_TRACE") != nullptr;
@@ -82,13 +76,10 @@ int gzip_multi_batch(const uint8_t *in, size_t n, const u8 *d_in, HostOut &o, st
         size_t nu = 0, out_total = 0;
         for (size_t k = idx; k < pos.size() && cs.size() < (1u << 22); k++) {
             Cand c;
-            c.at = pos[k]; c.next = k + 1 < pos.size() ? pos[k + 1] : n; c.unit = -1; c.crc = c.isize = 0;
-            size_t d = c.at;
-            const bool hdr_ok = gzip_header(in, c.next, &d) == SWC_OK;   // a real header never reaches the next member
-            c.dstart = d;
-            if (hdr_ok && c.next >= d + 8) {
-                c.crc = le32(in + c.next - 8); c.isize = le32(in + c.next - 4);
-                if ((u64)c.isize <= (u64)(c.next - 8 - d) * 1032 + 64) {    // Deflate cannot expand further than ~1032:1
+            c.at = pos[k]; c.next = k + 1 < pos.size() ? pos[k + 1] : n; c.unit = -1; c.isize = 0;
+            if (c.next - c.at >= 20) {                                   // a shorter member fails the 20-byte guard anyway
+                c.isize = le32(in + c.next - 4);
+                if ((u64)c.isize <= (u64)(c.next - c.at) * 1032 + 64) {     // Deflate cannot expand further than ~1032:1
                     const size_t cap16 = round16((size_t)c.isize);
                     if (out_total + cap16 > budget && !cs.empty()) break;
                     c.unit = (long)nu++;
@@ -99,38 +90,35 @@ int gzip_multi_batch(const uint8_t *in, size_t n, const u8 *d_in, HostOut &o, st
         }
         UnitTable t;
         UnitCols uc(t, nu);
-        const Col<uint32_t> crc = t.out<uint32_t>(nu);
         u64 *h_outoff = t.host(uc.out_off);
         for (size_t k = 0, run = 0; k < cs.size(); k++) {
             const Cand &c = cs[k];
             if (c.unit < 0) continue;
-            t.host(uc.in_off)[c.unit] = c.dstart; t.host(uc.in_len)[c.unit] = c.next - 8 - c.dstart;
+            t.host(uc.in_off)[c.unit] = c.at; t.host(uc.in_len)[c.unit] = c.next - c.at;
             h_outoff[c.unit] = run; t.host(uc.out_cap)[c.unit] = c.isize;
             run += round16((size_t)c.isize);
         }
         UnitCols::Results res;
-        std::vector<uint32_t> h_crc;
         DevBuf d_out;
         if (nu) {
             // an allocation failure is not an error of the archive: hand the rest to the caller's sequential walk
             if (t.alloc()) return SWC_OK;
             if (d_out.alloc(out_total + 64)) return SWC_OK;
-            { void *scr = nullptr; if (scratch_get(inflate_scratch_bytes(nu, out_total), &scr, stream)) return SWC_OK; }
+            { void *scr = nullptr; if (scratch_get(swc_unarchive_batch_scratch_bytes(nu, out_total), &scr, stream)) return SWC_OK; }
             int st = t.upload(stream);
             if (st) return st;
-            if ((st = deflate_batch_impl(uc.bind(t, d_in, d_out.as<u8>(), 0, nu), nullptr, out_total, nullptr, 0, stream))) return st;
-            if ((st = checks::crc32_units(d_out.as<u8>(), t.dev(uc.out_off), t.dev(uc.out_len), t.dev(uc.status), t.dev(crc), nu, stream))) return st;
-            if ((st = uc.fetch(t, res, stream)) || (st = t.fetch(crc, h_crc, stream))) return st;
+            if ((st = unarchive_batch_impl(true, uc.bind(t, d_in, d_out.as<u8>(), 0, nu), nullptr, out_total, nullptr, 0, stream))) return st;
+            if ((st = uc.fetch(t, res, stream))) return st;
         }
-        if (trace) fprintf(stderr, "[swc] gzip round: %zu units, %.1f MB out, decode+crc done at %.1f ms\n", nu, out_total / 1e6, now() - t0);
+        if (trace) fprintf(stderr, "[swc] gzip round: %zu units, %.1f MB out, decode done at %.1f ms\n", nu, out_total / 1e6, now() - t0);
         // ---- the in-order walk: accept the longest validated prefix
         size_t accepted = 0;
         for (; accepted < cs.size(); accepted++) {
             const Cand &c = cs[accepted];
             if (c.unit < 0) break;
             const size_t u = (size_t)c.unit;
-            if (res.status[u] != SWC_OK || c.dstart + (res.consumed[u] + 7) / 8 + 8 != c.next || res.out_len[u] != c.isize) break;
-            if (h_crc[u] != c.crc) { *result = SWC_GZIP_WRONG_CRC; *stop = true; accepted++; break; }   // the member is still returned
+            if ((res.status[u] != SWC_OK && res.status[u] != SWC_GZIP_WRONG_CRC) || res.consumed[u] != c.next - c.at) break;
+            if (res.status[u] == SWC_GZIP_WRONG_CRC) { *result = SWC_GZIP_WRONG_CRC; *stop = true; accepted++; break; }   // the member is still returned
         }
         if (accepted) {
             UnitTable g;
@@ -161,14 +149,28 @@ int gzip_multi_batch(const uint8_t *in, size_t n, const u8 *d_in, HostOut &o, st
         if (accepted == cs.size()) continue;                             // next round (or done)
         // ---- member idx did not validate: decode it the sequential way, then resynchronise on the candidate list
         bool crc_error = false;
-        const size_t member_at = *off;
-        int st = gzip_member(in, n, d_in, off, o, &crc_error);
+        int st = next_member(d_in, n, off, o, ends, starts, &crc_error);
         if (st) return st;
-        ends.push_back(o.len); starts.push_back(member_at);
         if (crc_error) { *result = SWC_GZIP_WRONG_CRC; *stop = true; return SWC_OK; }
         idx = (size_t)(std::lower_bound(pos.begin(), pos.end(), *off) - pos.begin());
     }
     return SWC_OK;
+}
+
+// GzipArchive.unarchive / ZlibArchive.unarchive GzipArchive.swift:38-47, ZlibArchive.swift:25-42
+int single_unarchive(bool gzip, const uint8_t *in, size_t n, uint8_t **out, size_t *out_len, size_t *consumed_bytes) {
+    if (!out || !out_len) return SWC_ERR_INVALID_ARG;
+    *out = nullptr; *out_len = 0;
+    if (consumed_bytes) *consumed_bytes = 0;
+    if (ensure_device()) return SWC_ERR_NO_DEVICE;
+    ApiLock api_lock;
+    DevBuf d_in;
+    UnitResult r;
+    int st = upload_input(d_in, in, n);
+    if (st || (st = archive_unit(gzip, d_in.as<u8>(), n, 0, r))) return st;
+    if (consumed_bytes) *consumed_bytes = r.consumed;
+    if (r.status != SWC_OK && r.status != (gzip ? SWC_GZIP_WRONG_CRC : SWC_ZLIB_WRONG_ADLER32)) return r.status;
+    return (st = to_host_alloc(r.out.p, r.out_len, out, out_len)) ? st : r.status;
 }
 
 template <typename F>
@@ -186,20 +188,7 @@ int host_check(const uint8_t *in, size_t n, F fn) {
 extern "C" {
 
 int32_t swc_gzip_unarchive(const uint8_t *in, size_t in_len, uint8_t **out, size_t *out_len, size_t *consumed_bytes) {
-    if (!out || !out_len) return SWC_ERR_INVALID_ARG;
-    *out = nullptr; *out_len = 0;
-    if (consumed_bytes) *consumed_bytes = 0;
-    if (ensure_device()) return SWC_ERR_NO_DEVICE;
-    ApiLock api_lock;
-    DevBuf d_in;
-    int st = upload_input(d_in, in, in_len);
-    if (st) return st;
-    HostOut o;
-    size_t off = 0; bool crc_error = false;
-    if ((st = gzip_member(in, in_len, d_in.as<u8>(), &off, o, &crc_error))) return st;
-    if (consumed_bytes) *consumed_bytes = off;
-    if ((st = o.release_to(out, out_len))) return st;
-    return crc_error ? SWC_GZIP_WRONG_CRC : SWC_OK;
+    return single_unarchive(true, in, in_len, out, out_len, consumed_bytes);
 }
 
 // GzipArchive.multiUnarchive GzipArchive.swift:52-77
@@ -221,9 +210,7 @@ static int gzip_multi(const uint8_t *in, size_t in_len, uint8_t **out, size_t *o
     if ((st = gzip_multi_batch(in, in_len, d_in.as<u8>(), o, ends, starts, &off, &result, &stop))) return st;
     while (off < in_len && !stop) {
         bool crc_error = false;
-        const size_t member_at = off;
-        if ((st = gzip_member(in, in_len, d_in.as<u8>(), &off, o, &crc_error))) return st;
-        ends.push_back(o.len); starts.push_back(member_at);
+        if ((st = next_member(d_in.as<u8>(), in_len, &off, o, ends, starts, &crc_error))) return st;
         if (crc_error) { result = SWC_GZIP_WRONG_CRC; break; }
     }
     if ((st = o.release_to(out, out_len)) || (st = give_sizes(ends, member_ends, out, out_len))) return st;
@@ -258,31 +245,7 @@ int32_t swc_zlib_header_parse(const uint8_t *in, size_t in_len, swc_zlib_header 
 }
 
 int32_t swc_zlib_unarchive(const uint8_t *in, size_t n, uint8_t **out, size_t *out_len) {
-    if (!out || !out_len) return SWC_ERR_INVALID_ARG;
-    *out = nullptr; *out_len = 0;
-    swc_zlib_header zh;
-    { const int hst = zlib_parse(in, n, &zh); if (hst) return hst; }
-    const size_t off = zh.header_len;
-    if (ensure_device()) return SWC_ERR_NO_DEVICE;
-    ApiLock api_lock;
-    DevBuf d_in;
-    int st = upload_input(d_in, in, n);
-    if (st) return st;
-    UnitResult r;
-    if ((st = deflate_unit_device(d_in.as<u8>(), n, off * 8, r))) return st;
-    if (r.status != SWC_OK) return r.status;
-    const size_t p = off + (r.consumed + 7) / 8;
-    int result = SWC_OK;
-    if (n - p < 4) {
-        result = SWC_ZLIB_WRONG_ADLER32;                             // ZlibArchive.swift:34-35 (payload still returned)
-    } else {
-        const uint32_t adler = (uint32_t)in[p] << 24 | (uint32_t)in[p + 1] << 16 | (uint32_t)in[p + 2] << 8 | in[p + 3];
-        u64 got = 0;
-        if ((st = checks::check_device(checks::ADLER32, r.out.as<u8>(), r.out_len, &got))) return st;
-        if ((uint32_t)got != adler) result = SWC_ZLIB_WRONG_ADLER32;
-    }
-    if ((st = to_host_alloc(r.out.p, r.out_len, out, out_len))) return st;
-    return result;
+    return single_unarchive(false, in, n, out, out_len, nullptr);
 }
 
 int32_t swc_crc32_batch(const uint8_t *in_base, const uint64_t *off, const uint64_t *len, const int32_t *status,

@@ -20,8 +20,19 @@ constexpr u32 CHUNK = 4096;
 // GF(2) helpers, the warp CRC and SHA-256: checks_device.cuh
 
 // ---------------------------------------------------------------- chunk kernels
+// The bytes a chunk pass covers: n bytes at data, or, when len is set, one unit of a batch read on the device: *len bytes at
+// data + *off, none when *status is not OK (Deflate reports the size it WOULD need on overflow), and then the result is 0.
+struct Span {
+    const u8 *data;
+    u64 n;
+    const u64 *off, *len;
+    const int32_t *status;
+    __device__ bool skipped() const { return len && *status != SWC_OK; }
+    __device__ u64 size() const { return !len ? n : skipped() ? 0 : *len; }
+};
+
 template <int KIND>   // 0 crc32, 1 bzip2 crc32, 2 crc64, 3 adler32
-__global__ void __launch_bounds__(128) chunk_kernel(const u8 *data, u64 n, u64 *partial) {
+__global__ void __launch_bounds__(128) chunk_kernel(Span sp, u64 *partial) {
     __shared__ u64 tab[256];
     for (u32 i = threadIdx.x; i < 256; i += blockDim.x) {
         if (KIND == 0) { u32 c = i; for (int k = 0; k < 8; k++) c = (c & 1) ? 0xEDB88320u ^ (c >> 1) : c >> 1; tab[i] = c; }
@@ -29,6 +40,8 @@ __global__ void __launch_bounds__(128) chunk_kernel(const u8 *data, u64 n, u64 *
         if (KIND == 2) { u64 c = i; for (int k = 0; k < 8; k++) c = (c & 1) ? 0xC96C5795D7870F42ull ^ (c >> 1) : c >> 1; tab[i] = c; }
     }
     __syncthreads();
+    const u8 *data = sp.len ? sp.data + *sp.off : sp.data;
+    const u64 n = sp.size();
     const u64 chunk = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     const u64 beg = chunk * CHUNK;
     if (beg >= n) return;
@@ -52,9 +65,11 @@ __global__ void __launch_bounds__(128) chunk_kernel(const u8 *data, u64 n, u64 *
     }
 }
 
-template <int KIND>
-__global__ void combine_kernel(const u64 *partial, u64 n, u64 *result) {
+template <int KIND, typename R>
+__global__ void combine_kernel(Span sp, const u64 *partial, R *result) {
+    const u64 n = sp.size();
     const u64 nchunks = (n + CHUNK - 1) / CHUNK;
+    if (sp.skipped()) { *result = 0; return; }
     if (KIND == 3) {
         u64 a = 1, b = 0;                         // CheckSums.swift:48-57
         for (u64 c = 0; c < nchunks; c++) {
@@ -63,7 +78,7 @@ __global__ void combine_kernel(const u64 *partial, u64 n, u64 *result) {
             b = (b + (len % 65521u) * a + s2) % 65521u;
             a = (a + s1) % 65521u;
         }
-        *result = (b << 16) + a;
+        *result = (R)((b << 16) + a);
         return;
     }
     if (nchunks == 0) { *result = 0; return; }    // CRC of the empty string is 0 in all three variants
@@ -78,17 +93,18 @@ __global__ void combine_kernel(const u64 *partial, u64 n, u64 *result) {
         if (KIND == 1) acc = mulmod32n(full ? p32n : xpow32n(len), (u32)acc) ^ (u32)partial[c];
         if (KIND == 2) acc = mulmod64r(full ? p64r : xpow64r(len), acc) ^ partial[c];
     }
-    *result = acc;
+    *result = (R)acc;
 }
 
-template <int KIND>
-static int run(const u8 *d_data, u64 n, u64 *d_result, u64 *d_partial, cudaStream_t s) {
-    const u64 nchunks = (n + CHUNK - 1) / CHUNK;
+// the grid covers `cap` bytes, at least the span's size
+template <int KIND, typename R>
+static int run(const Span &sp, u64 cap, R *d_result, u64 *d_partial, cudaStream_t s) {
+    const u64 nchunks = (cap + CHUNK - 1) / CHUNK;
     if (nchunks) {
-        chunk_kernel<KIND><<<(unsigned)((nchunks + 127) / 128), 128, 0, s>>>(d_data, n, d_partial);
+        chunk_kernel<KIND><<<(unsigned)((nchunks + 127) / 128), 128, 0, s>>>(sp, d_partial);
         count_launch();
     }
-    combine_kernel<KIND><<<1, 1, 0, s>>>(d_partial, n, d_result);
+    combine_kernel<KIND><<<1, 1, 0, s>>>(sp, d_partial, d_result);
     count_launch();
     SWC_CUDA_TRY(cudaGetLastError());
     return SWC_OK;
@@ -96,10 +112,15 @@ static int run(const u8 *d_data, u64 n, u64 *d_result, u64 *d_partial, cudaStrea
 
 size_t partial_bytes(u64 n) { return (size_t)(((n + CHUNK - 1) / CHUNK) + 1) * 8; }
 
-int crc32(const u8 *d, u64 n, u64 *d_result, u64 *d_partial, cudaStream_t s) { return run<0>(d, n, d_result, d_partial, s); }
-int bzip2_crc32(const u8 *d, u64 n, u64 *d_result, u64 *d_partial, cudaStream_t s) { return run<1>(d, n, d_result, d_partial, s); }
-int crc64(const u8 *d, u64 n, u64 *d_result, u64 *d_partial, cudaStream_t s) { return run<2>(d, n, d_result, d_partial, s); }
-int adler32(const u8 *d, u64 n, u64 *d_result, u64 *d_partial, cudaStream_t s) { return run<3>(d, n, d_result, d_partial, s); }
+int crc32(const u8 *d, u64 n, u64 *d_result, u64 *d_partial, cudaStream_t s) { return run<0>(Span{d, n}, n, d_result, d_partial, s); }
+int bzip2_crc32(const u8 *d, u64 n, u64 *d_result, u64 *d_partial, cudaStream_t s) { return run<1>(Span{d, n}, n, d_result, d_partial, s); }
+int crc64(const u8 *d, u64 n, u64 *d_result, u64 *d_partial, cudaStream_t s) { return run<2>(Span{d, n}, n, d_result, d_partial, s); }
+int adler32(const u8 *d, u64 n, u64 *d_result, u64 *d_partial, cudaStream_t s) { return run<3>(Span{d, n}, n, d_result, d_partial, s); }
+int unit_check(Kind k, const u8 *base, const u64 *off, const u64 *len, const int32_t *status, u64 cap, u32 *result, u64 *d_partial,
+               cudaStream_t s) {
+    const Span u{base, 0, off, len, status};
+    return k == CRC32 ? run<0>(u, cap, result, d_partial, s) : run<3>(u, cap, result, d_partial, s);
+}
 
 // ---------------------------------------------------------------- CRC-32 of many buffers: one warp per buffer
 // warp_crc (checks_device.cuh): each lane folds one of 32 contiguous segments (a multiple of 16 bytes, read with 16-byte

@@ -23,6 +23,10 @@ int gather_units(const u8 *src, const u64 *src_off, const u64 *len, u8 *dst, con
 // host convenience: run a 32/64-bit check over a device buffer and fetch the value (blocking)
 enum Kind { CRC32 = 0, BZIP2_CRC32 = 1, CRC64 = 2, ADLER32 = 3, XXH32 = 4 };
 int check_device(Kind k, const u8 *d, u64 n, u64 *value);
+// CRC32 or ADLER32 of one unit of a decode batch, chunked like check_device, its offset, length and status read on the device:
+// the grid covers `cap` >= length bytes, d_partial holds partial_bytes(cap); a unit whose status is not 0 gets 0
+int unit_check(Kind k, const u8 *base, const u64 *off, const u64 *len, const int32_t *status, u64 cap, u32 *result, u64 *d_partial,
+               cudaStream_t s);
 
 }  // namespace checks
 }  // namespace swc

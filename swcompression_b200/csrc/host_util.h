@@ -185,12 +185,12 @@ int decode_unit(UnitTable &t, const UnitCols &c, const u8 *d_in, size_t start, s
     return SWC_OK;
 }
 
-// Deflate stream starting at byte `start` + `start_bit` bits inside d_in[0..in_len)
-int deflate_unit_device(const u8 *d_in, size_t in_len, size_t start_bit_abs, UnitResult &r, size_t hint = 0);
-
 // batched Deflate on device-resident tables (api_deflate.cu); start_bits may be null; scratch == nullptr -> library pool
 int deflate_batch_impl(const DecodeIO &io, const uint8_t *start_bits, uint64_t out_total, void *scratch, size_t scratch_bytes,
                        cudaStream_t stream);
+// the same for GzipArchive / ZlibArchive.unarchive (unarchive_batch.cu); headers may be null (always for zlib)
+int unarchive_batch_impl(bool gzip, const DecodeIO &io, swc_gzip_header *headers, uint64_t out_total, void *scratch,
+                         size_t scratch_bytes, cudaStream_t stream);
 
 // large transfers between pageable host memory and the device: T threads x (stream + two pinned bounce buffers) (runtime.cu)
 int copy_pageable(void *dst, const void *src, size_t bytes, bool to_device);

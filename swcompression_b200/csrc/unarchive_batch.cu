@@ -9,7 +9,8 @@
 //            header status and, for gzip, the caller's swc_gzip_header array;
 //   Deflate  deflate_batch_impl on those columns, unchanged (K1w below 20 000 units, K1L from there, slow kernel, replay),
 //            writing the caller's out_len / status and, in the caller's consumed array, the Deflate bits;
-//   checksum checks::crc32_units (gzip) or checks::adler32_units (zlib) over every unit the Deflate stage decoded;
+//   checksum checks::crc32_units (gzip) or checks::adler32_units (zlib), one warp per unit the Deflate stage decoded; a
+//            one-unit batch (the single calls) spreads its unit over the whole GPU instead (checks::unit_check);
 //   trailer  unarchive_trailer_kernel, one thread per unit: the final status, out_len and consumed in the reference's order.
 #include "../../include/swcgpu.h"
 #include "archive_header.cuh"
@@ -116,11 +117,12 @@ __global__ void __launch_bounds__(256) unarchive_trailer_kernel(const u8 *in_bas
     consumed[i] = used;
 }
 
-int unarchive_batch(bool gzip, const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, uint8_t *out_base,
-                    const uint64_t *out_off, const uint64_t *out_cap, uint64_t out_total, uint64_t *out_len, uint64_t *consumed,
-                    int32_t *status, swc_gzip_header *headers, uint64_t n, void *scratch, size_t scratch_bytes, cudaStream_t stream) {
+}  // namespace
+
+int unarchive_batch_impl(bool gzip, const DecodeIO &io, swc_gzip_header *headers, uint64_t out_total, void *scratch,
+                         size_t scratch_bytes, cudaStream_t stream) {
+    const u64 n = io.n;
     if (n == 0) return SWC_OK;
-    const DecodeIO io{{in_base, in_off, in_len, out_base, out_off, out_cap, out_len, status, n}, consumed};
     if (missing(io)) return SWC_ERR_INVALID_ARG;
     const size_t need = swc_unarchive_batch_scratch_bytes(n, out_total);
     if (!scratch) {
@@ -133,27 +135,31 @@ int unarchive_batch(bool gzip, const uint8_t *in_base, const uint64_t *in_off, c
     const Scratch s = seat(scratch, n, scratch_bytes);
     const unsigned blocks = (unsigned)((n + 255) / 256);
     timing_mark(stream);
-    if (gzip) unarchive_header_kernel<true><<<blocks, 256, 0, stream>>>(in_base, in_off, in_len, s, headers, n);
-    else unarchive_header_kernel<false><<<blocks, 256, 0, stream>>>(in_base, in_off, in_len, s, nullptr, n);
+    if (gzip) unarchive_header_kernel<true><<<blocks, 256, 0, stream>>>(io.in_base, io.in_off, io.in_len, s, headers, n);
+    else unarchive_header_kernel<false><<<blocks, 256, 0, stream>>>(io.in_base, io.in_off, io.in_len, s, nullptr, n);
     count_launch();
     SWC_CUDA_TRY(cudaGetLastError());
     timing_mark(stream);
-    const DecodeIO dio{{in_base, s.d_off, s.d_len, out_base, out_off, out_cap, out_len, status, n}, consumed};
+    const DecodeIO dio{{io.in_base, s.d_off, s.d_len, io.out_base, io.out_off, io.out_cap, io.out_len, io.status, n}, io.consumed};
     int st = deflate_batch_impl(dio, nullptr, out_total, s.inflate, s.inflate_bytes, stream);
     if (st) return st;
-    st = gzip ? checks::crc32_units(out_base, out_off, out_len, status, s.check, n, stream)
-              : checks::adler32_units(out_base, out_off, out_len, status, s.check, n, stream);
+    // one warp would hold a lone large unit back; its out_total / 512 bytes of partials fit the ~1.33 x out_total Deflate scratch
+    if (n == 1)
+        st = checks::unit_check(gzip ? checks::CRC32 : checks::ADLER32, io.out_base, io.out_off, io.out_len, io.status, out_total,
+                                s.check, (u64 *)s.inflate, stream);
+    else
+        st = gzip ? checks::crc32_units(io.out_base, io.out_off, io.out_len, io.status, s.check, n, stream)
+                  : checks::adler32_units(io.out_base, io.out_off, io.out_len, io.status, s.check, n, stream);
     if (st) return st;
     timing_mark(stream);
-    if (gzip) unarchive_trailer_kernel<true><<<blocks, 256, 0, stream>>>(in_base, in_off, in_len, s, out_len, consumed, status, n);
-    else unarchive_trailer_kernel<false><<<blocks, 256, 0, stream>>>(in_base, in_off, in_len, s, out_len, consumed, status, n);
+    if (gzip) unarchive_trailer_kernel<true><<<blocks, 256, 0, stream>>>(io.in_base, io.in_off, io.in_len, s, io.out_len, io.consumed, io.status, n);
+    else unarchive_trailer_kernel<false><<<blocks, 256, 0, stream>>>(io.in_base, io.in_off, io.in_len, s, io.out_len, io.consumed, io.status, n);
     count_launch();
     SWC_CUDA_TRY(cudaGetLastError());
     timing_mark(stream);
     return SWC_OK;
 }
 
-}  // namespace
 }  // namespace swc
 
 using namespace swc;
@@ -170,8 +176,8 @@ int32_t swc_gzip_unarchive_batch(const uint8_t *in_base, const uint64_t *in_off,
                                  uint64_t n, void *scratch, size_t scratch_bytes, void *cuda_stream) {
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
-    return unarchive_batch(true, in_base, in_off, in_len, out_base, out_off, out_cap, out_capacity_total, out_len, consumed_bytes,
-                           status, headers, n, scratch, scratch_bytes, (cudaStream_t)cuda_stream);
+    const DecodeIO io{{in_base, in_off, in_len, out_base, out_off, out_cap, out_len, status, n}, consumed_bytes};
+    return unarchive_batch_impl(true, io, headers, out_capacity_total, scratch, scratch_bytes, (cudaStream_t)cuda_stream);
 }
 
 int32_t swc_zlib_unarchive_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
@@ -180,8 +186,8 @@ int32_t swc_zlib_unarchive_batch(const uint8_t *in_base, const uint64_t *in_off,
                                  uint64_t n, void *scratch, size_t scratch_bytes, void *cuda_stream) {
     if (ensure_device()) return SWC_ERR_NO_DEVICE;
     ApiLock api_lock;
-    return unarchive_batch(false, in_base, in_off, in_len, out_base, out_off, out_cap, out_capacity_total, out_len, consumed_bytes,
-                           status, nullptr, n, scratch, scratch_bytes, (cudaStream_t)cuda_stream);
+    const DecodeIO io{{in_base, in_off, in_len, out_base, out_off, out_cap, out_len, status, n}, consumed_bytes};
+    return unarchive_batch_impl(false, io, nullptr, out_capacity_total, scratch, scratch_bytes, (cudaStream_t)cuda_stream);
 }
 
 }  // extern "C"

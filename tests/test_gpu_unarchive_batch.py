@@ -232,10 +232,13 @@ def test_both_huffman_stages(S, oracle):
 @pytest.mark.parametrize("fmt", ["gzip", "zlib"])
 def test_hostile_layout(S, oracle, fmt):
     """unaligned and back-to-back units, cut archives followed by their own rest, output regions of every capacity residue
-    (exact, 1-15 bytes short: overflow with the size required, 1-15 long) inside sentinel bytes that must stay intact"""
+    (exact, 1-15 bytes short: overflow with the size required, 1-15 long) inside sentinel bytes that must stay intact; then
+    one unit alone, followed by another member's start, in a region far larger than its output (a one-unit batch spreads
+    its checksum over the whole region)"""
     import torch
     from swcompression_b200 import _lib
     rng = random.Random(66 if fmt == "gzip" else 67)
+    make = U.gzip_member if fmt == "gzip" else U.zlib_stream
     units, tails = [], []
     for j in range(90):
         raw = H.textlike(rng.choice([0, 1, 100, 3000, 20000]), 670 + j) if j % 5 else H.random_bytes(rng, rng.randrange(0, 2000))
@@ -249,32 +252,33 @@ def test_hostile_layout(S, oracle, fmt):
             units.append(bytes(b)); tails.append(None)
         else:
             units.append(a); tails.append(b"\x1f\x8b\x08\x00" if j % 2 else None)
-    expect = _expect(oracle, fmt, units)
-    sizes = [len(o) if s in (U.OK,) + U.PAYLOAD_CARRYING else None for s, o, _ in expect]
-    spare = max(len(o) for _, o, _ in expect) + 1024          # a failing unit stops at its error, within what the oracle wrote
-    out_off, out_cap, total = H.fenced_layout(sizes, spare)
-    buf, offs, lens = H.pack_hostile(units, rng, None, tails)
-    n = len(units)
-    d_in, d_off, d_len, d_oo, d_oc = _dev(buf), _dev(offs), _dev(lens), _dev(out_off), _dev(out_cap)
-    d_out = torch.full((total,), H.SENTINEL, dtype=torch.uint8, device="cuda")
-    d_ln, d_used = torch.zeros(n, dtype=torch.int64, device="cuda"), torch.zeros(n, dtype=torch.int64, device="cuda")
-    d_st = torch.full((n,), -1, dtype=torch.int32, device="cuda")
     L = _lib.lib()
-    scratch = torch.empty(L.swc_unarchive_batch_scratch_bytes(n, total), dtype=torch.uint8, device="cuda")
-    args = [_p(d_in), _p(d_off), _p(d_len), _p(d_out), _p(d_oo), _p(d_oc), total, _p(d_ln), _p(d_used), _p(d_st)]
-    if fmt == "gzip":
-        st = L.swc_gzip_unarchive_batch(*args, None, n, _p(scratch), scratch.numel(), _stream())
-    else:
-        st = L.swc_zlib_unarchive_batch(*args, n, _p(scratch), scratch.numel(), _stream())
-    assert st == 0
-    torch.cuda.synchronize()
-    out = d_out.cpu().numpy()
-    stv, lnv, usedv = d_st.cpu().numpy(), d_ln.cpu().numpy(), d_used.cpu().numpy()
-    outs = [bytes(out[int(o):int(o) + int(c)]) for o, c in zip(out_off, out_cap)]
-    bad = _compare(fmt, units, expect, stv, lnv, usedv, outs, caps=out_cap)
-    fence = H.fence_violations(out, out_off, out_cap)
-    assert not bad and fence.size == 0, (bad[:8], fence[:8])
-    assert (stv == 1).sum() > 5
+    for units, tails, alone in ((units, tails, False), ([make(H.textlike(100000, 669))], [b"\x1f\x8b\x08\x00"], True)):
+        expect = _expect(oracle, fmt, units)
+        sizes = [len(o) if s in (U.OK,) + U.PAYLOAD_CARRYING else None for s, o, _ in expect]
+        spare = max(len(o) for _, o, _ in expect) + 1024      # a failing unit stops at its error, within what the oracle wrote
+        out_off, out_cap, total = H.fenced_layout([None] if alone else sizes, 40 * spare if alone else spare)
+        buf, offs, lens = H.pack_hostile(units, rng, None, tails)
+        n = len(units)
+        d_in, d_off, d_len, d_oo, d_oc = _dev(buf), _dev(offs), _dev(lens), _dev(out_off), _dev(out_cap)
+        d_out = torch.full((total,), H.SENTINEL, dtype=torch.uint8, device="cuda")
+        d_ln, d_used = torch.zeros(n, dtype=torch.int64, device="cuda"), torch.zeros(n, dtype=torch.int64, device="cuda")
+        d_st = torch.full((n,), -1, dtype=torch.int32, device="cuda")
+        scratch = torch.empty(L.swc_unarchive_batch_scratch_bytes(n, total), dtype=torch.uint8, device="cuda")
+        args = [_p(d_in), _p(d_off), _p(d_len), _p(d_out), _p(d_oo), _p(d_oc), total, _p(d_ln), _p(d_used), _p(d_st)]
+        if fmt == "gzip":
+            st = L.swc_gzip_unarchive_batch(*args, None, n, _p(scratch), scratch.numel(), _stream())
+        else:
+            st = L.swc_zlib_unarchive_batch(*args, n, _p(scratch), scratch.numel(), _stream())
+        assert st == 0
+        torch.cuda.synchronize()
+        out = d_out.cpu().numpy()
+        stv, lnv, usedv = d_st.cpu().numpy(), d_ln.cpu().numpy(), d_used.cpu().numpy()
+        outs = [bytes(out[int(o):int(o) + int(c)]) for o, c in zip(out_off, out_cap)]
+        bad = _compare(fmt, units, expect, stv, lnv, usedv, outs, caps=out_cap)
+        fence = H.fence_violations(out, out_off, out_cap)
+        assert not bad and fence.size == 0, (alone, bad[:8], fence[:8])
+        assert (stv == 0).all() if alone else (stv == 1).sum() > 5
 
 
 def test_output_overflow_then_rerun(S):
@@ -337,37 +341,41 @@ def test_invalid_arguments(S):
 @pytest.mark.parametrize("fmt", ["gzip", "zlib"])
 def test_graph_capture(S, oracle, fmt):
     """with caller scratch the call is one enqueue: after an eager warm-up it is captured into a CUDA graph and the replay
-    gives the eager results (no host synchronisation or allocation on the path)"""
+    gives the eager results (no host synchronisation or allocation on the path), for a batch of 200 units and for one unit
+    whose capacity is far above its output (the one-unit checksum path)"""
     import torch
     rng = random.Random(70)
+    make = (lambda raw: U.gzip_member(raw, name=b"g")) if fmt == "gzip" else U.zlib_stream
     datas = []
     for j in range(200):
         raw = H.textlike(rng.randrange(0, 8000), 700 + j)
-        a = bytearray(U.gzip_member(raw, name=b"g") if fmt == "gzip" else U.zlib_stream(raw))
+        a = bytearray(make(raw))
         if j % 7 == 3:
             a[-2] ^= 4
         datas.append(bytes(a[:len(a) - 3] if j % 11 == 5 else a))
-    expect = _expect(oracle, fmt, datas)
+    one = make(H.textlike(300000, 699))
     from swcompression_b200.batch import Batch
-    b = Batch.from_units(fmt, datas, _caps(expect), headers=True)
-    b.run()
-    st0, ln0, used0 = b.results()
-    outs0 = b.outputs()
-    assert not _compare(fmt, datas, expect, st0, ln0, used0, outs0)
-    h0 = b.d_headers.clone() if b.d_headers is not None else None
-    b.d_status.fill_(-1); b.d_out_len.zero_(); b.d_consumed.zero_(); b.d_out.zero_()
-    if h0 is not None:
-        b.d_headers.zero_()
-    torch.cuda.synchronize()
-    s = torch.cuda.Stream()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.stream(s):
-        with torch.cuda.graph(g, stream=s):
-            b.run()
-    torch.cuda.synchronize()
-    assert (b.d_status.cpu().numpy() == -1).all()          # captured, not run
-    g.replay()
-    st1, ln1, used1 = b.results()
-    assert (st1 == st0).all() and (ln1 == ln0).all() and (used1 == used0).all() and b.outputs() == outs0
-    if h0 is not None:
-        assert torch.equal(b.d_headers, h0)
+    for datas, caps in ((datas, None), ([one], np.array([64 * len(one)], dtype=np.uint64))):
+        expect = _expect(oracle, fmt, datas)
+        b = Batch.from_units(fmt, datas, _caps(expect) if caps is None else caps, headers=True)
+        b.run()
+        st0, ln0, used0 = b.results()
+        outs0 = b.outputs()
+        assert not _compare(fmt, datas, expect, st0, ln0, used0, outs0)
+        h0 = b.d_headers.clone() if b.d_headers is not None else None
+        b.d_status.fill_(-1); b.d_out_len.zero_(); b.d_consumed.zero_(); b.d_out.zero_()
+        if h0 is not None:
+            b.d_headers.zero_()
+        torch.cuda.synchronize()
+        s = torch.cuda.Stream()
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.stream(s):
+            with torch.cuda.graph(g, stream=s):
+                b.run()
+        torch.cuda.synchronize()
+        assert (b.d_status.cpu().numpy() == -1).all()          # captured, not run
+        g.replay()
+        st1, ln1, used1 = b.results()
+        assert (st1 == st0).all() and (ln1 == ln0).all() and (used1 == used0).all() and b.outputs() == outs0
+        if h0 is not None:
+            assert torch.equal(b.d_headers, h0)
