@@ -332,6 +332,35 @@ int32_t swc_bzip2_decompress_batch(const uint8_t *in_base, const uint64_t *in_of
                                    uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
                                    uint64_t *out_len, uint64_t *consumed_bits, int32_t *status,
                                    uint64_t n, void *cuda_stream);
+/* One .bz2 stream per unit with the blocks of every stream decoded side by side, device memory, one asynchronous enqueue on
+ * `cuda_stream`.  Unit i is in_base[in_off[i] ..+ in_len[i]) in the layout above, decoded as BZip2.decompress(data:) decodes
+ * it: the first stream, the bytes behind it ignored (multi-stream input: swc_bzip2_multi_decompress).
+ *   Equality: for every unit and capacity, status[i] is what swc_bzip2_decompress_batch returns for the same unit and
+ *     capacity; on SWC_OK and SWC_BZIP2_WRONG_CRC the bytes [0, out_len[i]) and consumed_bits[i] are equal too.
+ *   Overflow: the one exception is out_len[i] on SWC_ERR_OUTPUT_OVERFLOW.  When the stream validated block-parallel it is
+ *     the exact decoded size, so one rerun with that capacity succeeds; otherwise it is the lower bound the stream kernel
+ *     reports.  consumed_bits[i] is 0 on a validated overflow.
+ *   Block table: max_blocks > 0 is its capacity (at most 2^32 - 1).  A stream whose block candidates (block magics at any
+ *     bit from bit 32 up to its first end-of-stream magic) do not fit in what is left of the table, or whose header, first
+ *     block or end magic is not where a valid stream has them, is decoded by the stream kernel: max_blocks changes the
+ *     speed, never the results.  With a caller scratch the call reads nothing back and allocates nothing, and its launches
+ *     depend only on (n, max_blocks, scratch_bytes), so it can be captured in a CUDA graph.  max_blocks == 0 lets the
+ *     library count the candidates and the stream kernel's scratch first (one synchronisation).
+ *   Scratch: scratch == NULL takes the library pool.  With a caller scratch of swc_bzip2_stream_batch_scratch_bytes(n,
+ *     max_blocks, sum of out_cap) bytes every unit gets its exact status; with max_blocks == 0 the library then keeps the
+ *     block table to what that scratch holds beside every unit's fallback.  A smaller scratch runs the block stage in
+ *     several slices; it must hold the tables and one block slot (about 16 MB), else the call returns SWC_ERR_INVALID_ARG.
+ *     Units are taken in order: a stream goes through the block stage only if the stream kernel's scratch (about 7.5 x
+ *     out_cap[i]) would still fit for it and every unit in front of it; otherwise the stream kernel decodes it.  A unit whose
+ *     stream-kernel scratch no longer fits reports SWC_ERR_UNSUPPORTED with out_len[i] = consumed_bits[i] = 0, and nothing
+ *     is written in its region.
+ *   Writes: nothing is written outside [out_off[i], out_off[i] + out_cap[i]). */
+size_t  swc_bzip2_stream_batch_scratch_bytes(uint64_t n, uint64_t max_blocks, uint64_t out_capacity_total);
+int32_t swc_bzip2_stream_decompress_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                                          uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                          uint64_t *out_len, uint64_t *consumed_bits, int32_t *status,
+                                          uint64_t n, uint64_t max_blocks,
+                                          void *scratch, size_t scratch_bytes, void *cuda_stream);
 
 /* ---- LZMA / LZMA2 -------------------------------------------------------------------------------------------
  * LZMA.decompress(data:)                                   Sources/LZMA/LZMA.swift:25-34

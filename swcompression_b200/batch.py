@@ -59,9 +59,17 @@ def pack_units(units, align=16):
 
 
 class Batch:
-    """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'lzma2', 'gzip', 'zlib', 'xz',
+    """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'bzip2_stream', 'lzma2', 'gzip', 'zlib', 'xz',
     'lz4_frame', 'lz4_block_compress', 'lz4_frame_compress', 'deflate_compress', 'gzip_archive', 'zlib_archive',
     'bzip2_compress').
+
+    'bzip2' and 'bzip2_stream' both decode the first .bz2 stream of each unit (BZip2.decompress(data:), BZip2.swift:50-95)
+    with the same statuses, bytes and consumed bits.  'bzip2' gives each stream one warp and reads the capacities back
+    first; 'bzip2_stream' decodes the blocks of all streams side by side and, on overflow of a stream whose blocks
+    validated, reports its exact size.  `max_blocks` is the capacity of its block table: with it the batch owns a scratch
+    of swc_bzip2_stream_batch_scratch_bytes (capped at `scratch_bytes`, which the library then runs in slices) and run()
+    reads nothing back (it can be captured in a CUDA graph).  None lets the library count the blocks first (one
+    synchronisation) and use its pool, or `scratch_bytes` of caller scratch.
 
     'gzip' / 'zlib' decode one archive per unit (GzipArchive.unarchive, GzipArchive.swift:38-47, 79-100 / ZlibArchive.unarchive,
     ZlibArchive.swift:25-42): the first member only, whose status, size and consumed bytes results() returns.  With
@@ -125,7 +133,14 @@ class Batch:
         self.d_dict_off = self.d_dict_len = None
         self.block_size = int(block_size) if block_size is not None else LZ4_FRAME_BLOCK_SIZE if codec == "lz4_frame_compress" else 1
         self.dict_id, self.max_blocks = dict_id, 0 if max_blocks is None else int(max_blocks)
-        if codec == "lz4_frame":
+        if codec == "bzip2_stream":
+            self.d_aux = None
+            if self.max_blocks or scratch_bytes is not None:
+                nbytes = _lib.lib().swc_bzip2_stream_batch_scratch_bytes(self.n, self.max_blocks, self.out_total)
+                if scratch_bytes is not None:
+                    nbytes = min(nbytes, int(scratch_bytes))
+                self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        elif codec == "lz4_frame":
             # an empty dictionary is still a dictionary: one spare byte keeps its pointer non-null
             self.dict_len = 0 if aux is None else len(aux)
             self.d_aux = None if aux is None else t(np.frombuffer(bytes(aux) + b"\0", dtype=np.uint8).copy())
@@ -266,6 +281,12 @@ class Batch:
         elif self.codec == "bzip2":
             st = L.swc_bzip2_decompress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out), p(self.d_out_off),
                                               p(self.d_out_cap), p(self.d_out_len), p(self.d_consumed), p(self.d_status), self.n, stream)
+        elif self.codec == "bzip2_stream":
+            opt = lambda t: None if t is None else p(t)
+            st = L.swc_bzip2_stream_decompress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out),
+                                                     p(self.d_out_off), p(self.d_out_cap), p(self.d_out_len), p(self.d_consumed),
+                                                     p(self.d_status), self.n, self.max_blocks, opt(self.d_scratch),
+                                                     0 if self.d_scratch is None else self.d_scratch.numel(), stream)
         elif self.codec == "lzma2":
             st = L.swc_lzma2_decompress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_aux), p(self.d_out), p(self.d_out_off),
                                               p(self.d_out_cap), p(self.d_out_len), p(self.d_consumed), p(self.d_status), self.n, stream)
@@ -276,7 +297,7 @@ class Batch:
 
     def results(self):
         """-> (status int32[n], out_len int64[n], consumed int64[n]) on the host (synchronises).  consumed is in bits for
-        'deflate' and 'bzip2', in bytes for 'lzma2', 'gzip', 'zlib' and 'lz4_frame', and 0 for 'xz' and the compress codecs."""
+        'deflate', 'bzip2' and 'bzip2_stream', in bytes for 'lzma2', 'gzip', 'zlib' and 'lz4_frame', and 0 for 'xz' and the compress codecs."""
         torch.cuda.synchronize(self.device)
         return self.d_status.cpu().numpy(), self.d_out_len.cpu().numpy(), self.d_consumed.cpu().numpy()
 

@@ -24,11 +24,6 @@ constexpr int MAX_LEN = 20;
 constexpr int NCH = 4;           // chains a lane keeps in flight in the chase (8 measured slower: one warp is issue-latency-bound on the bookkeeping)
 constexpr int NSEG = 512;        // chain pieces of the inverse BWT (see the chase)
 
-// Room for a block's BWT text (the RLE1 form) when the unit may write `cap` output bytes.  RLE1 turns every run of four
-// equal bytes into five, so a block that fits `cap` bytes of output can carry up to 5/4 x cap + 4 bytes of text; sizing the
-// text by `cap` alone reported overflow for units whose output fits exactly.
-__host__ __device__ __forceinline__ u64 bwt_capacity(u64 cap) { return (cap + (cap >> 2) + 8 + 3) & ~3ull; }
-
 struct WarpSmem {
     u16 syms[6][MAX_SYMS + 2];      // symbols sorted by (length, symbol) per table
     u32 limit[6][32];               // limit[t][L-1] = left-justified (20-bit) end of the length-L code range; [20..31] = 1<<20
@@ -176,7 +171,7 @@ __global__ void __launch_bounds__(WARPS * 32) bzip2_kernel(Args a) {
     __shared__ WarpSmem smem[WARPS];
     const u32 lane = lane_id(), warp = threadIdx.x >> 5;
     const u64 unit = (u64)blockIdx.x * WARPS + warp;
-    if (unit >= a.n) return;
+    if (unit >= a.n || (a.run && !a.run[unit])) return;
     WarpSmem &S = smem[warp];
     const u64 cap = a.out_cap[unit];
     u8 *out = a.out_base + a.out_off[unit];
@@ -580,12 +575,6 @@ done:
         a.consumed[unit] = (u64)(total_bits - br.avail);
         a.status[unit] = status;
     }
-}
-
-size_t scratch_per_unit(u64 cap) {
-    const u64 scr_cap = bwt_capacity(cap);
-    // bwt | succ (u32) | selectors | text
-    return (size_t)(scr_cap + 16 + scr_cap * 4 + 16 + 32768 + 16 + scr_cap + 256 + 255) & ~(size_t)255;
 }
 
 int launch(const Args &a, cudaStream_t stream) {

@@ -265,15 +265,12 @@ __global__ void __launch_bounds__(256) bzip2_magic_scan_kernel(const u8 *d, u64 
     u64 w = 0;
 #pragma unroll
     for (int k = 0; k < 7; k++) w = (w << 8) | (i + k < n ? d[i + k] : 0);   // bits of bytes i..i+6, MSB first
-#pragma unroll
-    for (int b = 0; b < 8; b++) {
-        if (i * 8 + b + 48 > n * 8) break;
-        const u64 v = (w >> (8 - b)) & 0xFFFFFFFFFFFFull;
-        const bool blk = v == 0x314159265359ull, eos = v == 0x177245385090ull;
-        if (blk || eos) {
-            const u64 slot = atomicAdd(count, 1ull);
-            if (slot < cap) list[slot] = ((i * 8 + b) << 1) | (eos ? 1u : 0u);
-        }
+    u32 blk, eos;
+    bzip2_magics_in_byte(w, (int)min((n - i) * 8 - 47, (u64)8), &blk, &eos);
+    for (u32 m = blk | eos; m; m &= m - 1) {
+        const u32 b = __ffs(m) - 1;
+        const u64 slot = atomicAdd(count, 1ull);
+        if (slot < cap) list[slot] = ((i * 8 + b) << 1) | ((eos >> b) & 1u);
     }
 }
 

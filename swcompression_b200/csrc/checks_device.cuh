@@ -8,6 +8,24 @@
 namespace swc {
 namespace checks {
 
+// ---------------------------------------------------------------- BZip2 magics at every bit offset
+// BZip2.swift:71-90 reads the 48-bit block magic 0x314159265359 or end-of-stream magic 0x177245385090 from wherever the
+// previous block ended, so a magic may start at any bit.  w holds bytes i .. i+6 MSB first (byte i in bits 55..48); a magic
+// starts at bit b (0 = the byte's most significant bit) of byte i when the 48 bits from there match.  Only the first
+// `limit` offsets are tested (fewer than 8 where the data ends inside the 48 bits).  Bit b of *blk / *eos = a match at b.
+__device__ __forceinline__ void bzip2_magics_in_byte(u64 w, int limit, u32 *blk, u32 *eos) {
+    u32 mb = 0, me = 0;
+#pragma unroll
+    for (int b = 0; b < 8; b++) {
+        const u64 v = (w >> (8 - b)) & 0xFFFFFFFFFFFFull;
+        if (b < limit) {
+            mb |= (u32)(v == 0x314159265359ull) << b;
+            me |= (u32)(v == 0x177245385090ull) << b;
+        }
+    }
+    *blk = mb; *eos = me;
+}
+
 // ---------------------------------------------------------------- GF(2) helpers
 // reflected 32-bit: bit 31 = x^0
 __device__ inline u32 mulmod32r(u32 a, u32 b) {
