@@ -12,6 +12,7 @@
  *   GzipError     Sources/GZip/GzipError.swift:10-35
  *   ZlibError     Sources/Zlib/ZlibError.swift:12-26
  *   XZError       Sources/XZ/XZError.swift:12-48
+ *   TarError      Sources/TAR/TarError.swift:10-18
  */
 #ifndef SWC_STATUS_H
 #define SWC_STATUS_H
@@ -97,7 +98,13 @@ enum swc_status {
     SWC_ZIP_COMPRESSION_NOT_SUPPORTED  = 908,
     SWC_ZIP_WRONG_LOCAL_HEADER         = 909,
     SWC_ZIP_WRONG_CRC                  = 910,  /* payload-carrying: the entries processed so far, the failing one last */
-    SWC_ZIP_WRONG_TEXT_FIELD           = 911
+    SWC_ZIP_WRONG_TEXT_FIELD           = 911,
+
+    /* TarError, Sources/TAR/TarError.swift:10-18 */
+    SWC_TAR_TOO_SMALL_FILE_IS_PASSED = 1001,
+    SWC_TAR_WRONG_FIELD              = 1002,
+    SWC_TAR_WRONG_HEADER_CHECKSUM    = 1003,
+    SWC_TAR_WRONG_PAX_HEADER_ENTRY   = 1004
 };
 
 #endif /* SWC_STATUS_H */

@@ -506,6 +506,67 @@ typedef struct swc_zip_entry {
 int32_t swc_zip_open(const uint8_t *in, size_t in_len, uint8_t **out, size_t *out_len, swc_zip_entry **entries, size_t *n_entries);
 int32_t swc_zip_info(const uint8_t *in, size_t in_len, swc_zip_entry **entries, size_t *n_entries);
 
+/* ---- TAR container -------------------------------------------------------------------------------------------
+ * TarContainer.open(container:) -> [TarEntry]         Sources/TAR/TarContainer.swift:187-224
+ * TarContainer.info(container:) -> [TarEntryInfo]     Sources/TAR/TarContainer.swift:239-261
+ * TarContainer.formatOf(container:) -> Format         Sources/TAR/TarContainer.swift:36-71
+ * All three drive TarParser.next() (TarParser.swift:35-79).  One record per non-special header, in walk order, holding
+ * what TarEntryInfo.init (TarEntryInfo.swift:184-242) resolves.  Offsets are relative to the unit's first byte; text
+ * fields are byte ranges into the unit, already resolved to the winning source (local PAX, global PAX, GNU L / K entry,
+ * header).  The host decodes text (String(cString:) repair), converts PAX times with Double(String) and splits the
+ * extended-header payloads into the unknown records. */
+enum {
+    SWC_TAR_MODE = 1u << 0, SWC_TAR_UID = 1u << 1, SWC_TAR_GID = 1u << 2, SWC_TAR_DEV_MAJOR = 1u << 3,
+    SWC_TAR_DEV_MINOR = 1u << 4, SWC_TAR_MTIME = 1u << 5, SWC_TAR_ATIME = 1u << 6, SWC_TAR_CTIME = 1u << 7,
+    SWC_TAR_UNAME = 1u << 8, SWC_TAR_GNAME = 1u << 9, SWC_TAR_CHARSET = 1u << 10, SWC_TAR_COMMENT = 1u << 11,
+    SWC_TAR_LOCAL = 1u << 12, SWC_TAR_GLOBAL = 1u << 13, SWC_TAR_PREFIX = 1u << 14,
+    SWC_TAR_PAX_TIME0 = 1u << 16               /* << k for pax_time[k], k = 0..5 */
+};
+enum { SWC_TAR_PRE_POSIX = 0, SWC_TAR_USTAR = 1, SWC_TAR_GNU = 2, SWC_TAR_PAX = 3 };   /* TarContainer.Format */
+typedef struct swc_tar_entry {
+    uint64_t header_off, data_off;       /* the entry's header; its data starts 512 bytes later */
+    int64_t  size;                       /* TarEntryInfo.size as info reports it: PAX size when given, else the header's */
+    int64_t  open_size;                  /* as open reports it: 0 for directories (their data is nil) */
+    int64_t  mode;                       /* permissions (& 0xFFF); SWC_TAR_MODE */
+    int64_t  uid, gid;                   /* ownerID / groupID, resolved; SWC_TAR_UID / SWC_TAR_GID */
+    int64_t  dev_major, dev_minor;       /* header only (ustar / GNU magic) */
+    int64_t  mtime, atime, ctime;        /* the header's times as integers (atime / ctime: GNU only) */
+    uint64_t name_off, name_len;         /* winning name; with SWC_TAR_PREFIX the header's prefix goes in front */
+    uint64_t prefix_off, prefix_len;
+    uint64_t link_off, link_len;         /* winning linkName */
+    uint64_t uname_off, uname_len, gname_off, gname_len, charset_off, charset_len, comment_off, comment_len;
+    uint64_t pax_time_off[6], pax_time_len[6];  /* last UTF-8 value of mtime, atime, ctime: local 0-2, global 3-5 */
+    uint64_t local_off, local_len, global_off, global_len;  /* extended-header payloads in force (unknown records) */
+    uint32_t present;                    /* SWC_TAR_* bits */
+    uint8_t  typeflag;                   /* raw typeflag byte (ContainerEntryType+Tar.swift) */
+    uint8_t  reserved[3];
+} swc_tar_entry;
+/* Walks units in_base[in_off[i] ..+ in_len[i]) (device memory, any alignment), one warp each, asynchronous on
+ * `cuda_stream`; it reads nothing back and can be captured in a CUDA graph.  Two optional columns (NULL: absent) let the
+ * units be another batch's outputs as that batch left them (out_off, out_len, out_cap, status):
+ *   in_cap[i]     the unit is at most in_cap[i] bytes: the walk never reads past min(in_len[i], in_cap[i]), so an
+ *                 out_len that reports a required size past the capacity (SWC_ERR_OUTPUT_OVERFLOW) stays in its region;
+ *   in_status[i]  a unit whose status is not SWC_OK is not walked: it reports 0 records and that status in info_status,
+ *                 open_status and format_status (the archive was never produced, so there is nothing to open).
+ * Unit i writes up to entry_cap[i] records at entries[entry_off[i] ..) and reports:
+ *   n_entries[i]      the records the walk produced (also when more than entry_cap[i]);
+ *   info_status[i]    info's status: SWC_OK, a TarError, or SWC_ERR_REFERENCE_TRAP where the reference traps or never
+ *                     returns (DESIGN §6); SWC_ERR_OUTPUT_OVERFLOW when it would be SWC_OK but the table is too small;
+ *   open_status[i]    open's status: info's, unless an earlier entry fails open's data bound (tooSmallFileIsPassed) or
+ *                     its data range is inverted or overflows (trap); overflow as for info;
+ *   format[i], format_status[i]  formatOf's result (SWC_TAR_*) and status; formatOf returns early, so it never reports
+ *                     an error behind the point where it returns.
+ * in_len[i] / 512 + 1 records suffice for every archive without a negative size. */
+int32_t swc_tar_walk_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                           const uint64_t *in_cap, const int32_t *in_status, swc_tar_entry *entries, const uint64_t *entry_off, const uint64_t *entry_cap,
+                           uint64_t *n_entries, int32_t *info_status, int32_t *open_status, int32_t *format,
+                           int32_t *format_status, uint64_t n, void *cuda_stream);
+/* The one-unit batch on a host container.  *entries (swc_alloc'ed, free with swc_free) is filled on SWC_OK; open's
+ * entry data is in[data_off ..+ open_size), nothing is copied.  swc_tar_format stores the format only on SWC_OK. */
+int32_t swc_tar_info(const uint8_t *in, size_t in_len, swc_tar_entry **entries, size_t *n_entries);
+int32_t swc_tar_open(const uint8_t *in, size_t in_len, swc_tar_entry **entries, size_t *n_entries);
+int32_t swc_tar_format(const uint8_t *in, size_t in_len, int32_t *format);
+
 /* ---- checks (device-side, used by the wrappers; exposed for the shim and the tests) ---------------------------
  * CheckSums.crc32 / bzip2crc32 / crc64 / adler32   Sources/Common/CheckSums.swift:12-57
  * XxHash32.hash                                     Sources/LZ4/XxHash32.swift:24-83

@@ -42,6 +42,29 @@ class Lz4FrameInfo(C.Structure):
                 ("frame_end", C.c_uint64)]
 
 
+class TarEntry(C.Structure):
+    """swc_tar_entry (include/swcgpu.h)"""
+    _fields_ = ([(f, C.c_uint64) for f in ("header_off", "data_off")]
+                + [(f, C.c_int64) for f in ("size", "open_size", "mode", "uid", "gid", "dev_major", "dev_minor", "mtime",
+                                            "atime", "ctime")]
+                + [(f, C.c_uint64) for f in ("name_off", "name_len", "prefix_off", "prefix_len", "link_off", "link_len",
+                                             "uname_off", "uname_len", "gname_off", "gname_len", "charset_off",
+                                             "charset_len", "comment_off", "comment_len")]
+                + [("pax_time_off", C.c_uint64 * 6), ("pax_time_len", C.c_uint64 * 6)]
+                + [(f, C.c_uint64) for f in ("local_off", "local_len", "global_off", "global_len")]
+                + [("present", C.c_uint32), ("typeflag", C.c_uint8), ("reserved", C.c_uint8 * 3)])
+
+
+def tar_record(e):
+    """swc_tar_entry -> dict of its fields (arrays as tuples, the reserved bytes dropped)"""
+    out = {}
+    for name, _ in TarEntry._fields_:
+        if name != "reserved":
+            v = getattr(e, name)
+            out[name] = tuple(v) if hasattr(v, "__len__") else int(v)
+    return out
+
+
 def lib():
     global _LIB
     if _LIB is None:
@@ -134,6 +157,10 @@ def lib():
         L.swc_xz_occupancy.argtypes = [vp, vp]
         L.swc_crc64_batch.argtypes = [vp, vp, vp, vp, vp, u64, vp]
         L.swc_xz_split_unarchive.argtypes = [vp, sz, C.POINTER(vp), szp, C.POINTER(vp), szp]
+        L.swc_tar_walk_batch.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, u64, vp]
+        L.swc_tar_info.argtypes = [vp, sz, C.POINTER(vp), szp]
+        L.swc_tar_open.argtypes = [vp, sz, C.POINTER(vp), szp]
+        L.swc_tar_format.argtypes = [vp, sz, C.POINTER(i32)]
         for name in ("swc_crc32", "swc_bzip2_crc32", "swc_adler32", "swc_xxh32", "swc_crc64", "swc_sha256"):
             getattr(L, name).argtypes = [vp, sz, vp]
         _LIB = L

@@ -20,6 +20,7 @@ meaning, same error cases), routed through the C ABI of libswcgpu.so.
 import ctypes as C
 import datetime
 import enum
+import re
 from dataclasses import dataclass, field
 
 from . import _lib
@@ -510,6 +511,173 @@ class ZipContainer:
         if st != 0:
             raise error_for(st, entries if st in _PAYLOAD_CODES else None)
         return entries
+
+
+# ---- TAR (Sources/TAR) ----
+_TAR_TYPES = {0: "regular", 48: "regular", 49: "hardLink", 50: "symbolicLink", 51: "characterSpecial", 52: "blockSpecial",
+              53: "directory", 54: "fifo", 55: "contiguous"}                       # ContainerEntryType+Tar.swift:9-32
+_TAR_FORMATS = ["prePosix", "ustar", "gnu", "pax"]
+_PAX_KNOWN = {b"uid", b"gid", b"uname", b"gname", b"size", b"atime", b"ctime", b"mtime", b"path", b"linkpath", b"charset",
+              b"comment"}                                                           # TarExtendedHeader.swift:67-91
+_DEC = re.compile(r"[+-]?([0-9]+\.?[0-9]*|\.[0-9]+)([eE][+-]?[0-9]+)?")
+_HEX = re.compile(r"[+-]?0[xX]([0-9a-fA-F]+\.?[0-9a-fA-F]*|\.[0-9a-fA-F]+)([pP][+-]?[0-9]+)?")
+_INF = re.compile(r"[+-]?(inf|infinity)", re.I)
+_NAN = re.compile(r"[+-]?nan(\([0-9A-Za-z_]*\))?", re.I)
+
+
+def swift_double(text):
+    """Swift's Double(String) as the reference's PAX times use it (TarExtendedHeader.swift:78-83): the C string of the
+    text (cut at its first NUL) parsed by strtod in the C locale, refused when empty, when it starts with whitespace, when
+    strtod leaves bytes behind, and when the value overflows to infinity or underflows to zero.  -> float or None"""
+    text = text.split("\0", 1)[0]
+    if not text or text[0] in " \t\n\v\f\r":
+        return None
+    if _INF.fullmatch(text):
+        return float("-inf") if text[0] == "-" else float("inf")
+    if _NAN.fullmatch(text):
+        return float("nan")
+    m = _HEX.fullmatch(text)
+    if m:
+        try:
+            v = float.fromhex(text)
+        except OverflowError:
+            return None
+        return None if v == 0 and any(c not in "0." for c in m.group(1)) else v
+    m = _DEC.fullmatch(text)
+    if not m:
+        return None
+    v = float(text)
+    if v in (float("inf"), float("-inf")):
+        return None
+    return None if v == 0 and any(c not in "0." for c in m.group(1)) else v
+
+
+def _pax_unknown(payload):
+    """the unknown records of an extended header the walk already accepted (TarExtendedHeader.swift:34-95)"""
+    out, i = {}, 0
+    while i < len(payload):
+        sp = payload.index(b" ", i)
+        length = int(payload[i:sp])
+        eq = payload.index(b"=", sp + 1)
+        key, vs = payload[sp + 1:eq], eq + 1
+        ve = max(vs, i + length - 1)
+        value, i = payload[vs:ve], ve + 1
+        try:
+            value = value.decode("utf-8")
+        except UnicodeDecodeError:
+            continue
+        if key not in _PAX_KNOWN:
+            out[key.decode("utf-8")] = value
+    return out
+
+
+@dataclass
+class TarEntryInfo:
+    """Sources/TAR/TarEntryInfo.swift:9-242; times are seconds since 1970 (Date(timeIntervalSince1970:))"""
+    name: str
+    size: int
+    type: str
+    linkName: str = ""
+    accessTime: float = None
+    creationTime: float = None
+    modificationTime: float = None
+    permissions: int = None
+    ownerID: int = None
+    groupID: int = None
+    ownerUserName: str = None
+    ownerGroupName: str = None
+    deviceMajorNumber: int = None
+    deviceMinorNumber: int = None
+    charset: str = None
+    comment: str = None
+    unknownExtendedHeaderRecords: dict = None
+    compressionMethod: str = "copy"
+
+
+@dataclass
+class TarEntry:
+    """Sources/TAR/TarEntry.swift"""
+    info: TarEntryInfo
+    data: bytes = None
+
+
+def tar_entry_info(data, r):
+    """TarEntryInfo of one swc_tar_entry record (a dict, _lib.tar_record) of the archive `data`: the device resolved the
+    sources, the host decodes the text (String(cString:) repair), the PAX times and the unknown records."""
+    def text(o, n):
+        return bytes(data[o:o + n]).decode("utf-8", "replace")
+    pr = r["present"]
+    opt = lambda bit, v: v if pr & bit else None
+    name = text(r["name_off"], r["name_len"])
+    if pr & (1 << 14):
+        prefix = text(r["prefix_off"], r["prefix_len"])
+        name = prefix + name if prefix.endswith("/") else prefix + "/" + name
+    times = []
+    for k, header_bit, header_value in ((0, 1 << 5, r["mtime"]), (1, 1 << 6, r["atime"]), (2, 1 << 7, r["ctime"])):
+        t = None
+        for j in (k, k + 3):                                                         # local, then global
+            if t is None and pr & (1 << (16 + j)):
+                t = swift_double(text(r["pax_time_off"][j], r["pax_time_len"][j]))
+        times.append(t if t is not None else float(header_value) if pr & header_bit else None)
+    unknown = None
+    if pr & (1 << 13):
+        unknown = _pax_unknown(bytes(data[r["global_off"]:r["global_off"] + r["global_len"]]))
+    if pr & (1 << 12):
+        local = _pax_unknown(bytes(data[r["local_off"]:r["local_off"] + r["local_len"]]))
+        unknown = dict(unknown or {}, **local)
+    return TarEntryInfo(
+        name=name, size=r["size"], type=_TAR_TYPES.get(r["typeflag"], "unknown"), linkName=text(r["link_off"], r["link_len"]),
+        modificationTime=times[0], accessTime=times[1], creationTime=times[2], permissions=opt(1, r["mode"]),
+        ownerID=opt(1 << 1, r["uid"]), groupID=opt(1 << 2, r["gid"]),
+        ownerUserName=text(r["uname_off"], r["uname_len"]) if pr & (1 << 8) else None,
+        ownerGroupName=text(r["gname_off"], r["gname_len"]) if pr & (1 << 9) else None,
+        deviceMajorNumber=opt(1 << 3, r["dev_major"]), deviceMinorNumber=opt(1 << 4, r["dev_minor"]),
+        charset=text(r["charset_off"], r["charset_len"]) if pr & (1 << 10) else None,
+        comment=text(r["comment_off"], r["comment_len"]) if pr & (1 << 11) else None, unknownExtendedHeaderRecords=unknown)
+
+
+def tar_entry(data, r):
+    """TarEntry as open returns it: directories have size 0 and no data (TarContainer.swift:197-211)"""
+    info = tar_entry_info(data, r)
+    if info.type == "directory":
+        info.size = 0
+        return TarEntry(info, None)
+    return TarEntry(info, bytes(data[r["data_off"]:r["data_off"] + r["open_size"]]))
+
+
+def _tar_records(fn, data):
+    buf, n = _lib.inbuf(data)
+    es, cnt = C.c_void_p(), C.c_size_t(0)
+    st = getattr(_lib.lib(), fn)(buf, n, C.byref(es), C.byref(cnt))
+    try:
+        check(st)
+        arr = C.cast(es, C.POINTER(_lib.TarEntry))
+        return [_lib.tar_record(arr[i]) for i in range(cnt.value)]
+    finally:
+        if es.value:
+            _lib.lib().swc_free(es)
+
+
+class TarContainer:
+    """Sources/TAR/TarContainer.swift:9-263 (reading)"""
+
+    @staticmethod
+    def info(container):
+        data = bytes(container)
+        return [tar_entry_info(data, r) for r in _tar_records("swc_tar_info", data)]
+
+    @staticmethod
+    def open(container):
+        data = bytes(container)
+        return [tar_entry(data, r) for r in _tar_records("swc_tar_open", data)]
+
+    @staticmethod
+    def formatOf(container):
+        """-> "prePosix" | "ustar" | "gnu" | "pax" (TarContainer.Format)"""
+        buf, n = _lib.inbuf(bytes(container))
+        f = C.c_int32(0)
+        check(_lib.lib().swc_tar_format(buf, n, C.byref(f)))
+        return _TAR_FORMATS[f.value]
 
 
 # ---- checks (CheckSums.swift / XxHash32.swift / Sha256.swift) ----

@@ -61,7 +61,12 @@ def pack_units(units, align=16):
 class Batch:
     """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'bzip2_stream', 'lzma2', 'gzip', 'zlib', 'xz',
     'lz4_frame', 'lz4_block_compress', 'lz4_frame_compress', 'deflate_compress', 'gzip_archive', 'zlib_archive',
-    'bzip2_compress').
+    'bzip2_compress', 'tar').
+
+    'tar' walks one TAR archive per unit (TarContainer.open / info / formatOf, TarContainer.swift:36-261) into a table of
+    swc_tar_entry records; `out_cap` is each unit's record capacity (None: in_len // 512 + 1).  results() gives info's
+    status and the record count, tar_results() every column, records(i) / entries(i) unit i's records.  Batch.tar_of
+    walks another batch's outputs where they lie.  run() reads nothing back (it can be captured in a CUDA graph).
 
     'bzip2' and 'bzip2_stream' both decode the first .bz2 stream of each unit (BZip2.decompress(data:), BZip2.swift:50-95)
     with the same statuses, bytes and consumed bits.  'bzip2' gives each stream one warp and reads the capacities back
@@ -112,6 +117,12 @@ class Batch:
         self.codec = codec
         self.device = torch.device(device)
         self.n = len(in_off)
+        if codec == "tar":
+            t = lambda a: torch.from_numpy(np.ascontiguousarray(np.asarray(a, dtype=np.uint64)).view(np.int64)).to(self.device)
+            lens = np.asarray(in_len, dtype=np.uint64)
+            self._init_tar(torch.from_numpy(np.array(in_buf, dtype=np.uint8)).to(self.device), t(in_off), t(lens),
+                           lens // np.uint64(512) + np.uint64(1) if out_cap is None else out_cap)
+            return
         caps = np.asarray(out_cap, dtype=np.uint64)
         if caps.ndim == 0:
             caps = np.full(self.n, int(caps), dtype=np.uint64)
@@ -207,6 +218,40 @@ class Batch:
             from .api import _CGzipHeader
             self.d_headers = torch.zeros(max(self.n, 1) * C.sizeof(_CGzipHeader), dtype=torch.uint8, device=self.device)
 
+    def _init_tar(self, d_in, d_in_off, d_in_len, entry_cap, d_in_cap=None, d_in_status=None):
+        self.d_in, self.d_in_off, self.d_in_len = d_in, d_in_off, d_in_len
+        self.d_in_cap, self.d_in_status = d_in_cap, d_in_status
+        caps = np.asarray(entry_cap, dtype=np.uint64)
+        if caps.ndim == 0:
+            caps = np.full(self.n, int(caps), dtype=np.uint64)
+        offs = np.zeros(self.n, dtype=np.uint64)
+        if self.n > 1:
+            offs[1:] = np.cumsum(caps[:-1])
+        self.h_entry_off, self.h_entry_cap = offs, caps
+        t = lambda a: torch.from_numpy(np.ascontiguousarray(a).view(np.int64)).to(self.device)
+        self.d_entry_off, self.d_entry_cap = t(offs), t(caps)
+        self.d_entries = torch.zeros(max(int(caps.sum()), 1) * C.sizeof(_lib.TarEntry), dtype=torch.uint8, device=self.device)
+        self.d_out_len = torch.zeros(self.n, dtype=torch.int64, device=self.device)          # n_entries
+        self.d_consumed = torch.zeros(self.n, dtype=torch.int64, device=self.device)
+        self.d_status = torch.full((self.n,), -1, dtype=torch.int32, device=self.device)     # info's status
+        self.d_open_status = torch.full((self.n,), -1, dtype=torch.int32, device=self.device)
+        self.d_format = torch.zeros(self.n, dtype=torch.int32, device=self.device)
+        self.d_format_status = torch.full((self.n,), -1, dtype=torch.int32, device=self.device)
+
+    @classmethod
+    def tar_of(cls, other, entry_cap=None):
+        """A 'tar' batch over another batch's device outputs (unit i: other.d_out[out_off[i] ..+ out_len[i]), with no
+        copy): a 'gzip' / 'xz' / 'bzip2_stream' batch of .tar.gz / .tar.xz / .tar.bz2 files feeds the walk in the same
+        stream.  Each unit is walked over at most other's out_cap bytes (an overflowing decode reports a required size
+        past its region), and a unit whose decode failed is not walked: it reports that status in every status column.
+        Entry tables default to out_cap // 512 + 1 records, enough for any archive the outputs can hold without a
+        negative size."""
+        b = cls.__new__(cls)
+        b.codec, b.device, b.n = "tar", other.device, other.n
+        caps = other.h_out_cap // np.uint64(512) + np.uint64(1) if entry_cap is None else entry_cap
+        b._init_tar(other.d_out, other.d_out_off, other.d_out_len, caps, other.d_out_cap, other.d_status)
+        return b
+
     @classmethod
     def from_units(cls, codec, units, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=None, headers=False,
                    dict_id=None, max_blocks=None, frame_flags=None, gzip_options=None, max_in_bytes=None):
@@ -287,6 +332,12 @@ class Batch:
                                                      p(self.d_out_off), p(self.d_out_cap), p(self.d_out_len), p(self.d_consumed),
                                                      p(self.d_status), self.n, self.max_blocks, opt(self.d_scratch),
                                                      0 if self.d_scratch is None else self.d_scratch.numel(), stream)
+        elif self.codec == "tar":
+            opt = lambda t: None if t is None else p(t)
+            st = L.swc_tar_walk_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), opt(self.d_in_cap), opt(self.d_in_status),
+                                      p(self.d_entries), p(self.d_entry_off),
+                                      p(self.d_entry_cap), p(self.d_out_len), p(self.d_status), p(self.d_open_status),
+                                      p(self.d_format), p(self.d_format_status), self.n, stream)
         elif self.codec == "lzma2":
             st = L.swc_lzma2_decompress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_aux), p(self.d_out), p(self.d_out_off),
                                               p(self.d_out_cap), p(self.d_out_len), p(self.d_consumed), p(self.d_status), self.n, stream)
@@ -300,6 +351,33 @@ class Batch:
         'deflate', 'bzip2' and 'bzip2_stream', in bytes for 'lzma2', 'gzip', 'zlib' and 'lz4_frame', and 0 for 'xz' and the compress codecs."""
         torch.cuda.synchronize(self.device)
         return self.d_status.cpu().numpy(), self.d_out_len.cpu().numpy(), self.d_consumed.cpu().numpy()
+
+    def tar_results(self):
+        """-> (n_entries, info_status, open_status, format, format_status) of a 'tar' batch, numpy arrays (synchronises)"""
+        torch.cuda.synchronize(self.device)
+        return (self.d_out_len.cpu().numpy(), self.d_status.cpu().numpy(), self.d_open_status.cpu().numpy(),
+                self.d_format.cpu().numpy(), self.d_format_status.cpu().numpy())
+
+    def records(self, i):
+        """unit i's swc_tar_entry records as dicts (_lib.tar_record), at most its entry capacity (synchronises)"""
+        torch.cuda.synchronize(self.device)
+        n = min(int(self.d_out_len[i].item()), int(self.h_entry_cap[i]))
+        size, o = C.sizeof(_lib.TarEntry), int(self.h_entry_off[i])
+        raw = self.d_entries[o * size:(o + n) * size].cpu().numpy().tobytes()
+        return [_lib.tar_record(_lib.TarEntry.from_buffer_copy(raw, k * size)) for k in range(n)]
+
+    def unit_bytes(self, i):
+        torch.cuda.synchronize(self.device)
+        o, n = int(self.d_in_off[i].item()), int(self.d_in_len[i].item())
+        if self.d_in_cap is not None:
+            n = min(n, int(self.d_in_cap[i].item()))
+        return bytes(self.d_in[o:o + n].cpu().numpy())
+
+    def entries(self, i):
+        """unit i of a 'tar' batch as TarContainer.info returns it: [TarEntryInfo] (synchronises)"""
+        from .api import tar_entry_info
+        data = self.unit_bytes(i)
+        return [tar_entry_info(data, r) for r in self.records(i)]
 
     def gzip_headers(self):
         """-> the swc_gzip_header of every unit of a 'gzip' batch made with headers=True (synchronises); offsets are

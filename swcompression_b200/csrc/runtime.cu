@@ -329,6 +329,10 @@ const char *swc_status_name(int32_t s) {
     case SWC_ZIP_WRONG_LOCAL_HEADER: return "ZipError.wrongLocalHeader";
     case SWC_ZIP_WRONG_CRC: return "ZipError.wrongCRC";
     case SWC_ZIP_WRONG_TEXT_FIELD: return "ZipError.wrongTextField";
+    case SWC_TAR_TOO_SMALL_FILE_IS_PASSED: return "TarError.tooSmallFileIsPassed";
+    case SWC_TAR_WRONG_FIELD: return "TarError.wrongField";
+    case SWC_TAR_WRONG_HEADER_CHECKSUM: return "TarError.wrongHeaderChecksum";
+    case SWC_TAR_WRONG_PAX_HEADER_ENTRY: return "TarError.wrongPaxHeaderEntry";
     default: return "unknown";
     }
 }

@@ -3,7 +3,8 @@
 DeflateError (Sources/Deflate/DeflateError.swift:10-19), BZip2Error (Sources/BZip2/BZip2Error.swift:12-44),
 LZMAError (Sources/LZMA/LZMAError.swift:10-25), LZMA2Error (Sources/LZMA2/LZMA2Error.swift:10-22),
 DataError (Sources/Common/DataError.swift:9-25), GzipError (Sources/GZip/GzipError.swift:10-35),
-ZlibError (Sources/Zlib/ZlibError.swift:12-26), XZError (Sources/XZ/XZError.swift:12-48), ZipError (Sources/ZIP/ZipError.swift:12-36).
+ZlibError (Sources/Zlib/ZlibError.swift:12-26), XZError (Sources/XZ/XZError.swift:12-48), ZipError (Sources/ZIP/ZipError.swift:12-36),
+TarError (Sources/TAR/TarError.swift:10-18).
 Payload-carrying cases (`wrongCRC(Data)`, `checksumMismatch([Data])`, ...) expose the decoded bytes as `.payload`.
 """
 
@@ -73,8 +74,14 @@ class ZipError(SWCompressionError):
              908: "compressionNotSupported", 909: "wrongLocalHeader", 910: "wrongCRC", 911: "wrongTextField"}
 
 
+class TarError(SWCompressionError):
+    """Sources/TAR/TarError.swift:10-18"""
+    cases = {1001: "tooSmallFileIsPassed", 1002: "wrongField", 1003: "wrongHeaderChecksum", 1004: "wrongPaxHeaderEntry"}
+
+
 _BY_RANGE = [(1, 99, EngineError), (101, 199, DeflateError), (201, 299, BZip2Error), (301, 399, LZMAError),
-             (401, 499, LZMA2Error), (501, 599, DataError), (601, 699, GzipError), (701, 799, ZlibError), (801, 899, XZError), (901, 999, ZipError)]
+             (401, 499, LZMA2Error), (501, 599, DataError), (601, 699, GzipError), (701, 799, ZlibError), (801, 899, XZError), (901, 999, ZipError),
+             (1001, 1099, TarError)]
 
 
 def error_for(code, payload=None):
