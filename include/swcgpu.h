@@ -477,6 +477,36 @@ int32_t swc_xz_unarchive(const uint8_t *in, size_t in_len, uint8_t **out, size_t
 int32_t swc_xz_unarchive_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
                                uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
                                uint64_t *out_len, int32_t *status, uint64_t n, void *cuda_stream);
+/* XZArchive.unarchive(archive:) over n whole .xz files with the blocks of every file decoded side by side, device memory, on
+ * `cuda_stream`.  Each stream's index, read backwards from the end of the unit, gives every block's start and the offset of
+ * its output; the blocks decode in parallel straight into the unit's region, the reference's forward walk then checks them,
+ * and a unit that does not come out SWC_OK that way is decoded by the kernel of swc_xz_unarchive_batch.
+ *   Equality: for every unit and capacity, status[i] and out_len[i] are what swc_xz_unarchive_batch returns for the same unit
+ *     and out_cap[i], and on SWC_OK and SWC_XZ_WRONG_CHECK so are the bytes [0, out_len[i]).  There are no exceptions (an
+ *     overflow is decoded by the same kernel, with the same declared-size hint).  Bytes of the region past out_len[i] are
+ *     unspecified.
+ *   parallel_blocks (device, n entries, or NULL): the number of blocks of unit i that were decoded block-parallel and
+ *     accepted, which is all of its blocks; 0 when the fallback kernel decoded the unit.
+ *   Block table: max_blocks > 0 is its capacity (at most 2^32 - 1).  A unit qualifies when the backward walk through stream
+ *     padding, footers, indexes and records reaches byte 0 and the declared total fits out_cap[i]; a qualifying unit is
+ *     placed when its records end inside the table, in unit order.  Every other unit goes to the fallback: max_blocks
+ *     changes the speed, never the results.  With a caller scratch and max_blocks > 0 the call reads nothing back and
+ *     allocates nothing, and its launches depend only on (n, max_blocks, scratch_bytes), so it can be captured in a CUDA
+ *     graph.  max_blocks == 0 lets the library count the records first (one synchronisation); with a caller scratch the
+ *     table is then the largest the scratch holds.
+ *   Scratch: scratch == NULL takes the library pool.  A caller scratch smaller than swc_xz_block_batch_scratch_bytes(n,
+ *     max_blocks) returns SWC_ERR_INVALID_ARG; the size depends on n and max_blocks only, never on the output.
+ *   Writes: nothing is written outside [out_off[i], out_off[i] + out_cap[i]), and no byte outside the unit's input range
+ *     affects a result: the backward walk reads in_base[in_off[i] ..+ in_len[i]) only, and each block is decoded with its
+ *     input bounded by the unit's end and its output bounded by its index record.
+ * The deviations of swc_xz_unarchive_batch (DESIGN §6) apply unchanged. */
+size_t  swc_xz_block_batch_scratch_bytes(uint64_t n, uint64_t max_blocks);
+int32_t swc_xz_block_unarchive_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                                     uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                     uint64_t *out_len, int32_t *status,
+                                     uint32_t *parallel_blocks /* device, n entries, or NULL */,
+                                     uint64_t n, uint64_t max_blocks,
+                                     void *scratch, size_t scratch_bytes, void *cuda_stream);
 /* resident warps per SM of the LZMA / LZMA2 batch kernel and of the XZ batch kernel on the current device (either pointer
  * may be NULL) */
 int32_t swc_xz_occupancy(int32_t *lzma_warps_per_sm, int32_t *xz_warps_per_sm);

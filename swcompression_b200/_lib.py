@@ -154,6 +154,9 @@ def lib():
         L.swc_zlib_unarchive.argtypes = [vp, sz, C.POINTER(vp), szp]
         L.swc_xz_unarchive.argtypes = [vp, sz, C.POINTER(vp), szp]
         L.swc_xz_unarchive_batch.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, u64, vp]
+        L.swc_xz_block_batch_scratch_bytes.restype = C.c_size_t
+        L.swc_xz_block_batch_scratch_bytes.argtypes = [u64, u64]
+        L.swc_xz_block_unarchive_batch.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, u64, u64, vp, sz, vp]
         L.swc_xz_occupancy.argtypes = [vp, vp]
         L.swc_crc64_batch.argtypes = [vp, vp, vp, vp, vp, u64, vp]
         L.swc_xz_split_unarchive.argtypes = [vp, sz, C.POINTER(vp), szp, C.POINTER(vp), szp]

@@ -60,7 +60,7 @@ def pack_units(units, align=16):
 
 class Batch:
     """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'bzip2_stream', 'lzma2', 'gzip', 'zlib', 'xz',
-    'lz4_frame', 'lz4_block_compress', 'lz4_frame_compress', 'deflate_compress', 'gzip_archive', 'zlib_archive',
+    'xz_blocks', 'lz4_frame', 'lz4_block_compress', 'lz4_frame_compress', 'deflate_compress', 'gzip_archive', 'zlib_archive',
     'bzip2_compress', 'tar').
 
     'tar' walks one TAR archive per unit (TarContainer.open / info / formatOf, TarContainer.swift:36-261) into a table of
@@ -81,6 +81,11 @@ class Batch:
     `headers=True` a 'gzip' batch also fills a device array of swc_gzip_header, which gzip_headers() reads back.
     'xz' decodes one whole .xz file per unit (XZArchive.unarchive, XZArchive.swift:27-50): every stream and block, the outputs
     concatenated.  It takes no scratch and no aux, and reports no consumed bytes (results() gives zeros in that column).
+    'xz_blocks' gives the same statuses, sizes and bytes as 'xz' with the blocks of every file decoded side by side (the
+    streams' indexes place them); parallel_blocks() tells how many blocks of each unit took that path (0: the whole unit
+    was decoded as 'xz' decodes it).  `max_blocks` is the capacity of its block table: with it the batch owns a scratch of
+    swc_xz_block_batch_scratch_bytes and run() reads nothing back (it can be captured in a CUDA graph).  None lets the
+    library count the blocks first (one synchronisation) and use its pool.
 
     'lz4_frame' decodes the first LZ4 frame of each unit (LZ4.decompress(data:dictionary:dictionaryID:), LZ4.swift:73-91):
     `aux` is the dictionary's bytes (None: nil), `dict_id` the dictionary ID (None: nil), and results() gives the consumed
@@ -150,6 +155,12 @@ class Batch:
                 nbytes = _lib.lib().swc_bzip2_stream_batch_scratch_bytes(self.n, self.max_blocks, self.out_total)
                 if scratch_bytes is not None:
                     nbytes = min(nbytes, int(scratch_bytes))
+                self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        elif codec == "xz_blocks":
+            self.d_aux = None
+            self.d_parallel = torch.zeros(self.n, dtype=torch.int32, device=self.device)
+            if self.max_blocks:
+                nbytes = _lib.lib().swc_xz_block_batch_scratch_bytes(self.n, self.max_blocks)
                 self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         elif codec == "lz4_frame":
             # an empty dictionary is still a dictionary: one spare byte keeps its pointer non-null
@@ -241,7 +252,7 @@ class Batch:
     @classmethod
     def tar_of(cls, other, entry_cap=None):
         """A 'tar' batch over another batch's device outputs (unit i: other.d_out[out_off[i] ..+ out_len[i]), with no
-        copy): a 'gzip' / 'xz' / 'bzip2_stream' batch of .tar.gz / .tar.xz / .tar.bz2 files feeds the walk in the same
+        copy): a 'gzip' / 'xz' / 'xz_blocks' / 'bzip2_stream' batch of .tar.gz / .tar.xz / .tar.bz2 files feeds the walk in the same
         stream.  Each unit is walked over at most other's out_cap bytes (an overflowing decode reports a required size
         past its region), and a unit whose decode failed is not walked: it reports that status in every status column.
         Entry tables default to out_cap // 512 + 1 records, enough for any archive the outputs can hold without a
@@ -280,6 +291,12 @@ class Batch:
         elif self.codec == "xz":
             st = L.swc_xz_unarchive_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out), p(self.d_out_off),
                                           p(self.d_out_cap), p(self.d_out_len), p(self.d_status), self.n, stream)
+        elif self.codec == "xz_blocks":
+            st = L.swc_xz_block_unarchive_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out),
+                                                p(self.d_out_off), p(self.d_out_cap), p(self.d_out_len), p(self.d_status),
+                                                p(self.d_parallel), self.n, self.max_blocks,
+                                                None if self.d_scratch is None else p(self.d_scratch),
+                                                0 if self.d_scratch is None else self.d_scratch.numel(), stream)
         elif self.codec == "lz4_block":
             st = L.swc_lz4_block_decompress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), None, 0, p(self.d_out),
                                                   p(self.d_out_off), p(self.d_out_cap), p(self.d_out_len), p(self.d_status),
@@ -348,9 +365,15 @@ class Batch:
 
     def results(self):
         """-> (status int32[n], out_len int64[n], consumed int64[n]) on the host (synchronises).  consumed is in bits for
-        'deflate', 'bzip2' and 'bzip2_stream', in bytes for 'lzma2', 'gzip', 'zlib' and 'lz4_frame', and 0 for 'xz' and the compress codecs."""
+        'deflate', 'bzip2' and 'bzip2_stream', in bytes for 'lzma2', 'gzip', 'zlib' and 'lz4_frame', and 0 for 'xz', 'xz_blocks'
+        and the compress codecs."""
         torch.cuda.synchronize(self.device)
         return self.d_status.cpu().numpy(), self.d_out_len.cpu().numpy(), self.d_consumed.cpu().numpy()
+
+    def parallel_blocks(self):
+        """-> uint32[n] of an 'xz_blocks' batch: the blocks of each unit decoded block-parallel and accepted (synchronises)"""
+        torch.cuda.synchronize(self.device)
+        return self.d_parallel.cpu().numpy().view(np.uint32)
 
     def tar_results(self):
         """-> (n_entries, info_status, open_status, format, format_status) of a 'tar' batch, numpy arrays (synchronises)"""
