@@ -456,6 +456,58 @@ int32_t swc_zlib_unarchive_batch(const uint8_t *in_base, const uint64_t *in_off,
                                  uint64_t out_capacity_total,
                                  uint64_t *out_len, uint64_t *consumed_bytes, int32_t *status,
                                  uint64_t n, void *scratch, size_t scratch_bytes, void *cuda_stream);
+/* GzipArchive.multiUnarchive(archive:) (GzipArchive.swift:52-100) over n multi-member gzip files (BGZF, `cat a.gz b.gz`),
+ * device memory, on `cuda_stream`, with the members of every file decoded side by side.  Candidate member starts (the
+ * signature 1f 8b 08 with the reserved flag bits clear and 20 bytes left in the unit, and always position 0) cut each unit
+ * into spans: from a candidate whose FEXTRA holds a BGZF "BC" subfield the span ends at c + BSIZE + 1 when that is a
+ * candidate or the unit end, else at the next candidate.  Each span decodes as one unit of the swc_gzip_unarchive_batch
+ * stages straight into place (its capacity the ISIZE in its last 4 bytes, its output at the sum of the ISIZEs in front of
+ * it), the reference's in-order walk accepts member k iff it is OK or wrongCRC, consumed exactly its span and starts where
+ * member k - 1 ended, and a sequential walk on the device decodes the rest of a unit from its first member not accepted.
+ *   Equality: for every unit whose capacity suffices, status[i] is what swc_gzip_multi_unarchive returns for the same
+ *     bytes.  On SWC_OK and SWC_GZIP_WRONG_CRC, out_base[out_off[i] ..+ out_len[i]) holds the members concatenated (on
+ *     wrongCRC up to and including the failing member), consumed_bytes[i] is the end of the last member returned, and the
+ *     member table holds its ends and starts.  A 0-byte unit is SWC_OK with 0 members; 1-19 bytes behind valid members
+ *     are wrongMagic.  On every other status consumed_bytes[i] = 0, n_members[i] = 0 and out_len[i] = 0, except:
+ *   Overflow: SWC_ERR_OUTPUT_OVERFLOW when a member does not fit out_cap[i].  The walk then goes on counting: every later
+ *     member is decoded without keeping its bytes, its header, Deflate stream and ISIZE checked but not its CRC-32, up to
+ *     the unit end or the first error.  out_len[i] is the bytes counted: the exact size when the unit's members validate
+ *     against their trailers, otherwise (a member past the capacity with a wrong CRC-32 or a later error) an upper bound
+ *     of what the walk keeps.  Either way a rerun with out_cap[i] >= out_len[i] does not overflow and is final.
+ *   Member table (n_members, member_off, member_cap, member_end, member_in_off: device, n entries for the first three; all
+ *     four arrays or none of them; n_members may be NULL on its own): n_members[i] is the number of members returned,
+ *     also when it exceeds member_cap[i]; at most member_cap[i] entries are written at member_off[i]: member_end, each
+ *     member's output end relative to out_off[i] (swc_gzip_multi_unarchive's member_ends), and member_in_off, each
+ *     member's start inside the unit.  One past the last member is consumed_bytes[i].  in_len[i] / 20 + 1 entries always
+ *     suffice.
+ *   parallel_members (device, n entries, or NULL): the members of unit i accepted from the parallel spans; the
+ *     sequential walk decoded the rest.  It equals n_members[i] for BGZF files and clean concatenations whose members
+ *     each decode to 0 or at least 16 bytes and fit out_cap[i]: a member whose output region would be 1-15 bytes (its
+ *     size, or what out_cap[i] leaves of it), and every member behind it, takes the sequential walk (the Deflate stage's
+ *     scratch for so small an output region cannot hold its literals).
+ *   Member table capacity: max_members > 0 (at most 2^32 - 1) holds the candidates of the units in order; a unit whose
+ *     candidates do not fit is decoded by the sequential walk alone: max_members changes the speed, never the results.
+ *     With a caller scratch and max_members > 0 the call reads nothing back and allocates nothing, and its launches
+ *     depend only on (n, max_members, scratch_bytes), so it can be captured in a CUDA graph.  max_members == 0 lets the
+ *     library count the candidates first (one synchronisation), and read in_len, out_off and out_cap back; its table then
+ *     holds at most in_len[i] / 20 + 1 entries per unit.
+ *   Scratch: scratch == NULL takes the library pool (reading out_off / out_cap back).  A caller scratch must hold
+ *     swc_gzip_member_batch_scratch_bytes(n, max_members, out_capacity_total) bytes, where out_capacity_total >=
+ *     out_off[i] + out_cap[i] for every unit (as for swc_gzip_unarchive_batch); one smaller than that for
+ *     out_capacity_total = 0 returns SWC_ERR_INVALID_ARG.  A member whose output region lies past the arena the scratch
+ *     covers takes the sequential walk, so a smaller scratch changes the speed, never the results or the memory touched.
+ *     With max_members == 0 the table is then the largest the scratch holds.
+ *   Writes: nothing is written outside [out_off[i], out_off[i] + out_cap[i]), and no byte outside the unit's input range
+ *     affects a result: the scan loads the aligned 16-byte lines that hold the unit's bytes and matches none outside it,
+ *     and every span and the sequential walk are bounded by the unit's end. */
+size_t  swc_gzip_member_batch_scratch_bytes(uint64_t n, uint64_t max_members, uint64_t out_capacity_total);
+int32_t swc_gzip_multi_unarchive_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                                       uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                       uint64_t *out_len, uint64_t *consumed_bytes, int32_t *status,
+                                       uint64_t *n_members, const uint64_t *member_off, const uint64_t *member_cap,
+                                       uint64_t *member_end, uint64_t *member_in_off,   /* table: may be NULL */
+                                       uint32_t *parallel_members /* device, n, or NULL */,
+                                       uint64_t n, uint64_t max_members, void *scratch, size_t scratch_bytes, void *cuda_stream);
 int32_t swc_xz_unarchive(const uint8_t *in, size_t in_len, uint8_t **out, size_t *out_len);
 /* XZArchive.unarchive(archive:) over n whole .xz files, device memory, asynchronous on `cuda_stream`: one launch, no host
  * read, no allocation, no synchronisation and no scratch, so the call can be captured in a CUDA graph.  Unit i is the file

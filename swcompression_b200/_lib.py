@@ -151,6 +151,10 @@ def lib():
         L.swc_unarchive_batch_scratch_bytes.argtypes = [C.c_uint64, C.c_uint64]
         L.swc_gzip_unarchive_batch.argtypes = [vp, vp, vp, vp, vp, vp, u64, vp, vp, vp, vp, u64, vp, sz, vp]
         L.swc_zlib_unarchive_batch.argtypes = [vp, vp, vp, vp, vp, vp, u64, vp, vp, vp, u64, vp, sz, vp]
+        L.swc_gzip_member_batch_scratch_bytes.restype = C.c_size_t
+        L.swc_gzip_member_batch_scratch_bytes.argtypes = [u64, u64, u64]
+        L.swc_gzip_multi_unarchive_batch.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, u64, u64, vp, sz,
+                                                     vp]
         L.swc_zlib_unarchive.argtypes = [vp, sz, C.POINTER(vp), szp]
         L.swc_xz_unarchive.argtypes = [vp, sz, C.POINTER(vp), szp]
         L.swc_xz_unarchive_batch.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, u64, vp]

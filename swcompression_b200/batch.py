@@ -60,8 +60,8 @@ def pack_units(units, align=16):
 
 class Batch:
     """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'bzip2_stream', 'lzma2', 'gzip', 'zlib', 'xz',
-    'xz_blocks', 'lz4_frame', 'lz4_block_compress', 'lz4_frame_compress', 'deflate_compress', 'gzip_archive', 'zlib_archive',
-    'bzip2_compress', 'tar').
+    'xz_blocks', 'gzip_multi', 'lz4_frame', 'lz4_block_compress', 'lz4_frame_compress', 'deflate_compress', 'gzip_archive',
+    'zlib_archive', 'bzip2_compress', 'tar').
 
     'tar' walks one TAR archive per unit (TarContainer.open / info / formatOf, TarContainer.swift:36-261) into a table of
     swc_tar_entry records; `out_cap` is each unit's record capacity (None: in_len // 512 + 1).  results() gives info's
@@ -86,6 +86,14 @@ class Batch:
     was decoded as 'xz' decodes it).  `max_blocks` is the capacity of its block table: with it the batch owns a scratch of
     swc_xz_block_batch_scratch_bytes and run() reads nothing back (it can be captured in a CUDA graph).  None lets the
     library count the blocks first (one synchronisation) and use its pool.
+    'gzip_multi' decodes every member of each unit (GzipArchive.multiUnarchive, GzipArchive.swift:52-100) with the members
+    of all units side by side; results() gives the status, the members' total size and the consumed bytes (the end of the
+    last member returned), members(i) unit i's [GzipArchive.Member] and parallel_members() how many members of each unit
+    the parallel spans gave (the rest took the sequential walk).  `member_cap` is each unit's member table capacity (None:
+    in_len // 20 + 1, always enough).  `max_members` is the capacity of the candidate table: with it the batch owns a
+    scratch of swc_gzip_member_batch_scratch_bytes (or `scratch_bytes`) and run() reads nothing back (it can be captured in
+    a CUDA graph).  None lets the library count the candidates first (one synchronisation) and use its pool, or
+    `scratch_bytes` of caller scratch.
 
     'lz4_frame' decodes the first LZ4 frame of each unit (LZ4.decompress(data:dictionary:dictionaryID:), LZ4.swift:73-91):
     `aux` is the dictionary's bytes (None: nil), `dict_id` the dictionary ID (None: nil), and results() gives the consumed
@@ -118,7 +126,8 @@ class Batch:
     cannot hold the largest unit fails the run with SWC_ERR_INVALID_ARG)."""
 
     def __init__(self, codec, in_buf, in_off, in_len, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=None,
-                 headers=False, dict_id=None, max_blocks=None, frame_flags=None, gzip_options=None, max_in_bytes=None):
+                 headers=False, dict_id=None, max_blocks=None, frame_flags=None, gzip_options=None, max_in_bytes=None,
+                 max_members=None, member_cap=None):
         self.codec = codec
         self.device = torch.device(device)
         self.n = len(in_off)
@@ -161,6 +170,25 @@ class Batch:
             self.d_parallel = torch.zeros(self.n, dtype=torch.int32, device=self.device)
             if self.max_blocks:
                 nbytes = _lib.lib().swc_xz_block_batch_scratch_bytes(self.n, self.max_blocks)
+                self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        elif codec == "gzip_multi":
+            self.d_aux = None
+            self.d_parallel = torch.zeros(self.n, dtype=torch.int32, device=self.device)
+            mcap = np.asarray(in_len, dtype=np.uint64) // np.uint64(20) + np.uint64(1) if member_cap is None else member_cap
+            mcap = np.broadcast_to(np.asarray(mcap, dtype=np.uint64), (self.n,)).copy()
+            moff = np.zeros(self.n, dtype=np.uint64)
+            if self.n > 1:
+                moff[1:] = np.cumsum(mcap[:-1])
+            self.h_member_off, self.h_member_cap = moff, mcap
+            self.d_member_off, self.d_member_cap = t(moff), t(mcap)
+            self.d_n_members = torch.zeros(self.n, dtype=torch.int64, device=self.device)
+            slots = max(int(mcap.sum()), 1)
+            self.d_member_end = torch.zeros(slots, dtype=torch.int64, device=self.device)
+            self.d_member_in_off = torch.zeros(slots, dtype=torch.int64, device=self.device)
+            self.max_members = 0 if max_members is None else int(max_members)
+            if self.max_members or scratch_bytes is not None:
+                nbytes = (_lib.lib().swc_gzip_member_batch_scratch_bytes(self.n, self.max_members, self.out_total)
+                          if scratch_bytes is None else int(scratch_bytes))
                 self.d_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         elif codec == "lz4_frame":
             # an empty dictionary is still a dictionary: one spare byte keeps its pointer non-null
@@ -252,8 +280,9 @@ class Batch:
     @classmethod
     def tar_of(cls, other, entry_cap=None):
         """A 'tar' batch over another batch's device outputs (unit i: other.d_out[out_off[i] ..+ out_len[i]), with no
-        copy): a 'gzip' / 'xz' / 'xz_blocks' / 'bzip2_stream' batch of .tar.gz / .tar.xz / .tar.bz2 files feeds the walk in the same
-        stream.  Each unit is walked over at most other's out_cap bytes (an overflowing decode reports a required size
+        copy): a 'gzip' / 'gzip_multi' / 'xz' / 'xz_blocks' / 'bzip2_stream' batch of .tar.gz / .tar.xz / .tar.bz2 files
+        feeds the walk in the same stream ('gzip_multi' outputs are each unit's members back to back, so a BGZF .tar.gz
+        is walked in place).  Each unit is walked over at most other's out_cap bytes (an overflowing decode reports a required size
         past its region), and a unit whose decode failed is not walked: it reports that status in every status column.
         Entry tables default to out_cap // 512 + 1 records, enough for any archive the outputs can hold without a
         negative size."""
@@ -265,10 +294,11 @@ class Batch:
 
     @classmethod
     def from_units(cls, codec, units, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=None, headers=False,
-                   dict_id=None, max_blocks=None, frame_flags=None, gzip_options=None, max_in_bytes=None):
+                   dict_id=None, max_blocks=None, frame_flags=None, gzip_options=None, max_in_bytes=None, max_members=None,
+                   member_cap=None):
         buf, offs, lens = pack_units(units)
         return cls(codec, buf, offs, lens, out_cap, device, aux, scratch_bytes, block_size, headers, dict_id, max_blocks,
-                   frame_flags, gzip_options, max_in_bytes)
+                   frame_flags, gzip_options, max_in_bytes, max_members, member_cap)
 
     def run(self):
         L = _lib.lib()
@@ -297,6 +327,14 @@ class Batch:
                                                 p(self.d_parallel), self.n, self.max_blocks,
                                                 None if self.d_scratch is None else p(self.d_scratch),
                                                 0 if self.d_scratch is None else self.d_scratch.numel(), stream)
+        elif self.codec == "gzip_multi":
+            opt = lambda t: None if t is None else p(t)
+            st = L.swc_gzip_multi_unarchive_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out),
+                                                  p(self.d_out_off), p(self.d_out_cap), p(self.d_out_len), p(self.d_consumed),
+                                                  p(self.d_status), p(self.d_n_members), p(self.d_member_off),
+                                                  p(self.d_member_cap), p(self.d_member_end), p(self.d_member_in_off),
+                                                  p(self.d_parallel), self.n, self.max_members, opt(self.d_scratch),
+                                                  0 if self.d_scratch is None else self.d_scratch.numel(), stream)
         elif self.codec == "lz4_block":
             st = L.swc_lz4_block_decompress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), None, 0, p(self.d_out),
                                                   p(self.d_out_off), p(self.d_out_cap), p(self.d_out_len), p(self.d_status),
@@ -375,6 +413,31 @@ class Batch:
         torch.cuda.synchronize(self.device)
         return self.d_parallel.cpu().numpy().view(np.uint32)
 
+    def parallel_members(self):
+        """-> uint32[n] of a 'gzip_multi' batch: the members of each unit accepted from the parallel spans (synchronises)"""
+        torch.cuda.synchronize(self.device)
+        return self.d_parallel.cpu().numpy().view(np.uint32)
+
+    def member_table(self, i):
+        """-> (member ends in the output, member starts in the unit) of unit i of a 'gzip_multi' batch, at most its member
+        capacity (synchronises)"""
+        torch.cuda.synchronize(self.device)
+        k = min(int(self.d_n_members[i].item()), int(self.h_member_cap[i]))
+        o = int(self.h_member_off[i])
+        return [int(v) for v in self.d_member_end[o:o + k].cpu()], [int(v) for v in self.d_member_in_off[o:o + k].cpu()]
+
+    def members(self, i):
+        """unit i of a 'gzip_multi' batch as GzipArchive.multiUnarchive returns it: [GzipArchive.Member], the headers parsed
+        from the unit's bytes at each member's start (synchronises)"""
+        from .api import GzipArchive, GzipHeader
+        ends, starts = self.member_table(i)
+        data, out = self.unit_bytes(i), self.output(i)
+        members, prev = [], 0
+        for e, s in zip(ends, starts):
+            members.append(GzipArchive.Member(GzipHeader(data, _member_off=s), out[prev:e]))
+            prev = e
+        return members
+
     def tar_results(self):
         """-> (n_entries, info_status, open_status, format, format_status) of a 'tar' batch, numpy arrays (synchronises)"""
         torch.cuda.synchronize(self.device)
@@ -392,7 +455,7 @@ class Batch:
     def unit_bytes(self, i):
         torch.cuda.synchronize(self.device)
         o, n = int(self.d_in_off[i].item()), int(self.d_in_len[i].item())
-        if self.d_in_cap is not None:
+        if getattr(self, "d_in_cap", None) is not None:
             n = min(n, int(self.d_in_cap[i].item()))
         return bytes(self.d_in[o:o + n].cpu().numpy())
 

@@ -215,22 +215,57 @@ int adler32_units(const u8 *base, const u64 *off, const u64 *len, const int32_t 
     return SWC_OK;
 }
 
-// gzip member signature scan (GzipHeader.swift:70-81: magic 1f 8b, method 8, reserved flag bits clear); positions are
-// appended in any order and sorted by the host wrapper
-__global__ void __launch_bounds__(256) gzip_scan_kernel(const u8 *d, u64 n, u64 *list, unsigned long long *count, u64 cap) {
-    const u64 base = ((u64)blockIdx.x * blockDim.x + threadIdx.x) * 16;
-    if (base >= n) return;
-    // 16 positions per thread from one aligned 16-byte load plus the 3 bytes that follow
-    const uint4 v = *(const uint4 *)(d + base);                       // the buffer is padded by >= 32 bytes
-    const u32 w[5] = {v.x, v.y, v.z, v.w, *(const u32 *)(d + base + 16)};
+// gzip member signature scan over unit ranges (GzipHeader.swift:70-81: magic 1f 8b, method 8, reserved flag bits clear):
+// position p of unit u is a candidate when the signature starts there and p + 20 <= in_len[u] (a shorter member fails
+// the 20-byte guard), or when p = 0 and s.with_zero (a multi-member walk always starts at 0).  Grid: blockIdx.y strides
+// the units, the x-threads stride the unit's 16-byte groups of positions, so the launch shape depends on n alone.  Each
+// candidate takes slot = atomicAdd(&count[u], 1): with `first` set (and first[u] != ~0) it goes to list[first[u] + slot],
+// with list alone (one unit) to list[slot] while slot < cap, and with neither it is only counted.  Positions come in any
+// order.  Units may be unaligned: a thread loads the aligned 16-byte lines that hold its 16 positions and the 3 bytes
+// behind them, skipping a line that starts past the unit, and no byte outside the unit is matched.
+__global__ void __launch_bounds__(256) gzip_scan_kernel(GzipScan s) {
+    for (u64 u = blockIdx.y; u < s.n; u += gridDim.y) {
+        if (s.first && s.first[u] == ~0ull) continue;
+        const u8 *p = s.base + s.off[u];
+        const u64 L = s.len[u];
+        for (u64 base = ((u64)blockIdx.x * blockDim.x + threadIdx.x) * 16; base < L; base += (u64)gridDim.x * blockDim.x * 16) {
+            const u8 *at = p + base, *stop = p + L;
+            const uint4 *line = (const uint4 *)((uintptr_t)at & ~(uintptr_t)15);
+            u32 v[12];
 #pragma unroll
-    for (int i = 0; i < 16; i++) {
-        const u32 x = __funnelshift_r(w[i >> 2], w[(i >> 2) + 1], (i & 3) * 8);
-        if ((x & 0xE0FFFFFFu) == 0x00088B1Fu && base + i + 20 <= n) {
-            const u64 slot = atomicAdd(count, 1ull);
-            if (slot < cap) list[slot] = base + i;
+            for (int k = 0; k < 3; k++) {
+                const uint4 x = (const u8 *)(line + k) < stop ? __ldg(line + k) : make_uint4(0, 0, 0, 0);
+                v[4 * k] = x.x; v[4 * k + 1] = x.y; v[4 * k + 2] = x.z; v[4 * k + 3] = x.w;
+            }
+            const u32 r = (u32)((uintptr_t)at & 15), q = r >> 2, sh = (r & 3) * 8;
+            u32 w[5];                                        // bytes base .. base + 19 of the unit
+#pragma unroll
+            for (int k = 0; k < 5; k++) {
+                const u32 a0 = q == 0 ? v[k] : q == 1 ? v[k + 1] : q == 2 ? v[k + 2] : v[k + 3];
+                const u32 a1 = q == 0 ? v[k + 1] : q == 1 ? v[k + 2] : q == 2 ? v[k + 3] : v[k + 4];
+                w[k] = __funnelshift_r(a0, a1, sh);
+            }
+#pragma unroll
+            for (int i = 0; i < 16; i++) {
+                const u32 x = __funnelshift_r(w[i >> 2], w[(i >> 2) + 1], (i & 3) * 8);
+                const u64 pos = base + i;
+                if (((x & 0xE0FFFFFFu) == 0x00088B1Fu && pos + 20 <= L) || (pos == 0 && s.with_zero)) {
+                    const u64 slot = atomicAdd(&s.count[u], 1ull);
+                    if (s.first) s.list[s.first[u] + slot] = pos;
+                    else if (s.list && slot < s.cap) s.list[slot] = pos;
+                }
+            }
         }
     }
+}
+
+int gzip_scan(const GzipScan &s, cudaStream_t stream) {
+    if (!s.n) return SWC_OK;
+    const unsigned y = (unsigned)(s.n < 65535 ? s.n : 65535), x = y >= 2048 ? 1u : 2048u / y;
+    gzip_scan_kernel<<<dim3(x, y), 256, 0, stream>>>(s);
+    count_launch();
+    SWC_CUDA_TRY(cudaGetLastError());
+    return SWC_OK;
 }
 
 int find_gzip_members(const u8 *d_in, u64 n, std::vector<size_t> &pos) {
@@ -241,12 +276,11 @@ int find_gzip_members(const u8 *d_in, u64 n, std::vector<size_t> &pos) {
     int st = arena_get(2, 256 + cap * 8, &p, 0);
     if (st) return st;
     unsigned long long *count = (unsigned long long *)p;
+    u64 *range = (u64 *)p + 1;                                        // the one unit: offset 0, length n
     u64 *list = (u64 *)((u8 *)p + 256);
-    SWC_CUDA_TRY(cudaMemsetAsync(count, 0, 8, 0));
-    const u64 threads = (n + 15) / 16;
-    gzip_scan_kernel<<<(unsigned)((threads + 255) / 256), 256>>>(d_in, n, list, count, cap);
-    count_launch();
-    SWC_CUDA_TRY(cudaGetLastError());
+    const u64 head[3] = {0, 0, n};
+    SWC_CUDA_TRY(cudaMemcpy(p, head, sizeof head, cudaMemcpyHostToDevice));
+    if ((st = gzip_scan(GzipScan{d_in, range, range + 1, 1, count, nullptr, list, cap, false}, 0))) return st;
     unsigned long long h = 0;
     SWC_CUDA_TRY(cudaMemcpy(&h, count, 8, cudaMemcpyDeviceToHost));
     if (h > cap) return SWC_OK;                                       // absurd candidate count: caller walks sequentially

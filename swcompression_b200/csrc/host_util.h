@@ -191,6 +191,8 @@ int deflate_batch_impl(const DecodeIO &io, const uint8_t *start_bits, uint64_t o
 // the same for GzipArchive / ZlibArchive.unarchive (unarchive_batch.cu); headers may be null (always for zlib)
 int unarchive_batch_impl(bool gzip, const DecodeIO &io, swc_gzip_header *headers, uint64_t out_total, void *scratch,
                          size_t scratch_bytes, cudaStream_t stream);
+// the inverse of swc_unarchive_batch_scratch_bytes: an output arena `bytes` of scratch covers for n units (0: none)
+uint64_t unarchive_batch_arena(uint64_t n, size_t bytes);
 
 // large transfers between pageable host memory and the device: T threads x (stream + two pinned bounce buffers) (runtime.cu)
 int copy_pageable(void *dst, const void *src, size_t bytes, bool to_device);

@@ -41,6 +41,12 @@ inline size_t scratch_header(u64 n, int tickets) { return (size_t)256 * tickets 
 inline size_t scratch_bytes(u64 n, u64 out_capacity_total) {           // one ticket block
     return (size_t)((out_capacity_total / 3 + 2) * 4 + n * 4 + 1024);
 }
+// the inverse: the largest output arena that `bytes` of scratch covers for n units (scratch_bytes(n, result) <= bytes; 0
+// when bytes < scratch_bytes(n, 0))
+inline u64 arena_covered(u64 n, size_t bytes) {
+    const size_t b0 = scratch_bytes(n, 0);
+    return bytes < b0 ? 0 : (u64)((bytes - b0) / 4) * 3 + 2;
+}
 // seats a.ticket (block `ticket` of `tickets`), a.rec_count (entries first .. first + a.n of the n-unit table) and a.rec_base
 void seat_scratch(BatchArgs &a, void *scratch, u64 n, u64 first, int tickets, int ticket);
 // bytes of the scratch region of a unit

@@ -160,6 +160,11 @@ int unarchive_batch_impl(bool gzip, const DecodeIO &io, swc_gzip_header *headers
     return SWC_OK;
 }
 
+uint64_t unarchive_batch_arena(uint64_t n, size_t bytes) {
+    const size_t cols = columns_bytes(n);
+    return bytes < cols ? 0 : inflate::arena_covered(n, bytes - cols);
+}
+
 }  // namespace swc
 
 using namespace swc;
