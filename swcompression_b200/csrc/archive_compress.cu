@@ -9,7 +9,6 @@
 //   link, parse, emit, seam      deflatec::run: each stream into staging in the scratch, which it never overflows
 //   finish     CTA per 64 KiB    out_len and status; header, stream and trailer into the caller's region of a unit that
 //                                fits, every byte once, 16-byte stores wherever the region allows
-#include <type_traits>
 #include <vector>
 #include "../../include/swcgpu.h"
 #include "compress_host.h"
@@ -45,42 +44,26 @@ struct Cols {
 
 struct Layout {
     Cols c;
-    size_t bytes = 0;
+    size_t bytes;
     Layout(void *base, u64 count) {
-        auto take = [&](auto *&ptr, u64 k) {
-            ptr = (std::remove_reference_t<decltype(ptr)>)((u8 *)base + bytes);
-            bytes += (k * sizeof(*ptr) + 255) & ~(size_t)255;
-        };
-        take(c.scr_off, count); take(c.tile_start, count + 1); take(c.chunk_start, count + 1); take(c.fin_start, count + 1);
-        take(c.eff_len, count); take(c.stage_off, count); take(c.stage_cap, count); take(c.s_len, count);
-        take(c.st, count); take(c.s_st, count); take(c.ck, count);
+        Carver k(base);
+        k.cols(count, c.scr_off);
+        k.cols(count + 1, c.tile_start, c.chunk_start, c.fin_start);
+        k.cols(count, c.eff_len, c.stage_off, c.stage_cap, c.s_len, c.st, c.s_st, c.ck);
+        bytes = k.at;
     }
 };
 
 __device__ __forceinline__ u64 header_len(const ArcArgs &a, u64 u) { return a.hdr_base ? a.hdr_len[u] : ZLIB_HDR; }
 __device__ __forceinline__ u64 trailer_len(const ArcArgs &a) { return a.hdr_base ? 8 : 4; }
 
-// the inclusive prefix sum of part[k][0..1024) in place (one CTA of 1024 threads)
-template <int K> __device__ __forceinline__ void cta_scan(u64 (*part)[1024]) {
-    __syncthreads();
-    for (int d = 1; d < 1024; d <<= 1) {
-        u64 v[K];
-#pragma unroll
-        for (int k = 0; k < K; k++) v[k] = threadIdx.x >= (u32)d ? part[k][threadIdx.x - d] : 0;
-        __syncthreads();
-#pragma unroll
-        for (int k = 0; k < K; k++) part[k][threadIdx.x] += v[k];
-        __syncthreads();
-    }
-}
-
 // Units [first, first + count), a contiguous run of them per thread.  Unit i is placed while the exclusive prefix sum of
 // in_len plus its own length is at most `fit` (and it is under 4 GiB); placed units get their scratch and staging behind
 // the `head` bytes of columns, in order.
 __global__ void __launch_bounds__(1024) arc_place_kernel(ArcArgs a, Cols c, u64 first, u64 count, u64 fit, u64 head) {
     __shared__ u64 part[4][1024];
-    const u64 per = (count + 1023) / 1024;
-    const u64 b = threadIdx.x * per < count ? threadIdx.x * per : count, e = b + per < count ? b + per : count;
+    u64 b, e;
+    cta_unit_run(count, b, e);
     const u64 *len = a.in_len + first;
     u64 sum = 0;
     for (u64 j = b; j < e; j++) sum += len[j];

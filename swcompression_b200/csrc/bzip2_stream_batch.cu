@@ -18,7 +18,6 @@
 //                                   at the end magic), the stored combined CRC is the fold of the block CRCs; else fallback
 //   fallback      one CTA, then     per-unit scratch offsets of the fallback units (exclusive sum inside the dead block
 //                 warp per unit     area), then bzip2_kernel in stream mode over exactly those units
-#include <type_traits>
 #include <vector>
 #include "../../include/swcgpu.h"
 #include "bzip2.cuh"
@@ -181,21 +180,15 @@ __global__ void __launch_bounds__(256) bz2s_scan_kernel(ScanArgs a) {
 // totals[0] = the candidates of the units that scanned clean, totals[1] = the fallback scratch of every unit.
 __global__ void __launch_bounds__(1024) bz2s_place_kernel(UnitCols c, const u64 *out_cap, u64 n, u64 max_blocks, u64 area) {
     __shared__ u64 part[2][1024];
-    const u64 per = (n + 1023) / 1024;
-    const u64 b = threadIdx.x * per < n ? threadIdx.x * per : n, e = b + per < n ? b + per : n;
+    u64 b, e;
+    cta_unit_run(n, b, e);
     u64 s = 0, sf = 0;
     for (u64 i = b; i < e; i++) {
         s += (c.flags[i] & F_OK) ? c.count[i] : 0;
         sf += bzip2::scratch_per_unit(out_cap[i]);
     }
     part[0][threadIdx.x] = s; part[1][threadIdx.x] = sf;
-    __syncthreads();
-    for (int d = 1; d < 1024; d <<= 1) {
-        const u64 v0 = threadIdx.x >= (u32)d ? part[0][threadIdx.x - d] : 0, v1 = threadIdx.x >= (u32)d ? part[1][threadIdx.x - d] : 0;
-        __syncthreads();
-        part[0][threadIdx.x] += v0; part[1][threadIdx.x] += v1;
-        __syncthreads();
-    }
+    cta_scan<2>(part);
     if (threadIdx.x == 1023) { c.totals[0] = part[0][1023]; c.totals[1] = part[1][1023]; }
     u64 at = part[0][threadIdx.x] - s, fat = part[1][threadIdx.x] - sf;
     for (u64 i = b; i < e; i++) {
@@ -235,29 +228,19 @@ __global__ void __launch_bounds__(256) bz2s_layout_kernel(UnitCols c, BlockCols 
 // its slowest warp is done, so the long blocks go first, 4 to a CTA, and the short ones (a stream's last block, idle
 // entries) fill in behind them.
 __global__ void __launch_bounds__(1024) bz2s_order_kernel(const u64 *unit_len, UnitCols c, BlockCols b, u64 e0, u64 cnt) {
-    __shared__ u32 start[65];
-    if (threadIdx.x < 65) start[threadIdx.x] = 0;
-    __syncthreads();
-    auto key = [&](u64 e) -> u32 {
-        const u64 len = b.in_len[e];
+    auto key = [&](u64 j) -> u32 {
+        const u64 e = e0 + j, len = b.in_len[e];
         if (!len) return 64;                                        // idle entry
         const u32 u = b.unit[e];
         const bool last = e + 1 == c.first_blk[u] + c.count[u];
         const u64 span = len - (last ? unit_len[u] - (c.end_bit[u] >> 3) : b.in_len[e + 1]);
         return __clzll((long long)span);
     };
-    for (u64 j = threadIdx.x; j < cnt; j += blockDim.x) atomicAdd(&start[key(e0 + j)], 1u);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        u32 at = 0;
-        for (int k = 0; k < 65; k++) { const u32 h = start[k]; start[k] = at; at += h; }
-    }
-    __syncthreads();
-    for (u64 j = threadIdx.x; j < cnt; j += blockDim.x) {
-        const u64 e = e0 + j, at = atomicAdd(&start[key(e)], 1u);
+    clz_order(cnt, key, [&](u64 j, u32 at) {
+        const u64 e = e0 + j;
         b.order[e0 + at] = (u32)j;
         b.l_in_off[at] = b.in_off[e]; b.l_in_len[at] = b.in_len[e]; b.l_start_bits[at] = b.start_bits[e];
-    }
+    });
 }
 
 // thread per launch position: the block kernel's results back into table order
@@ -358,20 +341,14 @@ __global__ void __launch_bounds__(256) bz2s_resolve_kernel(DecodeIO io, UnitCols
 // exclusive sum of scratch_per_unit(out_cap) over the fallback units inside the area, one CTA; a unit past the area reports
 // SWC_ERR_UNSUPPORTED and is not run
 __global__ void __launch_bounds__(1024) bz2s_fallback_place_kernel(DecodeIO io, UnitCols c, u64 area) {
-    __shared__ u64 part[1024];
-    const u64 n = io.n, per = (n + 1023) / 1024;
-    const u64 b = threadIdx.x * per < n ? threadIdx.x * per : n, e = b + per < n ? b + per : n;
+    __shared__ u64 part[1][1024];
+    u64 b, e;
+    cta_unit_run(io.n, b, e);
     u64 s = 0;
     for (u64 i = b; i < e; i++) s += c.run[i] ? bzip2::scratch_per_unit(io.out_cap[i]) : 0;
-    part[threadIdx.x] = s;
-    __syncthreads();
-    for (int d = 1; d < 1024; d <<= 1) {
-        const u64 v = threadIdx.x >= (u32)d ? part[threadIdx.x - d] : 0;
-        __syncthreads();
-        part[threadIdx.x] += v;
-        __syncthreads();
-    }
-    u64 at = part[threadIdx.x] - s;
+    part[0][threadIdx.x] = s;
+    cta_scan<1>(part);
+    u64 at = part[0][threadIdx.x] - s;
     for (u64 i = b; i < e; i++) {
         if (!c.run[i]) continue;
         const u64 need = bzip2::scratch_per_unit(io.out_cap[i]);
@@ -392,22 +369,15 @@ struct Layout {
     u8 *block_part, *area;
 
     Layout(void *base, u64 n, u64 nblk) {
-        size_t at = 0;
-        auto take = [&](auto *&ptr, u64 count) {
-            ptr = (std::remove_reference_t<decltype(ptr)>)((u8 *)base + at);
-            at += (count * sizeof(*ptr) + 255) & ~(size_t)255;
-        };
-        take(u.count, n); take(u.end_bit, n); take(u.first_blk, n); take(u.run_off, n); take(u.fb_off, n); take(u.flags, n);
-        take(u.run, n); take(u.totals, 2);
-        unit_bytes = at;
-        block_part = (u8 *)base + at;
-        take(b.in_off, nblk); take(b.in_len, nblk); take(b.start_bits, nblk); take(b.unit, nblk); take(b.out_len, nblk);
-        take(b.consumed, nblk); take(b.dst, nblk); take(b.status, nblk);
-        take(b.slot_off, nblk); take(b.slot_cap, nblk); take(b.slot_scr, nblk); take(b.order, nblk);
-        take(b.l_in_off, nblk); take(b.l_in_len, nblk); take(b.l_out_len, nblk); take(b.l_consumed, nblk); take(b.l_start_bits, nblk);
-        take(b.l_status, nblk);
-        fixed_bytes = at;
-        area = (u8 *)base + at;
+        Carver c(base);
+        c.cols(n, u.count, u.end_bit, u.first_blk, u.run_off, u.fb_off, u.flags, u.run);
+        c.cols(2, u.totals);
+        unit_bytes = c.at;
+        block_part = c.end();
+        c.cols(nblk, b.in_off, b.in_len, b.start_bits, b.unit, b.out_len, b.consumed, b.dst, b.status, b.slot_off, b.slot_cap,
+               b.slot_scr, b.order, b.l_in_off, b.l_in_len, b.l_out_len, b.l_consumed, b.l_start_bits, b.l_status);
+        fixed_bytes = c.at;
+        area = c.end();
     }
 };
 
@@ -420,17 +390,13 @@ struct Call {
     cudaStream_t s;
 };
 
-int scan(const Call &q, const Layout &l) {
+// the scan, unless the unit columns of `l` already hold it (`counted`), and the placement in a table of max_blocks entries
+// beside an area of `area` bytes
+int count_and_place(const Call &q, const Layout &l, u64 max_blocks, u64 area, bool counted) {
     const unsigned warps = (unsigned)((q.io.n * 32 + 255) / 256);
-    bz2s_scan_kernel<false><<<warps, 256, 0, q.s>>>(ScanArgs{q.io.in_base, q.io.in_off, q.io.in_len, q.io.n, l.u, l.b});
-    count_launch();
-    SWC_CUDA_TRY(cudaGetLastError());
-    return SWC_OK;
-}
-
-int place(const Call &q, const Layout &l, u64 max_blocks, u64 area) {
+    if (!counted) bz2s_scan_kernel<false><<<warps, 256, 0, q.s>>>(ScanArgs{q.io.in_base, q.io.in_off, q.io.in_len, q.io.n, l.u, l.b});
     bz2s_place_kernel<<<1, 1024, 0, q.s>>>(l.u, q.io.out_cap, q.io.n, max_blocks, area);
-    count_launch();
+    count_launch(counted ? 1 : 2);
     SWC_CUDA_TRY(cudaGetLastError());
     return SWC_OK;
 }
@@ -442,7 +408,7 @@ int decode(const Call &q, const Layout &l, u64 nblk, u64 slots, u64 area, bool c
     const unsigned unit_warps = (unsigned)((n * 32 + 255) / 256), unit_threads = (unsigned)((n + 255) / 256);
     int st;
     timing_mark(q.s);
-    if ((!counted && (st = scan(q, l))) || (st = place(q, l, nblk, area))) return st;
+    if ((st = count_and_place(q, l, nblk, area, counted))) return st;
     // idle table entries have no input and fail at once
     SWC_CUDA_TRY(cudaMemsetAsync(l.block_part, 0, l.fixed_bytes - l.unit_bytes, q.s));
     bz2s_slot_init_kernel<<<(unsigned)((slots + 255) / 256), 256, 0, q.s>>>(l.b, slots);
@@ -504,32 +470,25 @@ int32_t swc_bzip2_stream_decompress_batch(const uint8_t *in_base, const uint64_t
     if (missing(q.io) || max_blocks > 0xFFFFFFFFull || n > 0xFFFFFFFFull) return SWC_ERR_INVALID_ARG;
     int st;
     u64 nblk = max_blocks;
-    void *counted_at = nullptr;
     u64 fb_need = 0;
+    SplitScratch sc(scratch, q.s);
     if (max_blocks == 0) {
-        // the library counts first: the scan on the unit columns alone, then the totals back (one synchronisation)
-        const size_t unit_bytes = Layout(nullptr, n, 0).unit_bytes;
-        void *first = scratch;
-        if (scratch ? scratch_bytes < unit_bytes : (st = scratch_get(unit_bytes, &first, q.s)) != SWC_OK) return scratch ? SWC_ERR_INVALID_ARG : st;
-        const Layout l(first, n, 0);
-        if ((st = scan(q, l)) || (st = place(q, l, ~0ull, ~0ull))) return st;
+        // the library counts first: the scan on the unit columns alone, then the totals back
+        auto launch = [&](void *base, const u64 **t) {
+            const Layout l(base, n, 0);
+            *t = l.u.totals;
+            return count_and_place(q, l, ~0ull, ~0ull, false);
+        };
         u64 totals[2];
-        SWC_CUDA_TRY(cudaMemcpyAsync(totals, l.u.totals, 16, cudaMemcpyDeviceToHost, q.s));
-        SWC_CUDA_TRY(cudaStreamSynchronize(q.s));
+        if ((st = sc.count_first(scratch_bytes, Layout(nullptr, n, 0).unit_bytes, 2, totals, launch))) return st;
         if (totals[0] > 0xFFFFFFFFull) return SWC_ERR_UNSUPPORTED;
         nblk = totals[0] ? totals[0] : 1;
         fb_need = totals[1];
-        counted_at = first;
         if (scratch) {
             // the largest table that leaves the area one slot and the fallback of every unit: the units past it fall back,
             // so a scratch of swc_bzip2_stream_batch_scratch_bytes(n, 0, ...) gives every unit its exact status
             const u64 want = fb_need > slot_bytes() ? fb_need : slot_bytes();
-            u64 lo = 1, hi = nblk;
-            while (lo < hi) {
-                const u64 mid = lo + (hi - lo + 1) / 2;
-                if (fixed_bytes_for(n, mid) + want <= scratch_bytes) lo = mid; else hi = mid - 1;
-            }
-            nblk = lo;
+            nblk = largest_table(nblk, scratch_bytes, [&](u64 m) { return fixed_bytes_for(n, m) + want; });
         }
     }
     const size_t fixed = fixed_bytes_for(n, nblk);
@@ -551,11 +510,11 @@ int32_t swc_bzip2_stream_decompress_batch(const uint8_t *in_base, const uint64_t
         u64 slots = free_b / 2 / slot_bytes();
         slots = slots < 1 ? 1 : slots > nblk ? nblk : slots;
         area = slots * slot_bytes() > fb ? slots * slot_bytes() : fb;
-        if ((st = scratch_get(fixed + area, &scratch, q.s))) return st;
+        if ((st = sc.seat(fixed + area))) return st;
     }
     const u64 slots_fit = area / slot_bytes();
     const u64 slots = slots_fit < nblk ? slots_fit : nblk;
-    return decode(q, Layout(scratch, n, nblk), nblk, slots, area, scratch == counted_at);   // the pool may have moved
+    return decode(q, Layout(sc.p, n, nblk), nblk, slots, area, sc.counted);
 }
 
 }  // extern "C"

@@ -37,6 +37,43 @@ struct DecodeIO : UnitIO {
     u64 *consumed;
 };
 
+// The contiguous run [b, e) of n units that thread threadIdx.x of a 1024-thread CTA takes: ceil(n / 1024) of them, in order.
+__device__ __forceinline__ void cta_unit_run(u64 n, u64 &b, u64 &e) {
+    const u64 per = (n + 1023) / 1024;
+    b = threadIdx.x * per < n ? threadIdx.x * per : n;
+    e = b + per < n ? b + per : n;
+}
+
+// the inclusive prefix sum of part[k][0..1024) in place (one CTA of 1024 threads)
+template <int K> __device__ __forceinline__ void cta_scan(u64 (*part)[1024]) {
+    __syncthreads();
+    for (int d = 1; d < 1024; d <<= 1) {
+        u64 v[K];
+#pragma unroll
+        for (int k = 0; k < K; k++) v[k] = threadIdx.x >= (u32)d ? part[k][threadIdx.x - d] : 0;
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < K; k++) part[k][threadIdx.x] += v[k];
+        __syncthreads();
+    }
+}
+
+// One CTA: entries [0, cnt) in launch order by a counting sort on key(j) in 0..64, the leading zeros of a size, so the
+// largest come first.  put(j, at) gives entry j launch position `at`.
+template <typename Key, typename Put> __device__ __forceinline__ void clz_order(u64 cnt, Key key, Put put) {
+    __shared__ u32 start[65];
+    if (threadIdx.x < 65) start[threadIdx.x] = 0;
+    __syncthreads();
+    for (u64 j = threadIdx.x; j < cnt; j += blockDim.x) atomicAdd(&start[key(j)], 1u);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        u32 at = 0;
+        for (int k = 0; k < 65; k++) { const u32 h = start[k]; start[k] = at; at += h; }
+    }
+    __syncthreads();
+    for (u64 j = threadIdx.x; j < cnt; j += blockDim.x) put(j, atomicAdd(&start[key(j)], 1u));
+}
+
 // launch bookkeeping (swc_kernel_launches)
 void count_launch(int n = 1);
 // record a CUDA failure; returns SWC_ERR_CUDA
@@ -52,8 +89,9 @@ int cuda_fail(cudaError_t e, const char *where);
 void timing_mark(cudaStream_t stream);
 
 // scratch pool: grow-only per-device buffer, used when the caller passes no scratch
-int scratch_get(size_t bytes, void **p, cudaStream_t stream);
-// grow-only arenas reused across calls: slot 0 = kernel scratch, 1..3 = device staging of the *_batch_host paths
-int arena_get(int slot, size_t bytes, void **p, cudaStream_t stream);
+int scratch_get(size_t bytes, void **p, cudaStream_t stream, bool *kept = nullptr);
+// grow-only arenas reused across calls: slot 0 = kernel scratch, 1..3 = device staging of the *_batch_host paths.
+// *kept (optional): the arena was large enough, so it still holds what the last call left in it.
+int arena_get(int slot, size_t bytes, void **p, cudaStream_t stream, bool *kept = nullptr);
 
 }  // namespace swc

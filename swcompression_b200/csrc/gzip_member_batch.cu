@@ -15,7 +15,6 @@
 //                                    wrongCRC, consumed exactly its span and starts where member k - 1 ended
 //   fallback     thread per unit     from the first member that was not accepted, the sequential walk: gzip_parse,
 //                                    inflate_serial, serial CRC-32 and trailer, member after member
-#include <type_traits>
 #include <vector>
 #include "../../include/swcgpu.h"
 #include "archive_header.cuh"
@@ -131,21 +130,15 @@ __global__ void __launch_bounds__(1024) gzm_sort_kernel(Units u, u64 *cand, u64 
 
 // exclusive sum of the candidate counts in unit order; a unit is placed iff its candidates end inside the table
 __global__ void __launch_bounds__(1024) gzm_place_kernel(Units u, u64 n, u64 max_members) {
-    __shared__ u64 part[1024];
-    const u64 per = (n + 1023) / 1024;
-    const u64 b = threadIdx.x * per < n ? threadIdx.x * per : n, e = b + per < n ? b + per : n;
+    __shared__ u64 part[1][1024];
+    u64 b, e;
+    cta_unit_run(n, b, e);
     u64 s = 0;
     for (u64 i = b; i < e; i++) s += u.count[i];
-    part[threadIdx.x] = s;
-    __syncthreads();
-    for (int d = 1; d < 1024; d <<= 1) {
-        const u64 v = threadIdx.x >= (u32)d ? part[threadIdx.x - d] : 0;
-        __syncthreads();
-        part[threadIdx.x] += v;
-        __syncthreads();
-    }
-    if (threadIdx.x == 1023) u.sums[0] = part[1023];
-    u64 at = part[threadIdx.x] - s;
+    part[0][threadIdx.x] = s;
+    cta_scan<1>(part);
+    if (threadIdx.x == 1023) u.sums[0] = part[0][1023];
+    u64 at = part[0][threadIdx.x] - s;
     for (u64 i = b; i < e; i++) {
         const u64 nb = u.count[i];
         u.first[i] = at + nb <= max_members ? at : NONE;
@@ -307,21 +300,17 @@ struct Layout {
     void *inner;
 
     Layout(void *base, u64 n, u64 nblk) {
-        size_t at = 0;
-        auto take = [&](auto *&ptr, u64 count) {
-            ptr = (std::remove_reference_t<decltype(ptr)>)((u8 *)base + at);
-            at += (count * sizeof(*ptr) + 255) & ~(size_t)255;
-        };
-        take(u.count, n); take(u.fill, n); take(u.first, n); take(u.spans, n); take(u.resume, n); take(u.written, n);
-        take(u.members, n); take(u.run, n); take(u.sums, 1);
-        unit_bytes = at;
-        take(t.cand, nblk);
-        const size_t cols = at;
-        take(t.in_off, nblk); take(t.in_len, nblk); take(t.out_off, nblk); take(t.out_cap, nblk);
-        cols_bytes = at - cols;
-        take(t.out_len, nblk); take(t.consumed, nblk); take(t.status, nblk);
-        table_bytes = at;
-        inner = (u8 *)base + at;
+        Carver c(base);
+        c.cols(n, u.count, u.fill, u.first, u.spans, u.resume, u.written, u.members, u.run);
+        c.cols(1, u.sums);
+        unit_bytes = c.at;
+        c.cols(nblk, t.cand);
+        const size_t cols = c.at;
+        c.cols(nblk, t.in_off, t.in_len, t.out_off, t.out_cap);
+        cols_bytes = c.at - cols;
+        c.cols(nblk, t.out_len, t.consumed, t.status);
+        table_bytes = c.at;
+        inner = c.end();
     }
 };
 
@@ -335,10 +324,14 @@ struct Call {
     cudaStream_t s;
 };
 
-int count(const Call &q, const Layout &l, u64 max_members) {
-    SWC_CUDA_TRY(cudaMemsetAsync(l.u.count, 0, q.io.n * 8, q.s));
-    int st = checks::gzip_scan(checks::GzipScan{q.io.in_base, q.io.in_off, q.io.in_len, q.io.n, l.u.count, nullptr, nullptr, 0, true}, q.s);
-    if (st) return st;
+// the candidate counts, unless the unit columns of `l` already hold them (`counted`), and the placement in a table of
+// max_members entries
+int count(const Call &q, const Layout &l, u64 max_members, bool counted) {
+    if (!counted) {
+        SWC_CUDA_TRY(cudaMemsetAsync(l.u.count, 0, q.io.n * 8, q.s));
+        int st = checks::gzip_scan(checks::GzipScan{q.io.in_base, q.io.in_off, q.io.in_len, q.io.n, l.u.count, nullptr, nullptr, 0, true}, q.s);
+        if (st) return st;
+    }
     gzm_place_kernel<<<1, 1024, 0, q.s>>>(l.u, q.io.n, max_members);
     count_launch();
     SWC_CUDA_TRY(cudaGetLastError());
@@ -352,13 +345,7 @@ int decode(const Call &q, const Layout &l, u64 nblk, bool counted, u64 out_total
     const unsigned unit_threads = (unsigned)((n + 255) / 256);
     int st;
     timing_mark(q.s);
-    if (counted) {
-        gzm_place_kernel<<<1, 1024, 0, q.s>>>(l.u, n, nblk);
-        count_launch();
-        SWC_CUDA_TRY(cudaGetLastError());
-    } else if ((st = count(q, l, nblk))) {
-        return st;
-    }
+    if ((st = count(q, l, nblk, counted))) return st;
     if ((st = checks::gzip_scan(checks::GzipScan{q.io.in_base, q.io.in_off, q.io.in_len, n, l.u.fill, l.u.first, l.t.cand, 0, true}, q.s)))
         return st;
     timing_mark(q.s);
@@ -421,18 +408,16 @@ int32_t swc_gzip_multi_unarchive_batch(const uint8_t *in_base, const uint64_t *i
     if (table && !(member_off && member_cap && member_end && member_in_off)) return SWC_ERR_INVALID_ARG;
     int st;
     u64 nblk = max_members, arena = 0;
-    const bool caller = scratch != nullptr;
+    SplitScratch sc(scratch, q.s);
     if (max_members == 0) {
-        // the library counts first: the scan on the unit columns alone, then the candidate total back (one synchronisation)
-        const size_t unit_bytes = Layout(nullptr, n, 0).unit_bytes;
-        void *first = scratch;
-        if (scratch ? scratch_bytes < unit_bytes : (st = scratch_get(unit_bytes, &first, q.s)) != SWC_OK)
-            return scratch ? SWC_ERR_INVALID_ARG : st;
-        const Layout l(first, n, 0);
-        if ((st = count(q, l, ~0ull))) return st;
+        // the library counts first: the scan on the unit columns alone, then the candidate total back
+        auto launch = [&](void *base, const u64 **t) {
+            const Layout l(base, n, 0);
+            *t = l.u.sums;
+            return count(q, l, ~0ull, false);
+        };
         u64 total = 0;
-        SWC_CUDA_TRY(cudaMemcpyAsync(&total, l.u.sums, 8, cudaMemcpyDeviceToHost, q.s));
-        SWC_CUDA_TRY(cudaStreamSynchronize(q.s));
+        if ((st = sc.count_first(scratch_bytes, Layout(nullptr, n, 0).unit_bytes, 1, &total, launch))) return st;
         // the table is capped at in_len / 20 + 1 entries per unit, as many members as a unit can hold: a file of
         // look-alikes (one candidate every 4 bytes) must not size the scratch, its units past the cap fall back
         std::vector<u64> lens;
@@ -449,24 +434,19 @@ int32_t swc_gzip_multi_unarchive_batch(const uint8_t *in_base, const uint64_t *i
         if (max_members == 0) {
             // the largest table the caller's scratch holds beside the decode stage's scratch; the units past it fall back
             if (batch_scratch_bytes(n, 1, arena) > scratch_bytes) return SWC_ERR_INVALID_ARG;
-            u64 lo = 1, hi = nblk;
-            while (lo < hi) {
-                const u64 mid = lo + (hi - lo + 1) / 2;
-                if (batch_scratch_bytes(n, mid, arena) <= scratch_bytes) lo = mid; else hi = mid - 1;
-            }
-            nblk = lo;
+            nblk = largest_table(nblk, scratch_bytes, [&](u64 m) { return batch_scratch_bytes(n, m, arena); });
         } else if (scratch_bytes < batch_scratch_bytes(n, nblk, 0)) {
             return SWC_ERR_INVALID_ARG;
         }
     } else {
         scratch_bytes = batch_scratch_bytes(n, nblk, arena);
-        if ((st = scratch_get(scratch_bytes, &scratch, q.s))) return st;
+        if ((st = sc.seat(scratch_bytes))) return st;
     }
-    const Layout l(scratch, n, nblk);
+    const Layout l(sc.p, n, nblk);
     // the decode stage takes the rest of the scratch and the arena it covers; spans outside that arena take the fallback
     const size_t inner = scratch_bytes - l.table_bytes;
     const u64 out_total = unarchive_batch_arena(nblk, inner);
-    return decode(q, l, nblk, caller && max_members == 0, out_total, inner);   // a pool that grows loses the counts
+    return decode(q, l, nblk, sc.counted, out_total, inner);
 }
 
 }  // extern "C"

@@ -73,6 +73,19 @@ struct DevBuf {
 };
 
 inline size_t round16(size_t v) { return (v + 15) & ~(size_t)15; }
+inline size_t round256(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// Lays typed columns out from `base`, each on a 256-byte boundary so that no column overlaps its neighbour whatever its
+// type and length; `at` counts the bytes taken.  A null base only sizes the layout.  The batches that split their units
+// into sub-units take their unit columns first, at offsets that do not depend on the table size, so the counts taken on a
+// layout of n units and no table are valid in the same scratch's layout of n units and any table.
+struct Carver {
+    u8 *base;
+    size_t at = 0;
+    explicit Carver(void *b) : base((u8 *)b) {}
+    template <typename... T> void cols(u64 count, T *&...p) { ((p = (T *)(base + at), at += round256(count * sizeof(T))), ...); }
+    u8 *end() const { return base + at; }
+};
 
 // a batch's n u64 lengths (device) into `v` on the host, for planning the batch (blocking: waits for `s`)
 inline int read_lens(const u64 *d, u64 n, cudaStream_t s, std::vector<u64> &v) {
@@ -91,8 +104,8 @@ inline int read_lens(const u64 *d, u64 n, cudaStream_t s, std::vector<u64> &v) {
 template <typename T> struct Col { size_t off = 0, n = 0; bool dev_only = false; };
 class UnitTable {
   public:
-    template <typename T> Col<T> in(size_t n) { Col<T> c{host_.size(), n, false}; host_.resize(host_.size() + span(n * sizeof(T))); return c; }
-    template <typename T> Col<T> out(size_t n) { Col<T> c{out_bytes_, n, true}; out_bytes_ += span(n * sizeof(T)); return c; }
+    template <typename T> Col<T> in(size_t n) { Col<T> c{host_.size(), n, false}; host_.resize(host_.size() + round256(n * sizeof(T))); return c; }
+    template <typename T> Col<T> out(size_t n) { Col<T> c{out_bytes_, n, true}; out_bytes_ += round256(n * sizeof(T)); return c; }
     template <typename T> T *host(Col<T> c) { return (T *)(host_.data() + c.off); }
     template <typename T> T *dev(Col<T> c) const { return (T *)(dev_.as<u8>() + (c.dev_only ? host_.size() : 0) + c.off); }
     size_t bytes() const { return host_.size() + out_bytes_; }
@@ -110,7 +123,6 @@ class UnitTable {
         return SWC_OK;
     }
   private:
-    static size_t span(size_t b) { return (b + 255) & ~(size_t)255; }
     std::vector<u8> host_;
     size_t out_bytes_ = 0;
     DevBuf dev_;
@@ -183,6 +195,48 @@ int decode_unit(UnitTable &t, const UnitCols &c, const u8 *d_in, size_t start, s
         if (r.status != SWC_ERR_OUTPUT_OVERFLOW || !(cap = grow(cap, r.out_len))) break;
     }
     return SWC_OK;
+}
+
+// The scratch of a batch that splits its units into sub-units (DESIGN §2), and its count-first step for a call that
+// leaves the table size to the library.  count_first() seats unit_bytes of unit columns on the caller's scratch
+// (SWC_ERR_INVALID_ARG when that is smaller) or on the pool; launch(base, &totals) lays the codec's unit columns out at
+// base, launches its count and points `totals` at its k device totals, which come back into `out` with one
+// synchronisation.  seat() then takes the whole layout from the pool when the caller gave no scratch.  `counted` tells
+// whether the unit columns at `p` hold the counts: always on the caller's scratch, on the pool only if it kept its contents.
+struct SplitScratch {
+    void *p;                 // the caller's scratch, or the pool once seated
+    const bool caller;
+    cudaStream_t s;
+    bool counted = false;
+    SplitScratch(void *scratch, cudaStream_t stream) : p(scratch), caller(scratch != nullptr), s(stream) {}
+    template <typename Launch> int count_first(size_t scratch_bytes, size_t unit_bytes, int k, u64 *out, Launch launch) {
+        int st;
+        if (caller ? scratch_bytes < unit_bytes : (st = scratch_get(unit_bytes, &p, s)) != SWC_OK)
+            return caller ? SWC_ERR_INVALID_ARG : st;
+        const u64 *totals = nullptr;
+        if ((st = launch(p, &totals))) return st;
+        SWC_CUDA_TRY(cudaMemcpyAsync(out, totals, k * sizeof(u64), cudaMemcpyDeviceToHost, s));
+        SWC_CUDA_TRY(cudaStreamSynchronize(s));
+        counted = true;
+        return SWC_OK;
+    }
+    int seat(size_t bytes) {
+        if (caller) return SWC_OK;
+        bool kept = false;
+        const int st = scratch_get(bytes, &p, s, &kept);
+        counted = counted && kept;
+        return st;
+    }
+};
+
+// the largest table size m in [1, hi] whose layout, bytes_of(m) bytes, fits `cap`; 1 when none does
+template <typename Bytes> u64 largest_table(u64 hi, size_t cap, Bytes bytes_of) {
+    u64 lo = 1;
+    while (lo < hi) {
+        const u64 mid = lo + (hi - lo + 1) / 2;
+        if (bytes_of(mid) <= cap) lo = mid; else hi = mid - 1;
+    }
+    return lo;
 }
 
 // batched Deflate on device-resident tables (api_deflate.cu); start_bits may be null; scratch == nullptr -> library pool

@@ -336,20 +336,14 @@ __global__ void __launch_bounds__(256, 4) lz4_exec_kernel(Args a, const u64 *rec
 
 // exclusive prefix sum of per-unit record capacities (in_len / 3 + 2), one block
 __global__ void __launch_bounds__(1024) lz4_rec_scan_kernel(const u64 *blk_len, u64 n, u64 *base) {
-    __shared__ u64 part[1024];
-    const u64 per = (n + 1023) / 1024;
-    const u64 b = threadIdx.x * per, e = b + per < n ? b + per : n;
+    __shared__ u64 part[1][1024];
+    u64 b, e;
+    cta_unit_run(n, b, e);
     u64 sum = 0;
     for (u64 i = b; i < e; i++) sum += (blk_len[i] & ~(1ull << 63)) / 3 + 2;
-    part[threadIdx.x] = sum;
-    __syncthreads();
-    for (int d = 1; d < 1024; d <<= 1) {
-        u64 v = threadIdx.x >= (u32)d ? part[threadIdx.x - d] : 0;
-        __syncthreads();
-        part[threadIdx.x] += v;
-        __syncthreads();
-    }
-    u64 run = part[threadIdx.x] - sum;
+    part[0][threadIdx.x] = sum;
+    cta_scan<1>(part);
+    u64 run = part[0][threadIdx.x] - sum;
     for (u64 i = b; i < e; i++) { base[i] = run; run += (blk_len[i] & ~(1ull << 63)) / 3 + 2; }
 }
 

@@ -14,7 +14,6 @@
 //   exec          warp per block    lz4_exec_kernel / lz4_fallback_kernel, unchanged replay
 //   xxh32, check  warp per unit     content checksum over the decoded bytes; turns OK into checksumMismatch
 #include <climits>
-#include <type_traits>
 #include "../../include/swcgpu.h"
 #include "checks.cuh"
 #include "host_util.h"
@@ -192,18 +191,12 @@ struct UnitCols {
 // exclusive sums of the units' block counts and record slots, one CTA; marks the units that do not fit
 __global__ void __launch_bounds__(1024) lz4f_place_kernel(UnitCols c, u64 n, u64 max_blocks, u64 rec_cap) {
     __shared__ u64 part[2][1024];
-    const u64 per = (n + 1023) / 1024;
-    const u64 b = threadIdx.x * per < n ? threadIdx.x * per : n, e = b + per < n ? b + per : n;
+    u64 b, e;
+    cta_unit_run(n, b, e);
     u64 sb = 0, sr = 0;
     for (u64 i = b; i < e; i++) { sb += c.info[i].n_blocks; sr += c.rec_need[i]; }
     part[0][threadIdx.x] = sb; part[1][threadIdx.x] = sr;
-    __syncthreads();
-    for (int d = 1; d < 1024; d <<= 1) {
-        const u64 v0 = threadIdx.x >= (u32)d ? part[0][threadIdx.x - d] : 0, v1 = threadIdx.x >= (u32)d ? part[1][threadIdx.x - d] : 0;
-        __syncthreads();
-        part[0][threadIdx.x] += v0; part[1][threadIdx.x] += v1;
-        __syncthreads();
-    }
+    cta_scan<2>(part);
     if (threadIdx.x == 1023) { c.totals[0] = part[0][1023]; c.totals[1] = part[1][1023]; }
     u64 rb = part[0][threadIdx.x] - sb, rr = part[1][threadIdx.x] - sr;
     for (u64 i = b; i < e; i++) {
@@ -300,20 +293,15 @@ struct Layout {
     u8 *block_part;
 
     Layout(void *base, u64 n, u64 nblk) {
-        size_t at = 0;
-        auto take = [&](auto *&ptr, u64 count) {
-            ptr = (std::remove_reference_t<decltype(ptr)>)((u8 *)base + at);
-            at += (count * sizeof(*ptr) + 255) & ~(size_t)255;
-        };
-        take(u.info, n); take(u.rec_need, n); take(u.rec_first, n); take(u.first_blk, n); take(u.n_chain, n); take(u.no_dict, n);
-        take(u.chain_len, n); take(u.chain_status, n); take(u.cc_len, n); take(u.cc, n); take(u.totals, 2);
-        unit_bytes = at;
-        block_part = (u8 *)base + at;
-        take(b.off, nblk); take(b.len, nblk); take(b.par_len, nblk); take(b.ck_len, nblk); take(b.stored_ck, nblk); take(b.ck, nblk);
-        take(b.no_dict, nblk); take(b.out_off, nblk); take(b.cap, nblk); take(b.out_len, nblk); take(b.rec_base, nblk);
-        take(b.status, nblk); take(b.rec_count, nblk);
-        fixed_bytes = at;
-        recs = (u64 *)((u8 *)base + at);
+        Carver c(base);
+        c.cols(n, u.info, u.rec_need, u.rec_first, u.first_blk, u.n_chain, u.no_dict, u.chain_len, u.chain_status, u.cc_len, u.cc);
+        c.cols(2, u.totals);
+        unit_bytes = c.at;
+        block_part = c.end();
+        c.cols(nblk, b.off, b.len, b.par_len, b.ck_len, b.stored_ck, b.ck, b.no_dict, b.out_off, b.cap, b.out_len, b.rec_base,
+               b.status, b.rec_count);
+        fixed_bytes = c.at;
+        recs = (u64 *)c.end();
     }
 };
 
@@ -420,21 +408,19 @@ int32_t swc_lz4_frame_decompress_batch(const uint8_t *in_base, const uint64_t *i
     if (missing(q.io) || !consumed_bytes || max_blocks > 0xFFFFFFFFull) return SWC_ERR_INVALID_ARG;
     int st;
     u64 nblk = max_blocks, rec_cap = 0;
-    void *counted_at = nullptr;
+    SplitScratch sc(scratch, q.s);
     if (max_blocks == 0) {
-        // the library counts first: the walk on the unit columns alone, then the totals back (one synchronisation)
-        const size_t unit_bytes = Layout(nullptr, n, 0).fixed_bytes;
-        void *first = scratch;
-        if (scratch ? scratch_bytes < unit_bytes : (st = scratch_get(unit_bytes, &first, q.s)) != SWC_OK) return scratch ? SWC_ERR_INVALID_ARG : st;
-        const Layout l(first, n, 0);
-        if ((st = count_and_place(q, l, ~0ull, ~0ull))) return st;
+        // the library counts first: the walk on the unit columns alone, then the totals back
+        auto launch = [&](void *base, const u64 **t) {
+            const Layout l(base, n, 0);
+            *t = l.u.totals;
+            return count_and_place(q, l, ~0ull, ~0ull);
+        };
         u64 totals[2];
-        SWC_CUDA_TRY(cudaMemcpyAsync(totals, l.u.totals, 16, cudaMemcpyDeviceToHost, q.s));
-        SWC_CUDA_TRY(cudaStreamSynchronize(q.s));
+        if ((st = sc.count_first(scratch_bytes, Layout(nullptr, n, 0).unit_bytes, 2, totals, launch))) return st;
         if (totals[0] > 0xFFFFFFFFull) return SWC_ERR_UNSUPPORTED;
         nblk = totals[0] ? totals[0] : 1;
         rec_cap = totals[1];
-        counted_at = first;
         if (scratch && scratch_bytes < scratch_bytes_for(n, nblk, rec_cap)) return SWC_ERR_INVALID_ARG;
     } else if (scratch) {
         const size_t fixed = scratch_bytes_for(n, nblk, 0);
@@ -448,8 +434,8 @@ int32_t swc_lz4_frame_decompress_batch(const uint8_t *in_base, const uint64_t *i
         for (u64 i = 0; i < n; i++) total += lens[i];
         rec_cap = rec_slots_for(total, nblk);
     }
-    if (!scratch && (st = scratch_get(scratch_bytes_for(n, nblk, rec_cap), &scratch, q.s))) return st;
-    return decode(q, Layout(scratch, n, nblk), nblk, rec_cap, scratch == counted_at);   // the pool may have moved
+    if ((st = sc.seat(scratch_bytes_for(n, nblk, rec_cap)))) return st;
+    return decode(q, Layout(sc.p, n, nblk), nblk, rec_cap, sc.counted);
 }
 
 }  // extern "C"

@@ -13,7 +13,6 @@
 //   xxh32        warp per block   block checksums over the stored bytes in the output
 //   xxh32        warp per unit    content checksum over the input
 //   finish       warp per unit    header, checksum words, EndMark, content checksum; out_len and status
-#include <type_traits>
 #include <vector>
 #include "../../include/swcgpu.h"
 #include "compress_host.h"
@@ -54,20 +53,14 @@ __device__ __forceinline__ void put32(u8 *p, u32 v) { p[0] = (u8)v; p[1] = (u8)(
 __host__ __device__ __forceinline__ u64 blocks_of(u64 len, u64 bs) { return len / bs + (len % bs != 0); }
 
 __global__ void __launch_bounds__(1024) lz4fc_place_kernel(FrameArgs f, UnitCols c, u64 max_blocks) {
-    __shared__ u64 part[1024];
-    const u64 n = f.n, per = (n + 1023) / 1024;
-    const u64 b = threadIdx.x * per < n ? threadIdx.x * per : n, e = b + per < n ? b + per : n;
+    __shared__ u64 part[1][1024];
+    u64 b, e;
+    cta_unit_run(f.n, b, e);
     u64 sum = 0;
     for (u64 i = b; i < e; i++) sum += blocks_of(f.in_len[i], f.bs);
-    part[threadIdx.x] = sum;
-    __syncthreads();
-    for (int d = 1; d < 1024; d <<= 1) {
-        const u64 v = threadIdx.x >= (u32)d ? part[threadIdx.x - d] : 0;
-        __syncthreads();
-        part[threadIdx.x] += v;
-        __syncthreads();
-    }
-    u64 at = part[threadIdx.x] - sum;
+    part[0][threadIdx.x] = sum;
+    cta_scan<1>(part);
+    u64 at = part[0][threadIdx.x] - sum;
     for (u64 i = b; i < e; i++) {
         const u64 len = f.in_len[i], nb = blocks_of(len, f.bs);
         const bool fits = nb <= (at < max_blocks ? max_blocks - at : 0);
@@ -194,14 +187,11 @@ struct Layout {
     size_t bytes = 0;              // the columns
 
     Layout(void *base, u64 n, u64 nblk) {
-        auto take = [&](auto *&ptr, u64 count) {
-            ptr = (std::remove_reference_t<decltype(ptr)>)((u8 *)base + bytes);
-            bytes += (count * sizeof(*ptr) + 255) & ~(size_t)255;
-        };
-        take(u.first_blk, n); take(u.nb, n); take(u.pos, n); take(u.st, n); take(u.cc_len, n); take(u.cc, n);
-        take(b.in_off, nblk); take(b.in_len, nblk); take(b.dict_off, nblk); take(b.dict_len, nblk); take(b.cap, nblk);
-        take(b.res_len, nblk); take(b.out_off, nblk); take(b.ck_len, nblk); take(b.scr_off, nblk); take(b.status, nblk);
-        take(b.stored, nblk); take(b.ck, nblk);
+        Carver c(base);
+        c.cols(n, u.first_blk, u.nb, u.pos, u.st, u.cc_len, u.cc);
+        c.cols(nblk, b.in_off, b.in_len, b.dict_off, b.dict_len, b.cap, b.res_len, b.out_off, b.ck_len, b.scr_off, b.status,
+               b.stored, b.ck);
+        bytes = c.at;
     }
 };
 

@@ -38,13 +38,14 @@ struct Pool { void *p = nullptr; size_t bytes = 0; };
 static std::mutex g_pool_mu;
 static Pool g_pools[64][4];      // [device][slot]: 0 kernel scratch, 1-3 staging arenas of the *_batch_host paths
 
-int scratch_get(size_t bytes, void **p, cudaStream_t stream) { return arena_get(0, bytes, p, stream); }
+int scratch_get(size_t bytes, void **p, cudaStream_t stream, bool *kept) { return arena_get(0, bytes, p, stream, kept); }
 
-int arena_get(int slot, size_t bytes, void **p, cudaStream_t stream) {
+int arena_get(int slot, size_t bytes, void **p, cudaStream_t stream, bool *kept) {
     int dev = 0;
     SWC_CUDA_TRY(cudaGetDevice(&dev));
     std::lock_guard<std::mutex> lk(g_pool_mu);
     Pool &pool = g_pools[dev & 63][slot & 3];
+    if (kept) *kept = pool.p && pool.bytes >= bytes;
     if (pool.bytes < bytes) {
         if (pool.p) {
             SWC_CUDA_TRY(cudaStreamSynchronize(stream));

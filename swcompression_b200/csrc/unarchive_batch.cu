@@ -29,17 +29,13 @@ struct Scratch {
     void *inflate;
     size_t inflate_bytes;
 };
-size_t col(size_t b) { return (b + 255) & ~(size_t)255; }
-size_t columns_bytes(u64 n) { return 2 * col(n * 8) + 2 * col(n * 4); }
+size_t columns_bytes(u64 n) { return 2 * round256(n * 8) + 2 * round256(n * 4); }
 Scratch seat(void *p, u64 n, size_t bytes) {
-    u8 *s = (u8 *)p;
     Scratch r;
-    r.d_off = (u64 *)s;
-    r.d_len = (u64 *)(s + col(n * 8));
-    r.hstat = (int32_t *)(s + 2 * col(n * 8));
-    r.check = (u32 *)(s + 2 * col(n * 8) + col(n * 4));
-    r.inflate = s + columns_bytes(n);
-    r.inflate_bytes = bytes - columns_bytes(n);
+    Carver c(p);
+    c.cols(n, r.d_off, r.d_len, r.hstat, r.check);
+    r.inflate = c.end();
+    r.inflate_bytes = bytes - c.at;
     return r;
 }
 

@@ -16,7 +16,6 @@
 //            the block's LZMA2 decode has finished, or SHA-256 on lane 0.
 // The index is compared with the blocks by walking the stream's block headers and LZMA2 chunk headers again (no per-block
 // state is kept: the sizes of a block that decoded cleanly can be read back from its headers).
-#include <type_traits>
 #include "../../include/swcgpu.h"
 #include "checks_device.cuh"
 #include "host_util.h"
@@ -265,22 +264,16 @@ __global__ void __launch_bounds__(256) xzb_walk_kernel(UnitIO io, Units u, Table
 // exclusive sum of the qualifying units' record counts in unit order; a unit is placed iff its records end inside the
 // table (a prefix rule).  Marks every unit for the fallback.
 __global__ void __launch_bounds__(1024) xzb_place_kernel(Units u, u64 n, u64 max_blocks) {
-    __shared__ u64 part[1024];
-    const u64 per = (n + 1023) / 1024;
-    const u64 b = threadIdx.x * per < n ? threadIdx.x * per : n, e = b + per < n ? b + per : n;
+    __shared__ u64 part[1][1024];
+    u64 b, e;
+    cta_unit_run(n, b, e);
     u64 s = 0;
     for (u64 i = b; i < e; i++) s += (u.flags[i] & F_OK) ? u.count[i] : 0;
-    part[threadIdx.x] = s;
+    part[0][threadIdx.x] = s;
     if (threadIdx.x == 0) u.sums[0] = 0;
-    __syncthreads();
-    for (int d = 1; d < 1024; d <<= 1) {
-        const u64 v = threadIdx.x >= (u32)d ? part[threadIdx.x - d] : 0;
-        __syncthreads();
-        part[threadIdx.x] += v;
-        __syncthreads();
-    }
-    if (threadIdx.x == 1023) u.sums[1] = part[1023];
-    u64 at = part[threadIdx.x] - s, used = 0;
+    cta_scan<1>(part);
+    if (threadIdx.x == 1023) u.sums[1] = part[0][1023];
+    u64 at = part[0][threadIdx.x] - s, used = 0;
     for (u64 i = b; i < e; i++) {
         const bool ok = (u.flags[i] & F_OK) != 0;
         const u64 nb = ok ? u.count[i] : 0;
@@ -299,18 +292,7 @@ __global__ void __launch_bounds__(1024) xzb_place_kernel(Units u, u64 n, u64 max
 // of the block kernel holds its 2 x 28 304 B of model until its slower warp ends, so the long blocks go first, 2 to a CTA,
 // and a file's short last block fills in behind them instead of idling its partner's slot.
 __global__ void __launch_bounds__(1024) xzb_order_kernel(Units u, Table t) {
-    __shared__ u32 start[65];
-    const u64 cnt = u.sums[0];
-    if (threadIdx.x < 65) start[threadIdx.x] = 0;
-    __syncthreads();
-    for (u64 e = threadIdx.x; e < cnt; e += blockDim.x) atomicAdd(&start[__clzll((long long)t.size[e])], 1u);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        u32 at = 0;
-        for (int k = 0; k < 65; k++) { const u32 h = start[k]; start[k] = at; at += h; }
-    }
-    __syncthreads();
-    for (u64 e = threadIdx.x; e < cnt; e += blockDim.x) t.order[atomicAdd(&start[__clzll((long long)t.size[e])], 1u)] = (u32)e;
+    clz_order(u.sums[0], [&](u64 e) -> u32 { return __clzll((long long)t.size[e]); }, [&](u64 e, u32 at) { t.order[at] = (u32)e; });
 }
 
 // Warp per launch position: the block at the entry's start, as xz_kernel would decode it there (the input bounded by the
@@ -409,25 +391,22 @@ struct Layout {
     size_t unit_bytes, bytes;
 
     Layout(void *base, u64 n, u64 nblk) {
-        size_t at = 0;
-        auto take = [&](auto *&ptr, u64 count) {
-            ptr = (std::remove_reference_t<decltype(ptr)>)((u8 *)base + at);
-            at += (count * sizeof(*ptr) + 255) & ~(size_t)255;
-        };
-        take(u.count, n); take(u.total, n); take(u.first, n); take(u.flags, n); take(u.run, n); take(u.sums, 2);
-        unit_bytes = at;
-        take(t.unit, nblk); take(t.ctype, nblk); take(t.start, nblk); take(t.out_at, nblk); take(t.size, nblk);
-        take(t.order, nblk); take(t.status, nblk); take(t.end, nblk); take(t.got, nblk); take(t.unpadded, nblk);
-        bytes = at;
+        Carver c(base);
+        c.cols(n, u.count, u.total, u.first, u.flags, u.run);
+        c.cols(2, u.sums);
+        unit_bytes = c.at;
+        c.cols(nblk, t.unit, t.ctype, t.start, t.out_at, t.size, t.order, t.status, t.end, t.got, t.unpadded);
+        bytes = c.at;
     }
 };
 
 size_t block_scratch_bytes(u64 n, u64 nblk) { return Layout(nullptr, n, nblk).bytes; }
 
-int count_and_place(const UnitIO &io, const Layout &l, u64 max_blocks, cudaStream_t s) {
-    xzb_walk_kernel<false><<<(unsigned)((io.n + 255) / 256), 256, 0, s>>>(io, l.u, l.t);
+// the walk, unless the unit columns of `l` already hold it (`counted`), and the placement in a table of max_blocks entries
+int count_and_place(const UnitIO &io, const Layout &l, u64 max_blocks, bool counted, cudaStream_t s) {
+    if (!counted) xzb_walk_kernel<false><<<(unsigned)((io.n + 255) / 256), 256, 0, s>>>(io, l.u, l.t);
     xzb_place_kernel<<<1, 1024, 0, s>>>(l.u, io.n, max_blocks);
-    count_launch(2);
+    count_launch(counted ? 1 : 2);
     SWC_CUDA_TRY(cudaGetLastError());
     return SWC_OK;
 }
@@ -437,12 +416,7 @@ int block_batch(const UnitIO &io, u32 *parallel_blocks, const Layout &l, u64 nbl
     const unsigned unit_threads = (unsigned)((io.n + 255) / 256);
     int st;
     timing_mark(s);
-    if (counted) {
-        xzb_place_kernel<<<1, 1024, 0, s>>>(l.u, io.n, nblk);
-        count_launch();
-    } else if ((st = count_and_place(io, l, nblk, s))) {
-        return st;
-    }
+    if ((st = count_and_place(io, l, nblk, counted, s))) return st;
     xzb_walk_kernel<true><<<unit_threads, 256, 0, s>>>(io, l.u, l.t);
     xzb_order_kernel<<<1, 1024, 0, s>>>(l.u, l.t);
     count_launch(2);
@@ -497,30 +471,22 @@ int32_t swc_xz_block_unarchive_batch(const uint8_t *in_base, const uint64_t *in_
     int st;
     if ((st = configure())) return st;
     u64 nblk = max_blocks;
-    void *counted_at = nullptr;
+    SplitScratch sc(scratch, s);
     if (max_blocks == 0) {
-        // the library counts first: the walk on the unit columns alone, then the record total back (one synchronisation)
-        void *first = scratch;
-        if (!scratch && (st = scratch_get(Layout(nullptr, n, 0).unit_bytes, &first, s))) return st;
-        const Layout l(first, n, 0);
-        if ((st = count_and_place(io, l, ~0ull, s))) return st;
+        // the library counts first: the walk on the unit columns alone, then the record total back
+        auto launch = [&](void *base, const u64 **t) {
+            const Layout l(base, n, 0);
+            *t = l.u.sums + 1;
+            return count_and_place(io, l, ~0ull, false, s);
+        };
         u64 records = 0;
-        SWC_CUDA_TRY(cudaMemcpyAsync(&records, l.u.sums + 1, 8, cudaMemcpyDeviceToHost, s));
-        SWC_CUDA_TRY(cudaStreamSynchronize(s));
+        if ((st = sc.count_first(scratch_bytes, Layout(nullptr, n, 0).unit_bytes, 1, &records, launch))) return st;
         nblk = records < 1 ? 1 : records > 0xFFFFFFFFull ? 0xFFFFFFFFull : records;
-        counted_at = first;
-        if (scratch) {
-            // the largest table the caller's scratch holds; the units past it fall back
-            u64 lo = 1, hi = nblk;
-            while (lo < hi) {
-                const u64 mid = lo + (hi - lo + 1) / 2;
-                if (block_scratch_bytes(n, mid) <= scratch_bytes) lo = mid; else hi = mid - 1;
-            }
-            nblk = lo;
-        }
+        // the largest table the caller's scratch holds; the units past it fall back
+        if (scratch) nblk = largest_table(nblk, scratch_bytes, [&](u64 m) { return block_scratch_bytes(n, m); });
     }
-    if (!scratch && (st = scratch_get(block_scratch_bytes(n, nblk), &scratch, s))) return st;
-    return block_batch(io, parallel_blocks, Layout(scratch, n, nblk), nblk, scratch == counted_at, s);   // the pool may have moved
+    if ((st = sc.seat(block_scratch_bytes(n, nblk)))) return st;
+    return block_batch(io, parallel_blocks, Layout(sc.p, n, nblk), nblk, sc.counted, s);
 }
 
 int32_t swc_xz_occupancy(int32_t *lzma_warps_per_sm, int32_t *xz_warps_per_sm) {
