@@ -334,7 +334,7 @@ int32_t swc_bzip2_decompress_batch(const uint8_t *in_base, const uint64_t *in_of
                                    uint64_t n, void *cuda_stream);
 /* One .bz2 stream per unit with the blocks of every stream decoded side by side, device memory, one asynchronous enqueue on
  * `cuda_stream`.  Unit i is in_base[in_off[i] ..+ in_len[i]) in the layout above, decoded as BZip2.decompress(data:) decodes
- * it: the first stream, the bytes behind it ignored (multi-stream input: swc_bzip2_multi_decompress).
+ * it: the first stream, the bytes behind it ignored (multi-stream input: swc_bzip2_multi_decompress_batch).
  *   Equality: for every unit and capacity, status[i] is what swc_bzip2_decompress_batch returns for the same unit and
  *     capacity; on SWC_OK and SWC_BZIP2_WRONG_CRC the bytes [0, out_len[i]) and consumed_bits[i] are equal too.
  *   Overflow: the one exception is out_len[i] on SWC_ERR_OUTPUT_OVERFLOW.  When the stream validated block-parallel it is
@@ -361,6 +361,41 @@ int32_t swc_bzip2_stream_decompress_batch(const uint8_t *in_base, const uint64_t
                                           uint64_t *out_len, uint64_t *consumed_bits, int32_t *status,
                                           uint64_t n, uint64_t max_blocks,
                                           void *scratch, size_t scratch_bytes, void *cuda_stream);
+/* BZip2.multiDecompress(data:) (BZip2.swift:40-48) over n multi-stream .bz2 files (pbzip2 output, the multistream dumps,
+ * `cat a.bz2 b.bz2`), device memory, on `cuda_stream`, with the blocks of every stream of every file decoded side by side.
+ * The scan takes the block magics at every bit from bit 32 to the unit end into one block table; the blocks decode as in
+ * swc_bzip2_stream_decompress_batch and are laid out back to back; a thread per unit walks the streams as the reference
+ * does (header, each block the next table entry, combined CRC per stream, align) and the stream kernel decodes the rest of
+ * a unit from its first stream not accepted, stream after stream.
+ *   Equality: for every unit whose capacity suffices, status[i] is what swc_bzip2_multi_decompress returns for the same
+ *     bytes.  On SWC_OK out_base[out_off[i] ..+ out_len[i]) holds the streams back to back; on SWC_BZIP2_WRONG_CRC every
+ *     stream walked, up to and including the failing one, whose bytes [stream_end[k - 1], out_len[i]) are the reference's
+ *     payload (the table's last entry is the failing stream).  A 0-byte unit is SWC_OK with 0 streams.  On every other
+ *     status out_len[i] = n_streams[i] = 0, also for an error in a later stream (1-3 trailing bytes: wrongMagic; a trailing
+ *     "BZh0": wrongBlockSize), except:
+ *   Overflow: SWC_ERR_OUTPUT_OVERFLOW with out_len[i] > out_cap[i].  When every stream validated block-parallel out_len[i]
+ *     is the exact size, so one rerun with that capacity is final; otherwise it is the stream kernel's lower bound.
+ *   Stream table (n_streams, stream_off, stream_cap, stream_end, stream_in_off: device, n entries for the first three; the
+ *     last four all or none; n_streams may be NULL on its own): n_streams[i] is the number of streams returned, also when
+ *     it exceeds stream_cap[i]; at most stream_cap[i] entries are written at stream_off[i]: stream_end, each stream's
+ *     output end relative to out_off[i] (swc_bzip2_multi_decompress's stream_ends), and stream_in_off, each stream's first
+ *     byte inside the unit.  in_len[i] / 14 + 1 entries always suffice (an empty stream is 14 bytes).
+ *   parallel_streams (device, n entries, or NULL): the leading streams of unit i accepted from the block stage and fitting
+ *     out_cap[i]; the stream kernel decoded the rest.
+ *   Block table, scratch and graph capture: as swc_bzip2_stream_decompress_batch, with swc_bzip2_stream_batch_scratch_bytes,
+ *     except that a unit's candidates are its block magics in the whole unit and it is placed when its header is at byte 0
+ *     and a block or end magic at bit 32.  max_blocks and the scratch size change the speed, never the results, apart from
+ *     SWC_ERR_UNSUPPORTED when the stream kernel's scratch (about 7.5 x out_cap[i]) no longer fits for a unit.
+ *   Writes: nothing is written outside [out_off[i], out_off[i] + out_cap[i]) and the unit's stream table entries, and no
+ *     byte outside the unit's input range affects its result. */
+int32_t swc_bzip2_multi_decompress_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                                         uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                         uint64_t *out_len, int32_t *status,
+                                         uint64_t *n_streams, const uint64_t *stream_off, const uint64_t *stream_cap,
+                                         uint64_t *stream_end, uint64_t *stream_in_off,   /* table: may be NULL */
+                                         uint32_t *parallel_streams /* device, n, or NULL */,
+                                         uint64_t n, uint64_t max_blocks,
+                                         void *scratch, size_t scratch_bytes, void *cuda_stream);
 
 /* ---- LZMA / LZMA2 -------------------------------------------------------------------------------------------
  * LZMA.decompress(data:)                                   Sources/LZMA/LZMA.swift:25-34

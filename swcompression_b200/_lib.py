@@ -132,6 +132,7 @@ def lib():
         L.swc_bzip2_stream_batch_scratch_bytes.restype = C.c_size_t
         L.swc_bzip2_stream_batch_scratch_bytes.argtypes = [u64, u64, u64]
         L.swc_bzip2_stream_decompress_batch.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, u64, u64, vp, sz, vp]
+        L.swc_bzip2_multi_decompress_batch.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, u64, u64, vp, sz, vp]
         L.swc_lzma_decompress.argtypes = [vp, sz, C.POINTER(vp), szp, szp]
         L.swc_lzma_decompress_raw.argtypes = [vp, sz, i32, i32, i32, C.c_int64, C.c_int64, C.POINTER(vp), szp, szp]
         L.swc_lzma2_decompress.argtypes = [vp, sz, C.POINTER(vp), szp, szp]

@@ -59,7 +59,7 @@ def pack_units(units, align=16):
 
 
 class Batch:
-    """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'bzip2_stream', 'lzma2', 'gzip', 'zlib', 'xz',
+    """Device-resident batch for one codec ('deflate', 'lz4_block', 'bzip2', 'bzip2_stream', 'bzip2_multi', 'lzma2', 'gzip', 'zlib', 'xz',
     'xz_blocks', 'gzip_multi', 'lz4_frame', 'lz4_block_compress', 'lz4_frame_compress', 'deflate_compress', 'gzip_archive',
     'zlib_archive', 'bzip2_compress', 'tar').
 
@@ -75,6 +75,11 @@ class Batch:
     of swc_bzip2_stream_batch_scratch_bytes (capped at `scratch_bytes`, which the library then runs in slices) and run()
     reads nothing back (it can be captured in a CUDA graph).  None lets the library count the blocks first (one
     synchronisation) and use its pool, or `scratch_bytes` of caller scratch.
+    'bzip2_multi' decodes every stream of each unit (BZip2.multiDecompress, BZip2.swift:40-48) with the blocks of all
+    streams of all units side by side; results() gives the status, the streams' total size and 0 consumed bytes, streams(i)
+    unit i as multiDecompress returns it, stream_table(i) its stream ends and starts, and parallel_streams() how many
+    streams of each unit the block stage gave (the rest took the stream kernel).  `stream_cap` is each unit's stream table
+    capacity (None: in_len // 14 + 1, always enough); `max_blocks` and `scratch_bytes` work as for 'bzip2_stream'.
 
     'gzip' / 'zlib' decode one archive per unit (GzipArchive.unarchive, GzipArchive.swift:38-47, 79-100 / ZlibArchive.unarchive,
     ZlibArchive.swift:25-42): the first member only, whose status, size and consumed bytes results() returns.  With
@@ -127,7 +132,7 @@ class Batch:
 
     def __init__(self, codec, in_buf, in_off, in_len, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=None,
                  headers=False, dict_id=None, max_blocks=None, frame_flags=None, gzip_options=None, max_in_bytes=None,
-                 max_members=None, member_cap=None):
+                 max_members=None, member_cap=None, stream_cap=None):
         self.codec = codec
         self.device = torch.device(device)
         self.n = len(in_off)
@@ -158,8 +163,21 @@ class Batch:
         self.d_dict_off = self.d_dict_len = None
         self.block_size = int(block_size) if block_size is not None else LZ4_FRAME_BLOCK_SIZE if codec == "lz4_frame_compress" else 1
         self.dict_id, self.max_blocks = dict_id, 0 if max_blocks is None else int(max_blocks)
-        if codec == "bzip2_stream":
+        if codec in ("bzip2_stream", "bzip2_multi"):
             self.d_aux = None
+            if codec == "bzip2_multi":
+                self.d_parallel = torch.zeros(self.n, dtype=torch.int32, device=self.device)
+                scap = np.asarray(in_len, dtype=np.uint64) // np.uint64(14) + np.uint64(1) if stream_cap is None else stream_cap
+                scap = np.broadcast_to(np.asarray(scap, dtype=np.uint64), (self.n,)).copy()
+                soff = np.zeros(self.n, dtype=np.uint64)
+                if self.n > 1:
+                    soff[1:] = np.cumsum(scap[:-1])
+                self.h_stream_off, self.h_stream_cap = soff, scap
+                self.d_stream_off, self.d_stream_cap = t(soff), t(scap)
+                self.d_n_streams = torch.zeros(self.n, dtype=torch.int64, device=self.device)
+                slots = max(int(scap.sum()), 1)
+                self.d_stream_end = torch.zeros(slots, dtype=torch.int64, device=self.device)
+                self.d_stream_in_off = torch.zeros(slots, dtype=torch.int64, device=self.device)
             if self.max_blocks or scratch_bytes is not None:
                 nbytes = _lib.lib().swc_bzip2_stream_batch_scratch_bytes(self.n, self.max_blocks, self.out_total)
                 if scratch_bytes is not None:
@@ -280,9 +298,9 @@ class Batch:
     @classmethod
     def tar_of(cls, other, entry_cap=None):
         """A 'tar' batch over another batch's device outputs (unit i: other.d_out[out_off[i] ..+ out_len[i]), with no
-        copy): a 'gzip' / 'gzip_multi' / 'xz' / 'xz_blocks' / 'bzip2_stream' batch of .tar.gz / .tar.xz / .tar.bz2 files
-        feeds the walk in the same stream ('gzip_multi' outputs are each unit's members back to back, so a BGZF .tar.gz
-        is walked in place).  Each unit is walked over at most other's out_cap bytes (an overflowing decode reports a required size
+        copy): a 'gzip' / 'gzip_multi' / 'xz' / 'xz_blocks' / 'bzip2_stream' / 'bzip2_multi' batch of .tar.gz / .tar.xz /
+        .tar.bz2 files feeds the walk in the same stream ('gzip_multi' and 'bzip2_multi' outputs are each unit's members or
+        streams back to back, so a BGZF .tar.gz or a pbzip2 .tar.bz2 is walked in place).  Each unit is walked over at most other's out_cap bytes (an overflowing decode reports a required size
         past its region), and a unit whose decode failed is not walked: it reports that status in every status column.
         Entry tables default to out_cap // 512 + 1 records, enough for any archive the outputs can hold without a
         negative size."""
@@ -295,10 +313,10 @@ class Batch:
     @classmethod
     def from_units(cls, codec, units, out_cap, device="cuda:0", aux=None, scratch_bytes=None, block_size=None, headers=False,
                    dict_id=None, max_blocks=None, frame_flags=None, gzip_options=None, max_in_bytes=None, max_members=None,
-                   member_cap=None):
+                   member_cap=None, stream_cap=None):
         buf, offs, lens = pack_units(units)
         return cls(codec, buf, offs, lens, out_cap, device, aux, scratch_bytes, block_size, headers, dict_id, max_blocks,
-                   frame_flags, gzip_options, max_in_bytes, max_members, member_cap)
+                   frame_flags, gzip_options, max_in_bytes, max_members, member_cap, stream_cap)
 
     def run(self):
         L = _lib.lib()
@@ -387,6 +405,14 @@ class Batch:
                                                      p(self.d_out_off), p(self.d_out_cap), p(self.d_out_len), p(self.d_consumed),
                                                      p(self.d_status), self.n, self.max_blocks, opt(self.d_scratch),
                                                      0 if self.d_scratch is None else self.d_scratch.numel(), stream)
+        elif self.codec == "bzip2_multi":
+            opt = lambda t: None if t is None else p(t)
+            st = L.swc_bzip2_multi_decompress_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), p(self.d_out),
+                                                    p(self.d_out_off), p(self.d_out_cap), p(self.d_out_len), p(self.d_status),
+                                                    p(self.d_n_streams), p(self.d_stream_off), p(self.d_stream_cap),
+                                                    p(self.d_stream_end), p(self.d_stream_in_off), p(self.d_parallel), self.n,
+                                                    self.max_blocks, opt(self.d_scratch),
+                                                    0 if self.d_scratch is None else self.d_scratch.numel(), stream)
         elif self.codec == "tar":
             opt = lambda t: None if t is None else p(t)
             st = L.swc_tar_walk_batch(p(self.d_in), p(self.d_in_off), p(self.d_in_len), opt(self.d_in_cap), opt(self.d_in_status),
@@ -403,8 +429,8 @@ class Batch:
 
     def results(self):
         """-> (status int32[n], out_len int64[n], consumed int64[n]) on the host (synchronises).  consumed is in bits for
-        'deflate', 'bzip2' and 'bzip2_stream', in bytes for 'lzma2', 'gzip', 'zlib' and 'lz4_frame', and 0 for 'xz', 'xz_blocks'
-        and the compress codecs."""
+        'deflate', 'bzip2' and 'bzip2_stream', in bytes for 'lzma2', 'gzip', 'zlib' and 'lz4_frame', and 0 for 'xz', 'xz_blocks',
+        'bzip2_multi' and the compress codecs."""
         torch.cuda.synchronize(self.device)
         return self.d_status.cpu().numpy(), self.d_out_len.cpu().numpy(), self.d_consumed.cpu().numpy()
 
@@ -417,6 +443,37 @@ class Batch:
         """-> uint32[n] of a 'gzip_multi' batch: the members of each unit accepted from the parallel spans (synchronises)"""
         torch.cuda.synchronize(self.device)
         return self.d_parallel.cpu().numpy().view(np.uint32)
+
+    def parallel_streams(self):
+        """-> uint32[n] of a 'bzip2_multi' batch: the leading streams of each unit accepted from the block stage
+        (synchronises)"""
+        torch.cuda.synchronize(self.device)
+        return self.d_parallel.cpu().numpy().view(np.uint32)
+
+    def stream_table(self, i):
+        """-> (stream ends in the output, stream starts in the unit) of unit i of a 'bzip2_multi' batch, at most its stream
+        capacity (synchronises)"""
+        torch.cuda.synchronize(self.device)
+        k = min(int(self.d_n_streams[i].item()), int(self.h_stream_cap[i]))
+        o = int(self.h_stream_off[i])
+        return [int(v) for v in self.d_stream_end[o:o + k].cpu()], [int(v) for v in self.d_stream_in_off[o:o + k].cpu()]
+
+    def streams(self, i):
+        """unit i of a 'bzip2_multi' batch as BZip2.multiDecompress returns it: a list of bytes, one per stream; raises the
+        matching BZip2Error otherwise (on wrongCRC its payload is the failing stream's bytes) (synchronises)"""
+        from .errors import error_for
+        st, ln, _ = self.results()
+        ends, _ = self.stream_table(i)
+        out = self.output(i)
+        parts, prev = [], 0
+        for e in ends:
+            parts.append(out[prev:e])
+            prev = e
+        if int(st[i]) == 0:
+            return parts
+        if int(st[i]) == 210:                                   # wrongCRC: the failing stream is the table's last
+            raise error_for(210, parts[-1:])
+        raise error_for(int(st[i]), None)
 
     def member_table(self, i):
         """-> (member ends in the output, member starts in the unit) of unit i of a 'gzip_multi' batch, at most its member

@@ -167,6 +167,9 @@ __device__ __forceinline__ u32 xpow_bz(u64 nbytes) {
 }
 
 // ---------------------------------------------------------------- the kernel
+// MULTI: the multi-stream walk of Args::multi.  It is its own instantiation, so the single-stream and block launches run
+// exactly the code they ran before it.
+template <bool MULTI>
 __global__ void __launch_bounds__(WARPS * 32) bzip2_kernel(Args a) {
     __shared__ WarpSmem smem[WARPS];
     const u32 lane = lane_id(), warp = threadIdx.x >> 5;
@@ -175,18 +178,35 @@ __global__ void __launch_bounds__(WARPS * 32) bzip2_kernel(Args a) {
     WarpSmem &S = smem[warp];
     const u64 cap = a.out_cap[unit];
     u8 *out = a.out_base + a.out_off[unit];
-    // per-unit scratch: bwt bytes [scr_cap] | successor array u32 [scr_cap] | selectors u8 [32768]
+    // per-unit scratch: bwt bytes [scr_cap] | successor array u32 [scr_cap] | selectors u8 [32768].  MULTI forms the
+    // pointers per block from a reloaded offset instead: held across blocks they cost the walk a spill.
     const u64 scr_cap = bwt_capacity(cap);
-    u8 *scr = a.scratch + a.scr_off[unit];
+    u8 *scr = MULTI ? nullptr : a.scratch + a.scr_off[unit];
     u8 *bwt = scr;
     u32 *succ = (u32 *)(scr + scr_cap + 16);
     u8 *selectors = (u8 *)(succ + scr_cap) + 16;
 
+    // multi: lane 0 keeps the walk's stream count in taken[unit] and writes each stream's table entry, its start when
+    // the stream begins and its output end when it ends (its state lives in memory, not in registers)
+    auto entry = [&](u64 k) -> u64 { return k < a.multi.stream_cap[unit] ? a.multi.stream_off[unit] + k : ~0ull; };
+    auto stream_begins = [&](u64 at) {
+        if (lane == 0 && a.multi.stream_end) { const u64 e = entry(a.multi.taken[unit]); if (e != ~0ull) a.multi.stream_in_off[e] = at; }
+    };
+    auto stream_ends = [&](u64 end) {
+        if (lane) return;
+        const u64 k = a.multi.taken[unit];
+        if (a.multi.stream_end) { const u64 e = entry(k); if (e != ~0ull) a.multi.stream_end[e] = end; }
+        a.multi.taken[unit] = k + 1;
+    };
     Bits br;
-    br.init(a.in_base + a.in_off[unit], a.in_len[unit]);
+    {
+        const u64 base = MULTI ? a.multi.at_in[unit] : 0;
+        br.init(a.in_base + a.in_off[unit] + base, a.in_len[unit] - base);
+        if (MULTI) stream_begins(base);
+    }
     const i64 total_bits = br.avail;
     int status = SWC_OK;
-    u64 op = 0;
+    u64 op = MULTI ? a.multi.at_out[unit] : 0;
     u32 total_crc = 0;
 #define FAIL(c) do { status = (c); goto done; } while (0)
 
@@ -198,6 +218,8 @@ __global__ void __launch_bounds__(WARPS * 32) bzip2_kernel(Args a) {
         if (br.avail < (i64)sb) FAIL(SWC_BZIP2_WRONG_MAGIC);
         if (sb) (void)br.get((int)sb);
     } else {
+        if (MULTI && br.avail == 0) goto done;                                     // reader.isFinished: no stream
+    next_stream:
         if (br.avail < 32) FAIL(SWC_BZIP2_WRONG_MAGIC);                                  // BZip2.swift:53
         if (br.get(16) != 0x425A) FAIL(SWC_BZIP2_WRONG_MAGIC);                           // 'B','Z' (uint16() == 0x5a42 LE)
         if (br.get(8) != 104) FAIL(SWC_BZIP2_WRONG_VERSION);
@@ -211,11 +233,24 @@ __global__ void __launch_bounds__(WARPS * 32) bzip2_kernel(Args a) {
         const u32 block_crc = br.get(32);
         if (magic == 0x177245385090ull) {
             if (total_crc != block_crc) FAIL(SWC_BZIP2_WRONG_CRC);                   // :86
-            break;
+            if (!MULTI) break;
+            // multiDecompress (:40-48): the stream is returned, the reader aligned, and a new stream read while bytes are left
+            stream_ends(op);
+            br.need32();
+            br.skip((int)(br.avail & 7));                                            // total_bits is whole bytes
+            if (br.avail == 0) break;
+            stream_begins(a.multi.at_in[unit] + (u64)(total_bits - br.avail) / 8);
+            total_crc = 0;
+            goto next_stream;
         }
         if (magic != 0x314159265359ull) FAIL(SWC_BZIP2_WRONG_BLOCK_TYPE);
 
         // ------------------------------------------------ decode(_:_:) BZip2.swift:97-270
+        if (MULTI) {
+            scr = bwt = a.scratch + a.scr_off[unit];
+            succ = (u32 *)(scr + scr_cap + 16);
+            selectors = (u8 *)(succ + scr_cap) + 16;
+        }
         if (br.avail < 41) FAIL(SWC_BZIP2_WRONG_MAGIC);
         if (br.get(1) != 0) FAIL(SWC_BZIP2_RANDOMIZED_BLOCK);
         const u32 orig_ptr = br.get(24);
@@ -570,6 +605,15 @@ __global__ void __launch_bounds__(WARPS * 32) bzip2_kernel(Args a) {
     }
 done:
 #undef FAIL
+    if (MULTI) {
+        // the failing stream's bytes are the reference's payload, so on wrongCRC its entry is the table's last; any other
+        // error drops every stream
+        const bool kept = status == SWC_OK || status == SWC_BZIP2_WRONG_CRC;
+        if (status == SWC_BZIP2_WRONG_CRC) stream_ends(op);
+        if (!kept && status != SWC_ERR_OUTPUT_OVERFLOW) op = 0;
+        if (status == SWC_ERR_OUTPUT_OVERFLOW && op <= cap) op = cap + 1;          // a text overflow: still a bound
+        if (lane == 0 && a.multi.n_streams) a.multi.n_streams[unit] = kept ? a.multi.taken[unit] : 0;
+    }
     if (lane == 0) {
         a.out_len[unit] = op;
         a.consumed[unit] = (u64)(total_bits - br.avail);
@@ -586,7 +630,8 @@ int launch(const Args &a, cudaStream_t stream) {
         return (int)SWC_OK;
     });
     if (st) return st;
-    bzip2_kernel<<<(unsigned)((a.n + WARPS - 1) / WARPS), WARPS * 32, 0, stream>>>(a);
+    if (a.multi.at_in) bzip2_kernel<true><<<(unsigned)((a.n + WARPS - 1) / WARPS), WARPS * 32, 0, stream>>>(a);
+    else bzip2_kernel<false><<<(unsigned)((a.n + WARPS - 1) / WARPS), WARPS * 32, 0, stream>>>(a);
     count_launch();
     SWC_CUDA_TRY(cudaGetLastError());
     return SWC_OK;

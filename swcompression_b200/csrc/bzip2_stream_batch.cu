@@ -1,9 +1,10 @@
-// bzip2_stream_batch.cu — batched BZip2.decompress(data:) (reference Sources/BZip2/BZip2.swift:50-95) with the blocks of
-// every stream decoded side by side.  With a caller scratch and max_blocks > 0 the call is a fixed sequence of launches: no
-// host read, no allocation (DESIGN.md §4.17).
+// bzip2_stream_batch.cu — batched BZip2.decompress(data:) (reference Sources/BZip2/BZip2.swift:50-95) and
+// BZip2.multiDecompress(data:) (:40-48) with the blocks of every stream decoded side by side.  With a caller scratch and
+// max_blocks > 0 the call is a fixed sequence of launches: no host read, no allocation (DESIGN.md §4.17, §4.21).
 //
 //   scan<COUNT>   warp per unit     the BZh1-9 header, then block magics at every bit offset from bit 32 up to the first
-//                                   end-of-stream magic (the matcher of checks::find_bzip2_magics)
+//                                   end-of-stream magic (the matcher of checks::find_bzip2_magics); multi: up to the unit
+//                                   end, every stream's blocks in one run of the table
 //   place         one CTA           first_blk = exclusive sum of the candidate counts; a unit whose header fails, whose first
 //                                   block is not at bit 32, that has no end magic, whose candidates do not fit the table, or
 //                                   that the fallback could not hold behind every unit in front of it is marked for fallback
@@ -16,8 +17,11 @@
 //     copy        CTA per slot      slot -> region, 16-byte stores, clipped to out_cap
 //   resolve       warp per unit     the reference's in-order walk as a validator: block k ends at candidate k + 1 (the last
 //                                   at the end magic), the stored combined CRC is the fold of the block CRCs; else fallback
+//     multi:      thread per unit   the walk across streams (header, blocks that are the next table entries, end magic and
+//                                   combined CRC, align); the first stream not accepted or not fitting is the resume point
 //   fallback      one CTA, then     per-unit scratch offsets of the fallback units (exclusive sum inside the dead block
-//                 warp per unit     area), then bzip2_kernel in stream mode over exactly those units
+//                 warp per unit     area), then bzip2_kernel in stream mode over exactly those units (multi: from the
+//                                   resume point, stream after stream)
 #include <vector>
 #include "../../include/swcgpu.h"
 #include "bzip2.cuh"
@@ -37,9 +41,11 @@ enum : u8 { F_OK = 1, F_PLACED = 2 };                          // header, first 
 __host__ __device__ __forceinline__ u64 slot_bytes() { return SLOT_OUT + bzip2::scratch_per_unit(SLOT); }
 
 // the per-unit columns the stages hand to each other
+// multi: after the resolve, count / end_bit / run_off hold the resume point (streams taken, its input byte, its output
+// byte) and first_blk the stream kernel's consumed bits
 struct UnitCols {
-    u64 *count;        // block candidates in front of the first end magic
-    u64 *end_bit;      // bit of the first end magic in the unit (NONE: none)
+    u64 *count;        // block candidates in front of the first end magic (multi: in the whole unit)
+    u64 *end_bit;      // bit of the first end magic in the unit (NONE: none; multi: the unit's end)
     u64 *first_blk;    // the unit's first entry in the block table
     u64 *run_off;      // bytes of the unit's output placed so far (carried across slices)
     u64 *fb_off;       // fallback: scratch offset inside the area
@@ -72,8 +78,10 @@ struct ScanArgs {
 };
 
 // One warp per unit.  Each trip covers 512 bytes, 16 per lane in order, so lane order is position order; a lane's masks
-// of those 16 bytes stay in registers for FILL's second look.  The trip that meets the first end magic is the last.
-template <bool FILL>
+// of those 16 bytes stay in registers for FILL's second look.  The trip that meets the first end magic is the last; with
+// MULTI the scan runs to the unit end and takes every block magic (stream headers need no scan: the resolve reads them
+// where its walk puts them).
+template <bool FILL, bool MULTI>
 __global__ void __launch_bounds__(256) bz2s_scan_kernel(ScanArgs a) {
     const u64 unit = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (unit >= a.n) return;
@@ -87,7 +95,7 @@ __global__ void __launch_bounds__(256) bz2s_scan_kernel(ScanArgs a) {
         return;
     }
     u64 total = 0, end = NONE, slot = FILL ? a.u.first_blk[unit] : 0;
-    for (u64 base = 4; base + 6 <= L && end == NONE; base += 512) {
+    for (u64 base = 4; base + 6 <= L && (MULTI || end == NONE); base += 512) {
         const u64 b0 = base + 16 * lane;
         u32 bm[4] = {0, 0, 0, 0}, em[4] = {0, 0, 0, 0};
         // the lane's 16 bytes and the 6 behind them: the three aligned 16-byte lines that hold them (a line that starts
@@ -129,7 +137,9 @@ __global__ void __launch_bounds__(256) bz2s_scan_kernel(ScanArgs a) {
 #pragma unroll
         for (int j = 0; j < 16; j++) {
             const u32 mb = (bm[j >> 2] >> (8 * (j & 3))) & 0xFF, me = (em[j >> 2] >> (8 * (j & 3))) & 0xFF;
-            if (lane_end == NONE) {
+            if (MULTI) {
+                cnt += __popc(mb);
+            } else if (lane_end == NONE) {
                 if (me) {
                     const u32 e = __ffs(me) - 1;
                     cnt += __popc(mb & ((1u << e) - 1));
@@ -139,7 +149,7 @@ __global__ void __launch_bounds__(256) bz2s_scan_kernel(ScanArgs a) {
                 }
             }
         }
-        const u32 ends = __ballot_sync(SWC_FULL, lane_end != NONE);
+        const u32 ends = MULTI ? 0 : __ballot_sync(SWC_FULL, lane_end != NONE);
         const u32 fe = ends ? __ffs(ends) - 1 : 32;
         if (lane > fe) cnt = 0;
         u64 incl = cnt;
@@ -167,9 +177,11 @@ __global__ void __launch_bounds__(256) bz2s_scan_kernel(ScanArgs a) {
     if (!FILL && lane == 0) {
         // the first block must sit right behind the header (bit 32 is byte aligned)
         const bool first_at_32 = L >= 10 && p[4] == 0x31 && p[5] == 0x41 && p[6] == 0x59 && p[7] == 0x26 && p[8] == 0x53 && p[9] == 0x59;
+        // multi: an empty first stream has its end magic there
+        const bool end_at_32 = L >= 10 && p[4] == 0x17 && p[5] == 0x72 && p[6] == 0x45 && p[7] == 0x38 && p[8] == 0x50 && p[9] == 0x90;
         a.u.count[unit] = total;
-        a.u.end_bit[unit] = end;
-        a.u.flags[unit] = first_at_32 && end != NONE ? F_OK : 0;
+        a.u.end_bit[unit] = MULTI ? L * 8 : end;
+        a.u.flags[unit] = MULTI ? (first_at_32 || end_at_32 ? F_OK : 0) : first_at_32 && end != NONE ? F_OK : 0;
     }
 }
 
@@ -338,6 +350,72 @@ __global__ void __launch_bounds__(256) bz2s_resolve_kernel(DecodeIO io, UnitCols
     c.run[unit] = 0;
 }
 
+// Thread per unit: the reference's multiDecompress walk (BZip2.swift:40-95) over the unit's table entries in position order
+// as a validator.  A stream at byte P needs 32 bits and the header BZh1-9; from bit (P + 4) * 8 each block must be the next
+// table entry, start exactly where the walk stands, have decoded cleanly (its CRC included) and end where its consumed bits
+// say; at the end magic the stored CRC must be the fold of this stream's block CRCs, and the next stream starts at
+// ceil((e + 80) / 8).  A table entry the walk would step over (a look-alike in a payload, or in the CRC and padding in front
+// of the next header, whose bytes the layout has counted) ends acceptance at the current stream.  Reaching the unit end
+// with every stream accepted gives the final result (overflow included: its exact size); otherwise the first stream not
+// accepted, or the first that does not fit out_cap, is where the stream kernel resumes: its input byte goes to end_bit,
+// the output bytes in front of it to run_off and the streams taken to count.  The accepted streams' table entries are
+// written here.
+__global__ void __launch_bounds__(256) bz2m_resolve_kernel(UnitIO io, UnitCols c, BlockCols b, bzip2::Multi m, u32 *parallel) {
+    const u64 unit = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (unit >= io.n) return;
+    u64 at = 0, out = 0, taken = 0;                 // the resume point
+    u64 P = 0, sum = 0, s = 0;                      // the walk: next stream's byte, bytes and streams accepted
+    bool all = false;
+    const u64 L = io.in_len[unit], cap = io.out_cap[unit];
+    if (c.flags[unit] & F_PLACED) {
+        const u8 *p = io.in_base + io.in_off[unit];
+        const u64 f = c.first_blk[unit], nb = c.count[unit];
+        auto pos = [&](u64 k) { return (b.in_off[f + k] - io.in_off[unit]) * 8 + b.start_bits[f + k]; };
+        u64 k = 0;
+        for (;;) {
+            if (P == L) { all = true; break; }
+            if (L - P < 4 || p[P] != 'B' || p[P + 1] != 'Z' || p[P + 2] != 'h' || p[P + 3] < '1' || p[P + 3] > '9') break;
+            u64 bit = (P + 4) * 8, bytes = sum;
+            u32 crc = 0;
+            bool ok = true;
+            for (;;) {
+                if (bit + 80 > L * 8 || (k < nb && pos(k) < bit)) { ok = false; break; }
+                if (k < nb && pos(k) == bit) {
+                    if (b.status[f + k] != SWC_OK) { ok = false; break; }
+                    crc = ((crc << 1) | (crc >> 31)) ^ bits32_at(p, L, bit + 48);         // :83-84
+                    bytes += b.out_len[f + k];
+                    bit = (bit & ~7ull) + b.consumed[f + k];
+                    k++;
+                    continue;
+                }
+                const u64 magic = ((u64)bits32_at(p, L, bit) << 16) | (bits32_at(p, L, bit + 32) >> 16);
+                ok = magic == 0x177245385090ull && bits32_at(p, L, bit + 48) == crc;      // :86
+                break;
+            }
+            if (!ok) break;
+            if (m.stream_end && s < m.stream_cap[unit]) {
+                m.stream_end[m.stream_off[unit] + s] = bytes;
+                m.stream_in_off[m.stream_off[unit] + s] = P;
+            }
+            P = (bit + 80 + 7) / 8;
+            sum = bytes;
+            s++;
+            if (sum <= cap) { at = P; out = sum; taken = s; }
+        }
+    }
+    if (parallel) parallel[unit] = (u32)taken;
+    if (all) {
+        const bool over = sum > cap;
+        io.status[unit] = over ? SWC_ERR_OUTPUT_OVERFLOW : SWC_OK;
+        io.out_len[unit] = sum;
+        if (m.n_streams) m.n_streams[unit] = over ? 0 : s;
+        c.run[unit] = 0;
+        return;
+    }
+    if (m.n_streams) m.n_streams[unit] = 0;        // until the stream kernel finishes the unit
+    c.end_bit[unit] = at; c.run_off[unit] = out; c.count[unit] = taken;
+}
+
 // exclusive sum of scratch_per_unit(out_cap) over the fallback units inside the area, one CTA; a unit past the area reports
 // SWC_ERR_UNSUPPORTED and is not run
 __global__ void __launch_bounds__(1024) bz2s_fallback_place_kernel(DecodeIO io, UnitCols c, u64 area) {
@@ -385,16 +463,27 @@ size_t fixed_bytes_for(u64 n, u64 nblk) { return Layout(nullptr, n, nblk).fixed_
 // an upper bound of the fallback's scratch when every unit falls back: scratch_per_unit(c) <= 6 (c + c / 4 + 11) + 33 600
 u64 fallback_bound(u64 n, u64 out_total) { return 6 * (out_total + out_total / 4 + 11 * n) + 33600 * n; }
 
+// multi: the stream table and parallel_streams of swc_bzip2_multi_decompress_batch (the resume columns are filled in by
+// decode())
+struct Mode {
+    bool multi = false;
+    bzip2::Multi table = {};
+    u32 *parallel = nullptr;
+};
+
 struct Call {
-    DecodeIO io;
+    DecodeIO io;                // multi: consumed is null (the stream kernel's goes to a dead unit column)
     cudaStream_t s;
+    Mode mode;
 };
 
 // the scan, unless the unit columns of `l` already hold it (`counted`), and the placement in a table of max_blocks entries
 // beside an area of `area` bytes
 int count_and_place(const Call &q, const Layout &l, u64 max_blocks, u64 area, bool counted) {
     const unsigned warps = (unsigned)((q.io.n * 32 + 255) / 256);
-    if (!counted) bz2s_scan_kernel<false><<<warps, 256, 0, q.s>>>(ScanArgs{q.io.in_base, q.io.in_off, q.io.in_len, q.io.n, l.u, l.b});
+    const ScanArgs sa{q.io.in_base, q.io.in_off, q.io.in_len, q.io.n, l.u, l.b};
+    if (!counted && q.mode.multi) bz2s_scan_kernel<false, true><<<warps, 256, 0, q.s>>>(sa);
+    if (!counted && !q.mode.multi) bz2s_scan_kernel<false, false><<<warps, 256, 0, q.s>>>(sa);
     bz2s_place_kernel<<<1, 1024, 0, q.s>>>(l.u, q.io.out_cap, q.io.n, max_blocks, area);
     count_launch(counted ? 1 : 2);
     SWC_CUDA_TRY(cudaGetLastError());
@@ -412,7 +501,9 @@ int decode(const Call &q, const Layout &l, u64 nblk, u64 slots, u64 area, bool c
     // idle table entries have no input and fail at once
     SWC_CUDA_TRY(cudaMemsetAsync(l.block_part, 0, l.fixed_bytes - l.unit_bytes, q.s));
     bz2s_slot_init_kernel<<<(unsigned)((slots + 255) / 256), 256, 0, q.s>>>(l.b, slots);
-    bz2s_scan_kernel<true><<<unit_warps, 256, 0, q.s>>>(ScanArgs{q.io.in_base, q.io.in_off, q.io.in_len, n, l.u, l.b});
+    const ScanArgs sa{q.io.in_base, q.io.in_off, q.io.in_len, n, l.u, l.b};
+    if (q.mode.multi) bz2s_scan_kernel<true, true><<<unit_warps, 256, 0, q.s>>>(sa);
+    else bz2s_scan_kernel<true, false><<<unit_warps, 256, 0, q.s>>>(sa);
     count_launch(2);
     SWC_CUDA_TRY(cudaGetLastError());
     timing_mark(q.s);
@@ -431,43 +522,33 @@ int decode(const Call &q, const Layout &l, u64 nblk, u64 slots, u64 area, bool c
         SWC_CUDA_TRY(cudaGetLastError());
     }
     timing_mark(q.s);
-    bz2s_resolve_kernel<<<unit_warps, 256, 0, q.s>>>(q.io, l.u, l.b);
+    DecodeIO io = q.io;
+    if (q.mode.multi) {
+        bz2m_resolve_kernel<<<unit_threads, 256, 0, q.s>>>(io, l.u, l.b, q.mode.table, q.mode.parallel);
+        io.consumed = l.u.first_blk;
+    } else {
+        bz2s_resolve_kernel<<<unit_warps, 256, 0, q.s>>>(io, l.u, l.b);
+    }
     count_launch();
     timing_mark(q.s);
     // the block stage is over: its whole area is the fallback's scratch
-    bz2s_fallback_place_kernel<<<1, 1024, 0, q.s>>>(q.io, l.u, area);
+    bz2s_fallback_place_kernel<<<1, 1024, 0, q.s>>>(io, l.u, area);
     count_launch();
     SWC_CUDA_TRY(cudaGetLastError());
-    bzip2::Args fb{q.io, l.area, l.u.fb_off};
+    bzip2::Args fb{io, l.area, l.u.fb_off};
     fb.run = l.u.run;
+    if (q.mode.multi) {
+        fb.multi = q.mode.table;
+        fb.multi.at_in = l.u.end_bit; fb.multi.at_out = l.u.run_off; fb.multi.taken = l.u.count;
+    }
     if ((st = bzip2::launch(fb, q.s))) return st;
     timing_mark(q.s);
     return SWC_OK;
 }
 
-}  // namespace
-}  // namespace swc
-
-using namespace swc;
-
-extern "C" {
-
-size_t swc_bzip2_stream_batch_scratch_bytes(uint64_t n, uint64_t max_blocks, uint64_t out_capacity_total) {
-    const u64 nblk = max_blocks ? max_blocks : 1;
-    const u64 blocks = nblk * slot_bytes(), fb = fallback_bound(n, out_capacity_total);
-    return fixed_bytes_for(n, nblk) + (blocks > fb ? blocks : fb);
-}
-
-int32_t swc_bzip2_stream_decompress_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
-                                          uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
-                                          uint64_t *out_len, uint64_t *consumed_bits, int32_t *status,
-                                          uint64_t n, uint64_t max_blocks,
-                                          void *scratch, size_t scratch_bytes, void *cuda_stream) {
-    if (ensure_device()) return SWC_ERR_NO_DEVICE;
-    ApiLock api_lock;
-    if (n == 0) return SWC_OK;
-    const Call q{{{in_base, in_off, in_len, out_base, out_off, out_cap, out_len, status, n}, consumed_bits}, (cudaStream_t)cuda_stream};
-    if (missing(q.io) || max_blocks > 0xFFFFFFFFull || n > 0xFFFFFFFFull) return SWC_ERR_INVALID_ARG;
+// both entry points after their argument checks: size and seat the scratch, then decode
+int run_batch(const Call &q, u64 max_blocks, void *scratch, size_t scratch_bytes) {
+    const u64 n = q.io.n;
     int st;
     u64 nblk = max_blocks;
     u64 fb_need = 0;
@@ -502,7 +583,7 @@ int32_t swc_bzip2_stream_decompress_batch(const uint8_t *in_base, const uint64_t
         u64 fb = fb_need;
         if (max_blocks) {
             std::vector<u64> caps;
-            if ((st = read_lens(out_cap, n, q.s, caps))) return st;
+            if ((st = read_lens(q.io.out_cap, n, q.s, caps))) return st;
             for (u64 c : caps) fb += bzip2::scratch_per_unit(c);
         }
         size_t free_b = 0, total_b = 0;
@@ -515,6 +596,54 @@ int32_t swc_bzip2_stream_decompress_batch(const uint8_t *in_base, const uint64_t
     const u64 slots_fit = area / slot_bytes();
     const u64 slots = slots_fit < nblk ? slots_fit : nblk;
     return decode(q, Layout(sc.p, n, nblk), nblk, slots, area, sc.counted);
+}
+
+}  // namespace
+}  // namespace swc
+
+using namespace swc;
+
+extern "C" {
+
+size_t swc_bzip2_stream_batch_scratch_bytes(uint64_t n, uint64_t max_blocks, uint64_t out_capacity_total) {
+    const u64 nblk = max_blocks ? max_blocks : 1;
+    const u64 blocks = nblk * slot_bytes(), fb = fallback_bound(n, out_capacity_total);
+    return fixed_bytes_for(n, nblk) + (blocks > fb ? blocks : fb);
+}
+
+int32_t swc_bzip2_stream_decompress_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                                          uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                          uint64_t *out_len, uint64_t *consumed_bits, int32_t *status,
+                                          uint64_t n, uint64_t max_blocks,
+                                          void *scratch, size_t scratch_bytes, void *cuda_stream) {
+    if (ensure_device()) return SWC_ERR_NO_DEVICE;
+    ApiLock api_lock;
+    if (n == 0) return SWC_OK;
+    const Call q{{{in_base, in_off, in_len, out_base, out_off, out_cap, out_len, status, n}, consumed_bits}, (cudaStream_t)cuda_stream, {}};
+    if (missing(q.io) || max_blocks > 0xFFFFFFFFull || n > 0xFFFFFFFFull) return SWC_ERR_INVALID_ARG;
+    return run_batch(q, max_blocks, scratch, scratch_bytes);
+}
+
+int32_t swc_bzip2_multi_decompress_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len,
+                                         uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                         uint64_t *out_len, int32_t *status,
+                                         uint64_t *n_streams, const uint64_t *stream_off, const uint64_t *stream_cap,
+                                         uint64_t *stream_end, uint64_t *stream_in_off, uint32_t *parallel_streams,
+                                         uint64_t n, uint64_t max_blocks,
+                                         void *scratch, size_t scratch_bytes, void *cuda_stream) {
+    if (ensure_device()) return SWC_ERR_NO_DEVICE;
+    ApiLock api_lock;
+    if (n == 0) return SWC_OK;
+    Call q{{{in_base, in_off, in_len, out_base, out_off, out_cap, out_len, status, n}, nullptr}, (cudaStream_t)cuda_stream, {}};
+    const int tables = !!stream_off + !!stream_cap + !!stream_end + !!stream_in_off;
+    if (missing((const UnitIO &)q.io) || (tables != 0 && tables != 4) || max_blocks > 0xFFFFFFFFull || n > 0xFFFFFFFFull)
+        return SWC_ERR_INVALID_ARG;
+    q.mode.multi = true;
+    q.mode.table.n_streams = n_streams;
+    q.mode.table.stream_off = stream_off; q.mode.table.stream_cap = stream_cap;
+    q.mode.table.stream_end = stream_end; q.mode.table.stream_in_off = stream_in_off;
+    q.mode.parallel = parallel_streams;
+    return run_batch(q, max_blocks, scratch, scratch_bytes);
 }
 
 }  // extern "C"
